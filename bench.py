@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- secp256k1 verifies/sec of the go-ibft message-verification hot path on N B200s (one process per GPU).
+"""bench.py -- secp256k1 verifies/sec of the go-ibft message-verification hot path on N H100s (one process per GPU).
 
 A "step" is one pass of the hot path over one batch: the 10k-validator COMMIT round of SURVEY.md §8(d) config 3
 (10,000 committed seals + 10,000 COMMIT sender signatures, 1 % adversarial, weighted voting power) replicated to
-ITEMS_PER_GPU = 2^20 packed tuples per GPU (128 MiB of tuples: larger than the 126 MB L2, so no flush is needed between
+ITEMS_PER_GPU = 2^20 packed tuples per GPU (128 MiB of tuples: larger than the H100's 50 MB L2, so no flush is needed between
 iterations).  Every step runs: K1+K2 recover kernel over the rank's shard -> (N>1: one NCCL all-gather of the
 pass/fail bitmap words) -> K3 quorum kernels over the complete bitmap.
 
@@ -16,6 +16,9 @@ pass/fail bitmap words) -> K3 quorum kernels over the complete bitmap.
   strong_scaling  ONE 10,000-seal round and ONE config-5 backlog (100k messages, 16 heights x 10k validators) split over the N
           ranks, every rank holding only its shard: device-timed latency (H2D .. D2H) p50/p95 per N (go-ibft_b200/sharding.py ShardedVerifier)
   ingress   64 threads of single-message IsValidValidator calls through the reference-facing verifier (the coalescer)
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (the verdict bitmap and the per-group quorum
+results, see dump_outputs) as .npy files, so that two builds can be compared output for output on identical inputs.
 """
 from __future__ import annotations
 
@@ -48,7 +51,7 @@ def tile_items(items: np.ndarray, n: int) -> np.ndarray:
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, gpu_index: int):
         super().__init__(daemon=True)
@@ -243,7 +246,7 @@ def workload_config(n_gpus):
                         "voting power, 1% adversarial) replicated to 2^20 packed tuples per GPU",
             "items_per_gpu": ITEMS_PER_GPU, "global_items": ITEMS_PER_GPU * n_gpus, "validators": 10000,
             "parallelism": f"shard{n_gpus} + one all-gather of (bitmap words | partial voted sets)" if n_gpus > 1 else "single",
-            "l2": "inputs (128 MiB of tuples per GPU) exceed the 126 MB L2; no flush needed"}
+            "l2": "inputs (128 MiB of tuples per GPU) exceed the 50 MB L2 of an H100; no flush needed"}
 
 
 def _pct(xs, q):
@@ -564,6 +567,19 @@ def config4_legs(ib, local_rank, stream):
     return out
 
 
+def dump_outputs(out_dir, bitmap_words, n_items, results):
+    """The outputs of the timed path's last step, as a caller of ibft_verify_batch_device + ibft_quorum_reduce_device receives
+    them: verdicts.npy, one float32 0/1 per item (the bitmap unpacked, 4 MiB at 2^20 items), and quorum.npy, one float64 row per
+    group: the 320-bit voting-power sum as ten 32-bit halves (little-endian, exact in float64), n_valid, n_distinct,
+    has_quorum."""
+    os.makedirs(out_dir, exist_ok=True)
+    bits = np.unpackbits(np.ascontiguousarray(bitmap_words).view(np.uint8), bitorder="little")[:n_items]
+    np.save(os.path.join(out_dir, "verdicts.npy"), bits.astype(np.float32))
+    power = np.ascontiguousarray(results["power"]).view(np.uint32).reshape(len(results), 10)
+    rows = np.concatenate([power, np.stack([results["n_valid"], results["n_distinct"], results["has_quorum"]], axis=1)], axis=1)
+    np.save(os.path.join(out_dir, "quorum.npy"), rows.astype(np.float64))
+
+
 _REAL_STDOUT = None
 
 
@@ -595,6 +611,8 @@ def main():
     ap.add_argument("--no-key-cache-leg", action="store_true", help="skip the extra leg that times the key-registry path")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--skip-extras", action="store_true", help="headline + e2e + strong-scaling legs only (development: short multi-GPU runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the verdicts and quorum results of the last timed step to DIR/*.npy (see dump_outputs)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
@@ -717,6 +735,9 @@ def main():
         sampler.stop()
     ms_per_step = ms_total / args.steps
     value = n_global / (ms_per_step * 1e-3)
+    if args.dump_outputs and rank == 0:
+        res = np.frombuffer(t_results.cpu().numpy().tobytes(), dtype=ib.RESULT_DTYPE)
+        dump_outputs(args.dump_outputs, full_bitmap().cpu().numpy(), n_global, res)
 
     # ---- e2e: host buffers through ibft_verify_batch (H2D + kernels + D2H inside the timed region)
     # the step's inputs live in PINNED host memory (torch pin_memory); the C ABI detects that and DMA-copies straight from it
@@ -901,27 +922,8 @@ def main():
     info = eng.device_info()
     kernel_rate = n_local / (ms_kernel * 1e-3)  # per GPU
     achieved = kernel_rate * ALGO_IMAD_PER_VERIFY
-    peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    hbm_peak_gbs, hbm_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
-    if os.path.exists(peaks_path):
-        try:
-            pk = json.load(open(peaks_path))
-            hbm_peak_gbs, hbm_src = float(pk.get("hbm_gbs", hbm_peak_gbs)), "MEASURED_PEAKS.json"
-        except Exception:
-            pass
+    hbm_peak_gbs, hbm_src = 3350.0, "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
     hbm_gbs = kernel_rate * ALGO_BYTES_PER_VERIFY / 1e9
-    # DRAM traffic of the dominant kernel from the committed ncu --set full capture of this same configuration (per launch)
-    traffic, traffic_src, executed = None, None, None
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tpath):
-        try:
-            tj = json.load(open(tpath))
-            if int(tj.get("items_per_launch", 0)) == n_local:
-                traffic = float(tj["dram_bytes_read"]) + float(tj["dram_bytes_write"])
-                traffic_src = tj.get("capture")
-                executed = tj.get("executed")
-        except Exception:
-            pass
     line = {
         "metric": "secp256k1_verifies_per_sec", "value": value, "unit": "verifies/s", "n_gpus": n_gpus, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -934,16 +936,10 @@ def main():
         "strong_scaling": strong,
         "gpu_launches": int(launches),
         "roofline": {"bound": "int32-imad-issue", "achieved": achieved / 1e12, "peak": imad_peak / 1e12, "unit": "T IMAD-class instr/s",
-                     "frac": achieved / imad_peak, "traffic": traffic, "traffic_unit": "DRAM bytes per k_recover launch (ncu)",
-                     "traffic_source": traffic_src, "algorithmic_bytes_per_launch": ALGO_BYTES_PER_VERIFY * n_local,
-                     "executed_per_ncu": executed,
-                     "issue_active_pct": (executed or {}).get("issue_active_pct"),
-                     "fmaheavy_pipe_pct": (executed or {}).get("fmaheavy_pipe_cycles_active_pct"),
-                     "binding_pipe_note": "from the committed ncu --set full capture of this kernel: the FMA-heavy pipe (IMAD / IMAD.WIDE; an IMAD.WIDE holds it 4 "
-                                          "cycles per warp instruction) is the pipe that binds -- issue-active is low BECAUSE that pipe is busy",
+                     "frac": achieved / imad_peak, "algorithmic_bytes_per_launch": ALGO_BYTES_PER_VERIFY * n_local,
                      "note": "frac uses SURVEY 8d's canonical-algorithm count (5.0e5 IMAD-class instr/verify); the kernel executes fewer "
                              "multiply instructions than that (GLV, combined generator table, safegcd, fused IMAD.WIDE), so frac can "
-                             "exceed 1; executed_per_ncu gives the real instruction counts",
+                             "exceed 1",
                      "kernel": "k_recover", "kernel_ms": ms_kernel, "kernel_verifies_per_s_per_gpu": kernel_rate,
                      "algorithmic_instr_per_verify": ALGO_IMAD_PER_VERIFY,
                      "peak_source": "dependent-free mad.lo.u32 probe on this GPU (ibft_probe_int_peak), measured live",
@@ -956,8 +952,8 @@ def main():
                               "reps": len(lat), "p50": lat[len(lat) // 2], "p95": lat[int(len(lat) * 0.95)],
                               "pinned_input_p50": lat_pin[len(lat_pin) // 2], "pinned_input_p95": lat_pin[int(len(lat_pin) * 0.95)],
                               "device_only_p50": lat_dev[len(lat_dev) // 2], "device_only_p95": lat_dev[int(len(lat_dev) * 0.95)],
-                              "kernel": "k_recover_split (chain warps + helper warp; AUTO path for 7,105..14,208 signatures)",
-                              "round_1000_seals": {"kernel": "k_recover_qsplit (four-lane chain warps + helper warp; AUTO path up to 7,104 signatures)", "p50": lat_small[len(lat_small) // 2],
+                              "kernel": "k_recover_split (chain warps + helper warp; AUTO path for SMs x 48 + 1 .. SMs x 96 signatures: 6,337..12,672 on an H100)",
+                              "round_1000_seals": {"kernel": "k_recover_qsplit (four-lane chain warps + helper warp; AUTO path up to SMs x 48 signatures: 6,336 on an H100)", "p50": lat_small[len(lat_small) // 2],
                                                    "p95": lat_small[int(len(lat_small) * 0.95)],
                                                    "device_only_p50": lat_small_dev[len(lat_small_dev) // 2]}},
     }

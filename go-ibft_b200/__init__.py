@@ -1,6 +1,6 @@
-"""go-ibft_b200 -- B200-native batched message-verification engine behind go-ibft's core.Verifier / core.Messages.
+"""go-ibft_b200 -- H100 (sm_90a) batched message-verification engine behind go-ibft's core.Verifier / core.Messages.
 
-Only the hot path of SURVEY.md §8 lives here: csrc/ (hand-written sm_100a CUDA kernels + the C ABI of
+Only the hot path of SURVEY.md §8 lives here: csrc/ (hand-written sm_90a CUDA kernels + the C ABI of
 include/ibft_verify.h) and the host-side mirror of the reference interfaces for that path.
 """
 from .engine import (Engine, EngineError, GROUP_DTYPE, ITEM_DTYPE, KIND_DIGEST, KIND_INVALID, KIND_PAYLOAD, KIND_SEAL,  # noqa: F401

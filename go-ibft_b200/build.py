@@ -1,6 +1,6 @@
-"""In-tree build of the CUDA engine (libibftverify.so) for sm_100a with nvcc.
+"""In-tree build of the CUDA engine (libibftverify.so) for sm_90a (H100) with nvcc.
 
-The shared object is git-ignored but travels to the GPU box with the repo snapshot.  nvcc cross-compiles without a GPU.
+The shared object is a build product (git-ignored); nvcc cross-compiles it without a GPU.
 """
 from __future__ import annotations
 
@@ -10,7 +10,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libibftverify.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "-shared", "-diag-suppress", "550"]
 
 

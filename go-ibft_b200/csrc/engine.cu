@@ -1,4 +1,4 @@
-// engine.cu -- CUDA kernels (sm_100a) and the C ABI (include/ibft_verify.h) of the batched verification engine.
+// engine.cu -- CUDA kernels (sm_90a, H100) and the C ABI (include/ibft_verify.h) of the batched verification engine.
 //
 // Kernels (SURVEY.md §2.2 checklist):
 //   k_recover        K1+K2 fused: Keccak-256 of the payload / seal wrap, secp256k1 public-key recovery, address
@@ -156,7 +156,7 @@ __device__ __forceinline__ void learn_key(const slot_dev* __restrict__ slots, ui
 #define IBFT_MIN_BLOCKS 3
 #endif
 // BLOCK = 128 for throughput (12 resident warps/SM at 166 registers); BLOCK = 32 for latency-critical small batches (a
-// 10k-validator COMMIT round is only 313 warps: one-warp CTAs spread them over all 148 SMs instead of 79).
+// 10k-validator COMMIT round is only 313 warps: one-warp CTAs spread them over all 132 SMs of an H100 instead of 79).
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK, (IBFT_MIN_BLOCKS * IBFT_BLOCK) / BLOCK)
 k_recover(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __restrict__ arena, size_t arena_len,
@@ -419,7 +419,7 @@ k_recover_quad(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
 // three: the helper takes the digest, r^-1, the GLV splits, the square root and u1*G (a comb without doublings) off the
 // chain, which only computes u2*R -- on an isomorphic curve, so that it does not have to wait for the root (verify_core.cuh,
 // "Split pipeline").  Hand-off through shared memory and named barriers (bar.arrive by the helper, bar.sync by the chain).
-// Capacity of one wave: SMs x 96 signatures (14,208 on a B200).
+// Capacity of one wave: SMs x 96 signatures (12,672 on an H100).
 // ------------------------------------------------------------------------------------------------------------
 #define IBFT_SPLIT_CHAINS 3
 #define IBFT_SPLIT_SIGS (32 * IBFT_SPLIT_CHAINS)
@@ -1114,7 +1114,7 @@ __global__ void k_quorum_merge(const uint32_t* __restrict__ parts, uint32_t n_pa
 // buffer its peers have mapped over NVLink (CUDA IPC); this kernel publishes "my round `epoch` is complete", waits for the
 // peers' flags, then reads their words straight out of peer memory -- OR-ing the voted sets, summing the counts, and assembling
 // the complete bitmap -- so that the all-gather and the merge are ONE launch (the NCCL path costs a collective launch + the
-// merge kernel: ~25-30 us of a 0.5 ms round).  Buffer of rank r: [2 parities][words_per_rank] words, then flags[2].  Rounds
+// merge kernel).  Buffer of rank r: [2 parities][words_per_rank] words, then flags[2].  Rounds
 // alternate parities: a rank can only start writing parity p for round e+2 after it has seen every peer's flag for round e+1,
 // i.e. after every peer has finished reading round e.  The wait is bounded (spin_limit polls): on timeout the kernel reports
 // through *timeout_flag and merges nothing -- it never hangs the device.
@@ -1662,7 +1662,7 @@ struct ibft_engine {
   std::mutex keys_mu;                  // key registry upkeep (built_count, h_learn_counts)
   uint32_t* d_learn_counts = nullptr;  // key registry: one "keys learned" counter per table slot (read back in one copy)
   uint32_t* h_learn_counts = nullptr;  // pinned
-  int sm_count = 148;
+  int sm_count = 132;  // replaced by the device's count at engine creation
   uint32_t* d_ctable = nullptr;  // combined generator table (IBFT_WC > 0)
   cudaFuncAttributes recover_attr{};
   // hashing (ibft_keccak256_batch / ibft_proposal_hash_batch): own lock, own stream, own grow-only scratch -- a hash call
@@ -1788,7 +1788,7 @@ static int engine_alloc(ibft_engine* e) {
 #if IBFT_WC > 0
   {
     // position 0 is the combined table of the interleaved window loop; positions 1.. are the comb tables of the split
-    // latency kernel's helper warps (36 MB in all, L2-resident while a round is being verified)
+    // latency kernel's helper warps (36 MB in all: they fit in the H100's 50 MB L2 while a round is being verified)
     size_t entries = (size_t)IBFT_CTAB_ENTRIES;
     CU(cudaMalloc(&e->d_ctable, (size_t)IBFT_CTAB_POSITIONS * entries * IBFT_GTAB_ENTRY_WORDS * 4));
     k_build_ctable<<<dim3((unsigned)((entries + 63) / 64), IBFT_CTAB_POSITIONS), 64, 0, L->stream>>>(e->d_ctable);
@@ -2098,12 +2098,11 @@ static int launch_recover(ibft_engine* e, lane* L, const ibft_sig_item* d_items,
                           vote_sink sink = vote_sink{nullptr, nullptr, nullptr}, uint32_t worklist_index = 0) {
   if (hi <= lo) return IBFT_OK;
   uint32_t* const worklist = L->d_worklist ? L->d_worklist + (size_t)worklist_index * ((size_t)L->cap_items + 1) : nullptr;
-  // path selection (ibft_set_recover_path).  AUTO picks by how many warps each of the SM's four schedulers would hold
-  // (B200, kernel time of one batch: profiles/latency_r01_v9.md):
-  //   <= SMs x 24 signatures   four-lane chain warps + helper warp, one CTA (3 + 1 warps) per SM                   0.41 ms
-  //   <= SMs x 48              the same, two CTAs per SM (two warps per scheduler)                                  0.51 ms
-  //   <= SMs x 96              chain warps + helper warp, one CTA (3 + 1 warps) per SM (a 10k-validator round)      0.68 ms
-  //   <= SMs x 192             the same, two CTAs per SM (one-thread kernel: 1.16 ms)                               0.90 ms
+  // path selection (ibft_set_recover_path).  AUTO picks by how many warps each of the SM's four schedulers would hold:
+  //   <= SMs x 24 signatures   four-lane chain warps + helper warp, one CTA (3 + 1 warps) per SM
+  //   <= SMs x 48              the same, two CTAs per SM (two warps per scheduler)
+  //   <= SMs x 96              chain warps + helper warp, one CTA (3 + 1 warps) per SM (a 10k-validator round)
+  //   <= SMs x 192             the same, two CTAs per SM
   //   beyond                   one thread per signature: one-warp CTAs while one wave covers them, then the 128-thread
   //                            throughput kernel
   const uint32_t cnt = hi - lo;
@@ -2123,7 +2122,7 @@ static int launch_recover(ibft_engine* e, lane* L, const ibft_sig_item* d_items,
     else
     // long payloads (ROUND_CHANGE messages with their certificates: up to 909 KB of signed bytes each): the helper warp of the
     // latency kernels hashes for three (or 24) signatures one after the other, which serialises the sponges that dominate such a
-    // batch -- one thread per signature hashes them all in parallel (config 4, 10,000 x 909 KB: 156 ms -> see DESIGN.md §6)
+    // batch -- one thread per signature hashes them all in parallel (config 4: 10,000 x 909 KB)
     if (arena_len / cnt > 256) path = IBFT_PATH_THREAD;
     else if (cnt <= (uint32_t)e->sm_count * 2u * IBFT_QSPLIT_SIGS) path = IBFT_PATH_QSPLIT;
     else if (cnt <= (uint32_t)e->sm_count * 2u * IBFT_SPLIT_SIGS) path = IBFT_PATH_SPLIT;

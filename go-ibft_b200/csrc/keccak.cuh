@@ -99,8 +99,7 @@ IBFT_HD uint64_t load_le64_partial(const uint8_t* p, int n) {  // n in [0,8]
 }
 
 // 8 message bytes from an ARBITRARILY aligned address as one little-endian lane.  Device: three aligned 32-bit loads + two
-// funnel shifts instead of eight byte loads (a byte-wise absorb made the loads, not the permutation, the cost of a long sponge:
-// 10.5 us per 136-byte block on one thread).  The aligned word that holds the last wanted byte is always inside the allocation.
+// funnel shifts instead of eight byte loads (a byte-wise absorb made the loads, not the permutation, the cost of a long sponge).  The aligned word that holds the last wanted byte is always inside the allocation.
 IBFT_HD uint64_t load_le64_any(const uint8_t* p) {
 #if defined(__CUDA_ARCH__)
   const uint32_t sh = ((uint32_t)(uintptr_t)p & 3u) * 8u;

@@ -277,8 +277,8 @@ struct exec_quad {
     uint4* buf = xb + par * 2u * nt;
     par ^= 1u;
     // slot of (quad Q of the warp, product k) = 8k + ((Q + 2k) & 7): the eight quads reading product k hit eight different
-    // 16-byte bank groups, and so do the eight lanes of every quarter-warp when they write (ncu r01_v10: the plain layout
-    // "slot = lane" cost 1.06 M shared-memory bank conflicts per 1,000-signature launch on the reads)
+    // 16-byte bank groups, and so do the eight lanes of every quarter-warp when they write (the plain layout "slot = lane"
+    // makes the eight quads reading one product collide in the same bank group)
     const uint32_t wb = t & ~31u, Q = (t >> 2) & 7u;
     if (role < count) {
       const uint32_t sl = wb + 8u * (uint32_t)role + ((Q + 2u * (uint32_t)role) & 7u);
@@ -414,7 +414,7 @@ static_assert(IBFT_WG % IBFT_WR == 0, "generator window must be a multiple of th
 // other half of the (d1, d2) plane is reached by negating y.  (2^(WC-1)+1) * (2^WC+1) * 64 bytes: 2.1 MB for WC = 8
 // (L2 resident), 537 MB for WC = 12 (HBM; 704 B of gathers per signature) -- built on the device at engine creation.
 #ifndef IBFT_WC
-#define IBFT_WC 8  // measured on B200: off 34.9 M, 8 -> 37.8 M (+8 %), 12 -> 38.8 M verifies/s
+#define IBFT_WC 8  // 2.1 MB, L2 resident; WC = 12 trades HBM gathers for fewer additions
 #endif
 #define IBFT_CTAB_D2 ((1 << IBFT_WC) + 1)
 #define IBFT_CTAB_ENTRIES (((1 << (IBFT_WC - 1)) + 1) * IBFT_CTAB_D2)
@@ -477,8 +477,7 @@ struct gtab_view {
 // Per-signature table {1..8}*R (affine x, y; 16 words per entry).  On the device it lives in SHARED memory, interleaved
 // across the CTA's threads -- word (entry*16 + limb) of thread t sits at base[(entry*16 + limb) * stride + t] -- so that
 // every lane always hits its own bank whatever entry it selects (conflict-free), and none of it ever reaches HBM.  (Kept
-// in thread-local memory, the tables were written back through L2: 0.86 GB of DRAM writes per 2^20-signature launch in ncu
-// r01_v4, 5x the algorithmic traffic.)  The host emulation passes a plain array with stride 1.
+// in thread-local memory, the tables were written back through L2 to DRAM: several times the algorithmic traffic.)  The host emulation passes a plain array with stride 1.
 struct rtab_view {
   uint32_t* base;
   uint32_t stride;

@@ -2,9 +2,9 @@
 //
 // Part of the hot path behind core.Verifier.IsValidValidator / IsValidCommittedSeal
 // (reference core/backend.go:41-45, :53-55): the reference ships no arithmetic, so there is no
-// reference code to mirror here -- the design is B200-first:
-//   * saturated 32-bit limbs, because the sm_100a integer multiplier is the 32x32+64 IMAD.WIDE(.X)
-//     (measured 32 thread-ops/clk/SM, tools/imad_peak.cu): a 256x256 product is 64 of them;
+// reference code to mirror here -- the design follows the GPU's integer pipe:
+//   * saturated 32-bit limbs, because the sm_90a integer multiplier is the 32x32+64 IMAD.WIDE(.X)
+//     (tools/imad_peak.cu measures its rate): a 256x256 product is 64 of them;
 //   * products accumulate in two interleaved carry chains ("even"/"odd" columns) so that every
 //     mad.lo.cc/madc.hi.cc pair fuses into ONE IMAD.WIDE.U32.X and two independent chains are always in
 //     flight (the pipe needs ILP 2 per warp);
@@ -22,8 +22,8 @@
 #define IBFT_HD inline
 #endif
 
-// Code-size control.  The recover kernel is I-cache bound when everything is inlined (ncu r01_v1: 45% of the
-// stall samples are no_instruction on 735 KB of SASS), so the multiplier / squarer -- and optionally the adders --
+// Code-size control.  The recover kernel is I-cache bound when everything is inlined (hundreds of KB of SASS,
+// most stalls waiting for instructions), so the multiplier / squarer -- and optionally the adders --
 // are real device functions, passed BY VALUE so that the ABI keeps every operand in registers (no stack traffic).
 #if defined(__CUDACC__) && !defined(IBFT_INLINE_FE)
 #define IBFT_FN __host__ __device__ __noinline__
@@ -354,9 +354,9 @@ __device__ __forceinline__ uint32_t absdiff4(uint32_t* d, const uint32_t* x, con
 // R[0..15] = a * b
 IBFT_HD void mul_wide_8x8(uint32_t* R, const uint32_t* a, const uint32_t* b) {
 #if IBFT_PTX && defined(IBFT_KARATSUBA)
-  // OPT-IN (measured slower, see DESIGN.md): one level of (subtractive) Karatsuba, 48 wide MACs instead of 64.  The IMAD.WIDE pipe is the bottleneck of the whole
+  // OPT-IN (slower in practice, see DESIGN.md): one level of (subtractive) Karatsuba, 48 wide MACs instead of 64.  The IMAD.WIDE pipe is the bottleneck of the whole
   // kernel (4 issue cycles per warp-instruction) while the ALU pipe that takes the ~70 extra add/xor instructions is
-  // less than half used (ncu r01_v2), so trading 16 MACs for carry-chain adds is a net win on sm_100a.
+  // less than half used, so trading 16 MACs for carry-chain adds looks like a win on paper.
   //   a*b = z0 + (z0 + z2 + (a0-a1)(b1-b0)) 2^128 + z2 2^256
   uint32_t z0[8], z2[8], m[8], da[4], db[4];
   mul4x4(z0, a[0], a[1], a[2], a[3], b[0], b[1], b[2], b[3]);

@@ -2,7 +2,7 @@
 // signature verification only handles public data).
 //
 // Replaces the two Fermat ladders of the first kernel version (a^(p-2): 255 squarings; a^(n-2): ~320 generic mod-n
-// multiplications, 20 % of all instructions in ncu profile r01_v1).  The algorithm works on 9 signed 30-bit limbs so that
+// multiplications, a large share of all instructions).  The algorithm works on 9 signed 30-bit limbs so that
 // a 2x2 transition matrix of 30 divsteps can be applied with 32x32->64 multiply-adds without overflow:
 //   repeat:  t = matrix of 30 divsteps on the low 30 bits of (f, g)            [ALU-pipe work: ctz, shifts, adds]
 //            (d, e) <- t * (d, e) / 2^30  (mod m)                               [72 wide MACs]

@@ -353,7 +353,7 @@ class GpuVerifier : public Verifier {
   }
 
   // INGRESS COALESCER.  The reference calls IsValidValidator once per inbound gossip message from any number of goroutines
-  // (core/ibft.go:1101-1128).  One device call per message would cost a whole kernel launch (~0.4 ms) for one signature and
+  // (core/ibft.go:1101-1128).  One device call per message would cost a whole kernel launch and one serial chain for one signature and
   // serialise the callers.  Instead a miss is queued; a caller that finds fewer than two flushes in flight becomes a leader: it takes
   // everything queued (its own request included), makes a single device call for the batch, publishes the verdicts and wakes the
   // others (two leaders at most: the engine runs two host-buffer calls side by side, so the next batch goes up while the previous

@@ -1,4 +1,4 @@
-// Package gpubackend binds the B200 verification engine (include/ibft_verify.h, libibftverify.so) through cgo and
+// Package gpubackend binds the H100 verification engine (include/ibft_verify.h, libibftverify.so) through cgo and
 // implements the hot-path half of go-ibft's core.Backend: core.Verifier (core/backend.go:37-56).
 //
 // COMPILE-UNVERIFIED: the authoring image has no Go toolchain.  The C ABI below is exercised by the ctypes harness

@@ -1,5 +1,5 @@
 /*
- * ibft_verify.h -- C ABI of the B200-native batched message-verification engine for go-ibft.
+ * ibft_verify.h -- C ABI of the H100 (sm_90a) batched message-verification engine for go-ibft.
  *
  * This is the drop-in boundary.  go-ibft has NO FFI of its own: the hot path sits behind the Go
  * interfaces core.Verifier (core/backend.go:37-56) and core.Messages (core/ibft.go:23-46), whose
@@ -276,7 +276,7 @@ int ibft_sign_batch(ibft_engine* e, const uint8_t* privkeys, const uint8_t* dige
 
 /* measurement / test hooks ------------------------------------------------------------------------- */
 /* Kernel selection of the recover step (the verdicts are identical on every path; only latency / throughput differ):
- *   AUTO    by batch size: up to SMs x 48 signatures (7,104 on a B200) QSPLIT, up to SMs x 192 (28,416) SPLIT, beyond
+ *   AUTO    by batch size: up to SMs x 48 signatures (6,336 on an H100) QSPLIT, up to SMs x 192 (25,344) SPLIT, beyond
  *           that THREAD (the throughput kernel);
  *   THREAD  always one thread per signature;  QUAD  always four lanes per signature;
  *   SPLIT   chain warps (one lane per signature) + a helper warp per CTA that takes the digest, r^-1, sqrt and u1*G off the

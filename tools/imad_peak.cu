@@ -1,7 +1,7 @@
-// Integer-pipe micro-benchmark for sm_100a: measures the issue-rate ceilings that bound the
+// Integer-pipe micro-benchmark for sm_90a (H100): measures the issue-rate ceilings that bound the
 // secp256k1 kernels (IMAD, IMAD.WIDE, IMAD.WIDE.X carry chains, IADD3, LOP3, SHF and mixes).
 // Test/measurement tool only (not part of the product path). Build:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o imad_peak imad_peak.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o imad_peak imad_peak.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
 // Development tool: dependent-chain latency (cycles per operation, one warp per SM sub-partition) of the field and group
-// operations, serial and four-lane.   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -diag-suppress 550 -I include tools/op_latency.cu -o tools/op_latency
+// operations, serial and four-lane.   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -diag-suppress 550 -I include tools/op_latency.cu -o tools/op_latency
 #include "../go-ibft_b200/csrc/engine.cu"
 #include <cstdio>
 

@@ -1,6 +1,6 @@
 // Development tool: per-stage clock64() stamps of ONE signature's serial chain (thread 0 of CTA 0), for the one-thread and the
 // four-lane recover kernels.  Builds the whole engine translation unit with IBFT_STAGE_CLOCKS.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -diag-suppress 550 -I include tools/stage_clocks.cu -o tools/stage_clocks
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -diag-suppress 550 -I include tools/stage_clocks.cu -o tools/stage_clocks
 //   tools/stage_clocks items.bin [n_items]      (items.bin: packed 128-byte tuples, e.g. dumped from tests/golden/config3.npz)
 #define IBFT_STAGE_CLOCKS 1
 #include "../go-ibft_b200/csrc/engine.cu"
