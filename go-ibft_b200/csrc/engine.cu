@@ -1646,6 +1646,10 @@ struct lane {
   pending_call pending;
   uint32_t* d_worklist = nullptr;  // key-registry path: [0] = count, [1..] = indices left to the recover pass
   cudaEvent_t wl_ev[4] = {nullptr, nullptr, nullptr, nullptr};  // last use of each worklist (orders launches that arrive on different streams)
+  // worklists the known-key passes of the current host-buffer call filled (bit k = worklist k), and whether one of them was
+  // filled twice (its head then holds only the later pass); copied to last_wl_* when the call completes
+  uint32_t wl_used = 0, last_wl_used = 0;
+  bool wl_reused = false, last_wl_reused = false;
   const uint8_t* dev_arena = nullptr;
   size_t dev_arena_len = 0;
 };
@@ -1800,15 +1804,16 @@ static int engine_alloc(ibft_engine* e) {
   return IBFT_OK;
 }
 
-// test hook: copy `count` entries of the combined generator table starting at entry `first` (64 bytes each, x then y as 8
-// little-endian words); returns IBFT_ERR_INVALID_ARG when the library was built without a combined table
+// test hook: copy `count` entries of the generator comb tables starting at entry `first` (64 bytes each, x then y as 8
+// little-endian words); entry p * entries + i is entry i of comb position p (position 0 = the combined table).  Returns
+// IBFT_ERR_INVALID_ARG when the library was built without a combined table
 extern "C" int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count, uint8_t* out, int* wc, uint32_t* entries) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
   if (wc) *wc = IBFT_WC;
 #if IBFT_WC > 0
   if (entries) *entries = (uint32_t)IBFT_CTAB_ENTRIES;
   if (count == 0) return IBFT_OK;
-  if (!out || (size_t)first + count > (size_t)IBFT_CTAB_ENTRIES) { set_err("range"); return IBFT_ERR_INVALID_ARG; }
+  if (!out || (size_t)first + count > (size_t)IBFT_CTAB_POSITIONS * IBFT_CTAB_ENTRIES) { set_err("range"); return IBFT_ERR_INVALID_ARG; }
   CU(cudaSetDevice(e->p.device));
   CU(cudaMemcpy(out, e->d_ctable + (size_t)first * IBFT_GTAB_ENTRY_WORDS, (size_t)count * 64, cudaMemcpyDeviceToHost));
   return IBFT_OK;
@@ -1817,6 +1822,56 @@ extern "C" int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count,
   (void)first; (void)out;
   return count == 0 ? IBFT_OK : IBFT_ERR_INVALID_ARG;
 #endif
+}
+
+// test hook: the key registry entry of validator `validator` (validator-index order) of a table slot -- its state
+// (IBFT_KEY_*), the learned affine key (x, y as 8 little-endian words each) and `count` comb entries starting at `first`
+// (entry j * 128 + m - 1 = m * 2^(8j) * Q, same format as ibft_debug_ctable).  Waits for the device.
+extern "C" int ibft_debug_keytab(ibft_engine* e, uint32_t table_slot, uint32_t validator, uint32_t first, uint32_t count, uint8_t* out,
+                                 uint32_t* state_out, uint8_t* key_out) {
+  if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+#if IBFT_WC > 0
+  all_lanes_lock lk(e);
+  if (table_slot >= e->p.max_table_slots || !e->slots[table_slot].valid) { set_err("slot %u not set", table_slot); return IBFT_ERR_NO_TABLE; }
+  const slot_host& s = e->slots[table_slot];
+  if (!s.d_key_state) { set_err("engine has no key registry"); return IBFT_ERR_INVALID_ARG; }
+  if (validator >= s.n || (count && !out) || (size_t)first + count > (size_t)IBFT_KEYTAB_POSITIONS * IBFT_KEYTAB_ENTRIES) {
+    set_err("range");
+    return IBFT_ERR_INVALID_ARG;
+  }
+  CU(cudaSetDevice(e->p.device));
+  CU(cudaDeviceSynchronize());
+  if (state_out) CU(cudaMemcpy(state_out, s.d_key_state + validator, 4, cudaMemcpyDeviceToHost));
+  if (key_out) CU(cudaMemcpy(key_out, s.d_key_xy + 16 * (size_t)validator, 64, cudaMemcpyDeviceToHost));
+  if (count)
+    CU(cudaMemcpy(out, s.d_key_tab + (size_t)validator * IBFT_KEYTAB_WORDS + (size_t)first * IBFT_GTAB_ENTRY_WORDS, (size_t)count * 64,
+                  cudaMemcpyDeviceToHost));
+  return IBFT_OK;
+#else
+  (void)table_slot; (void)validator; (void)first; (void)count; (void)out; (void)state_out; (void)key_out;
+  set_err("library built without a key registry");
+  return IBFT_ERR_INVALID_ARG;
+#endif
+}
+
+// test hook: number of items the known-key pass of the most recent completed host-buffer call handed to the recover pass
+// (the sum of the heads of the worklists that call filled; 0 when it took no known-key pass)
+extern "C" int ibft_debug_known_handed_back(ibft_engine* e, uint32_t* n_out) {
+  if (!e || !n_out) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  lane* L = &e->lanes[e->last_lane.load()];
+  std::lock_guard<std::mutex> lk(L->mu);
+  if (L->pending.active) { set_err("a submitted call is still pending"); return IBFT_ERR_INVALID_ARG; }
+  if (L->last_wl_reused) { set_err("the last call filled one worklist twice: its count is not kept"); return IBFT_ERR_INVALID_ARG; }
+  uint32_t total = 0;
+  CU(cudaSetDevice(e->p.device));
+  for (uint32_t k = 0; k < 4; k++) {
+    if (!((L->last_wl_used >> k) & 1u)) continue;
+    uint32_t head = 0;
+    CU(cudaMemcpy(&head, L->d_worklist + (size_t)k * ((size_t)L->cap_items + 1), 4, cudaMemcpyDeviceToHost));
+    total += head;
+  }
+  *n_out = total;
+  return IBFT_OK;
 }
 
 extern "C" int ibft_engine_create(const ibft_engine_params* params, ibft_engine** out) {
@@ -2098,6 +2153,11 @@ static int launch_recover(ibft_engine* e, lane* L, const ibft_sig_item* d_items,
                           vote_sink sink = vote_sink{nullptr, nullptr, nullptr}, uint32_t worklist_index = 0) {
   if (hi <= lo) return IBFT_OK;
   uint32_t* const worklist = L->d_worklist ? L->d_worklist + (size_t)worklist_index * ((size_t)L->cap_items + 1) : nullptr;
+  auto note_worklist = [&]() {  // host-side record for ibft_debug_known_handed_back
+    const uint32_t bit = 1u << (worklist_index & 3u);
+    if (L->wl_used & bit) L->wl_reused = true;
+    L->wl_used |= bit;
+  };
   // path selection (ibft_set_recover_path).  AUTO picks by how many warps each of the SM's four schedulers would hold:
   //   <= SMs x 24 signatures   four-lane chain warps + helper warp, one CTA (3 + 1 warps) per SM
   //   <= SMs x 48              the same, two CTAs per SM (two warps per scheduler)
@@ -2141,6 +2201,7 @@ static int launch_recover(ibft_engine* e, lane* L, const ibft_sig_item* d_items,
     // known-key latency path: verify against the learned keys, then recover whatever was not accepted (worklist; the second
     // launch finds it empty -- and returns at once -- when every signature of the round verified)
     uint32_t blocks = (cnt + IBFT_SPLIT_SIGS - 1) / IBFT_SPLIT_SIGS;
+    note_worklist();
     CU(cudaStreamWaitEvent(st, L->wl_ev[worklist_index & 3u], 0));
     CU(cudaMemsetAsync(worklist, 0, 4, st));
     k_verify_split<<<blocks, 32 * (IBFT_SPLIT_CHAINS + 1), IBFT_VSPLIT_SMEM, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups,
@@ -2169,6 +2230,7 @@ static int launch_recover(ibft_engine* e, lane* L, const ibft_sig_item* d_items,
     // key-registry path (one thread per signature, any batch size): verify what can be verified, then recover the rest from
     // the worklist (dense second launch; the threads beyond the worklist's length leave at once)
     // device-resident callers may use different streams: launches sharing a worklist are ordered on the device
+    note_worklist();
     CU(cudaStreamWaitEvent(st, L->wl_ev[worklist_index & 3u], 0));
     CU(cudaMemsetAsync(worklist, 0, 4, st));
     if (small_batch) {
@@ -2257,6 +2319,8 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
     return IBFT_ERR_CAPACITY;
   }
   CU(cudaSetDevice(e->p.device));
+  L->wl_used = 0;
+  L->wl_reused = false;
   size_t voted_words = 0;
   if (n_groups) {
     int rc = plan_groups(e, L, groups, n_groups, L->h_gdev, &voted_words);
@@ -2406,6 +2470,8 @@ static int wait_locked(ibft_engine* e, lane* L) {
     return IBFT_ERR_CUDA;
   }
   L->last_status_n = pc.n;
+  L->last_wl_used = L->wl_used;
+  L->last_wl_reused = L->wl_reused;
   if (pc.n) {
     size_t words = (pc.n + 31) / 32;
     memcpy(pc.bitmap_out, L->h_bitmap, words * 4);

@@ -189,6 +189,7 @@ IBFT_PT jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, fe* h_out =
   jac r;
   if (h_out) *h_out = fe_from_u32(1);
   if (p.inf) {
+    IBFT_BRANCH(IBFT_BR_ADD_INF);
     r.x = qx;
     r.y = qy;
     r.z = fe_from_u32(1);
@@ -201,7 +202,11 @@ IBFT_PT jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, fe* h_out =
   fe h = fe_sub(u2, p.x);
   fe rr = fe_sub(s2, p.y);
   if (fe_is_zero(h)) {
-    if (fe_is_zero(rr)) return jac_double(p);  // P + P (rare; kept inline so that `p` never has its address taken)
+    if (fe_is_zero(rr)) {
+      IBFT_BRANCH(IBFT_BR_ADD_DBL);
+      return jac_double(p);  // P + P (rare; kept inline so that `p` never has its address taken)
+    }
+    IBFT_BRANCH(IBFT_BR_ADD_NEG);
     r = p;
     r.inf = true;  // P + (-P)
     return r;
@@ -338,7 +343,10 @@ IBFT_HD xyzz xyzz_double_x(const EX& ex, const xyzz& p) {
 //         -> {R*(Q-X3), S1*PPP, ZZZ12*PPP}.   q is never the point at infinity (zero digits are skipped by the caller).
 template <class EX>
 IBFT_HD xyzz xyzz_add_x(const EX& ex, const xyzz& p, const xyzz& q) {
-  if (p.inf) return q;
+  if (p.inf) {
+    IBFT_BRANCH(IBFT_BR_XADD_INF);
+    return q;
+  }
   xyzz r;
   fe a[4], b[4], o[4];
   a[0] = p.x; b[0] = q.zz; a[1] = q.x; b[1] = p.zz; a[2] = p.y; b[2] = q.zzz; a[3] = q.y; b[3] = p.zzz;
@@ -361,8 +369,12 @@ IBFT_HD xyzz xyzz_add_x(const EX& ex, const xyzz& p, const xyzz& q) {
   // exceptional cases, tested last so that the zero tests overlap the generic computation: every lane of a quad holds the
   // same state, so the whole quad takes these (rare) branches together
   if (fe_is_zero(P)) {
-    if (fe_is_zero(R)) return xyzz_double_x(ex, p);  // same point
-    r.inf = true;                                     // opposite points
+    if (fe_is_zero(R)) {
+      IBFT_BRANCH(IBFT_BR_XADD_DBL);
+      return xyzz_double_x(ex, p);  // same point
+    }
+    IBFT_BRANCH(IBFT_BR_XADD_NEG);
+    r.inf = true;                   // opposite points
   }
   return r;
 }

@@ -49,6 +49,20 @@ __device__ unsigned long long g_stage_clk[16];
 #define IBFT_STAGE(i) do { } while (0)
 #endif
 
+// Test instrumentation (tests/emul): counts the exceptional branches of the group law (IBFT_BR_*), so that the emulation tests
+// can show that their crafted signatures reach them.  tests/emul defines IBFT_BRANCH before including the headers; everywhere
+// else it expands to nothing.
+#define IBFT_BR_ADD_DBL 0      // jac_add_affine: P + P (doubling)
+#define IBFT_BR_ADD_NEG 1      // jac_add_affine: P + (-P) (infinity)
+#define IBFT_BR_ADD_INF 2      // jac_add_affine: accumulator at infinity
+#define IBFT_BR_XADD_DBL 3     // xyzz_add_x: P + P
+#define IBFT_BR_XADD_NEG 4     // xyzz_add_x: P + (-P)
+#define IBFT_BR_XADD_INF 5     // xyzz_add_x: accumulator at infinity
+#define IBFT_BR_COUNT 6
+#ifndef IBFT_BRANCH
+#define IBFT_BRANCH(i) do { } while (0)
+#endif
+
 #if defined(__CUDA_ARCH__) && !defined(IBFT_PORTABLE_FE)
 #define IBFT_PTX 1
 #else

@@ -34,6 +34,7 @@ EXPORTS = [
     "ibft_verify_wait", "ibft_bind_groups", "ibft_verify_batch_device", "ibft_quorum_reduce_device", "ibft_quorum_partial_words", "ibft_quorum_mark_device", "ibft_quorum_merge_device", "ibft_quorum_exchange_device",
     "ibft_exchange_alloc", "ibft_exchange_open", "ibft_exchange_close", "ibft_exchange_free", "ibft_exchange_clear",
     "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
+    "ibft_debug_keytab", "ibft_debug_known_handed_back",
 ]
 
 
@@ -102,6 +103,8 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.ibft_sign_batch.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]
     lib.ibft_probe_int_peak.argtypes = [c_void_p, POINTER(c_double), POINTER(c_double)]
     lib.ibft_debug_ctable.argtypes = [c_void_p, c_uint32, c_uint32, c_void_p, POINTER(c_int), POINTER(c_uint32)]
+    lib.ibft_debug_keytab.argtypes = [c_void_p, c_uint32, c_uint32, c_uint32, c_uint32, c_void_p, POINTER(c_uint32), c_void_p]
+    lib.ibft_debug_known_handed_back.argtypes = [c_void_p, POINTER(c_uint32)]
     lib.ibft_debug_op.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_uint32]
     if path is None:
         _LIB = lib
@@ -359,9 +362,26 @@ class Engine:
         return int(wc.value), int(n.value)
 
     def combined_table_entries(self, first: int, count: int) -> np.ndarray:
+        """entries of the generator comb tables: index p * entries + i = entry i of comb position p (position 0 = combined table)"""
         out = np.zeros((count, 16), dtype=np.uint32)
         self._check(self.lib.ibft_debug_ctable(self.handle, first, count, _ptr(out), None, None))
         return out
+
+    def key_table(self, slot: int, validator: int, first: int = 0, count: int = 0):
+        """Key registry entry of a validator (index order): (state, key as 16 little-endian words x||y, `count` comb entries from
+        `first`, entry j * 128 + m - 1 = m * 2^(8j) * Q)."""
+        out = np.zeros((count, 16), dtype=np.uint32)
+        key = np.zeros(16, dtype=np.uint32)
+        st = c_uint32()
+        self._check(self.lib.ibft_debug_keytab(self.handle, slot, validator, first, count, _ptr(out) if count else None, ctypes.byref(st),
+                                               _ptr(key)))
+        return int(st.value), key, out
+
+    def known_handed_back(self) -> int:
+        """items the known-key pass of the most recent completed host-buffer call left to the recover pass"""
+        n = c_uint32()
+        self._check(self.lib.ibft_debug_known_handed_back(self.handle, ctypes.byref(n)))
+        return int(n.value)
 
     # ---- primitive parity hooks (tests)
     def debug_op(self, op: str, a: list[int], b: list[int] | None = None, c: list[bytes] | None = None, out_stride: int = 32):

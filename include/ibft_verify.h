@@ -314,10 +314,23 @@ int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* wide_mac_per
 #define IBFT_DBG_FE_ADD 8   /* out = a+b mod p */
 #define IBFT_DBG_FE_SUB 9   /* out = a-b mod p */
 #define IBFT_DBG_GLV 10     /* out(64) = |k1| (16B BE) || |k2| (16B BE) || sign1 || sign2 padded -- see tests */
-/* Combined generator table (builds with IBFT_WC > 0): *wc = window (0 when absent), *entries = table size; copies `count`
- * 64-byte entries (x, y as 8 little-endian words each) starting at `first`.  Entry index = d1 * (2^wc + 1) + d2 + 2^(wc-1)
- * holds d1*G + d2*lambda*G. */
+/* Generator comb tables (builds with IBFT_WC > 0): *wc = window (0 when absent), *entries = entries of one comb position;
+ * copies `count` 64-byte entries (x, y as 8 little-endian words each) starting at `first`, positions laid out one after the
+ * other: entry p * entries + d1 * (2^wc + 1) + d2 + 2^(wc-1) holds (d1 + d2*lambda) * 2^(wc*p) * G, p = 0..16 (position 0 is
+ * the combined table d1*G + d2*lambda*G). */
 int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count, uint8_t* out, int* wc, uint32_t* entries);
+/* Key registry entry of validator `validator` (validator-index order) of a table slot: *state_out = 0 unknown, 1 learned,
+ * 2 comb table built; key_out (64 bytes) = the learned affine key, x then y as 8 little-endian words; out = `count` comb
+ * entries starting at `first` in the format of ibft_debug_ctable, entry j * 128 + m - 1 = m * 2^(8j) * Q (j = 0..16,
+ * m = 1..128).  Any output may be NULL.  Waits for the device. */
+int ibft_debug_keytab(ibft_engine* e, uint32_t table_slot, uint32_t validator, uint32_t first, uint32_t count, uint8_t* out,
+                      uint32_t* state_out, uint8_t* key_out);
+/* Number of items the known-key pass (IBFT_FLAG_KEY_CACHE) of the most recent completed host-buffer call left to the recover
+ * pass -- signatures of member signers whose key is not known yet or that the verification against the key rejected (the
+ * chain + helper form also settles out-of-range (r, s, v) itself).  0 when the call took no known-key pass.  Same "most recent
+ * call" rule as ibft_last_item_status; IBFT_ERR_INVALID_ARG when that call was so large (more than two 2^17-item chunks) that
+ * it reused a worklist. */
+int ibft_debug_known_handed_back(ibft_engine* e, uint32_t* n_out);
 int ibft_debug_op(ibft_engine* e, int op, const uint8_t* a, const uint8_t* b, const uint8_t* c, uint32_t n,
                   uint8_t* out, uint32_t out_stride);
 

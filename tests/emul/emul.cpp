@@ -5,7 +5,13 @@
 // can be checked against the oracle on a CPU-only box.  This library is never loaded by the product; the product
 // path (csrc/engine.cu) fails loudly without a CUDA device.  The PTX carry-chain multipliers are exercised on the
 // GPU by tests/test_gpu_primitives.py through ibft_debug_op.
+#include <atomic>
 #include <cstring>
+
+// exceptional branches of the group law taken since the last emul_branch_reset (IBFT_BR_* of secp_fe.cuh); entries
+// [IBFT_BR_COUNT, 2 IBFT_BR_COUNT) count the same branches taken inside the split pipelines' final "+ u1 G" only
+static std::atomic<unsigned long long> g_branch[16];
+#define IBFT_BRANCH(i) g_branch[i].fetch_add(1, std::memory_order_relaxed)
 
 #include "../../go-ibft_b200/csrc/verify_core.cuh"
 #include "../../go-ibft_b200/csrc/secp_gtable.inc"
@@ -72,6 +78,16 @@ static gtab_view emul_gview() {
 #else
 static gtab_view emul_gview() { return gtab_view{IBFT_GTABLE}; }
 #endif
+
+// runs f and adds the branches it took to the final-add counters (single-threaded callers only: the tests)
+template <class F>
+static bool count_final_add(F f) {
+  unsigned long long before[IBFT_BR_COUNT];
+  for (int i = 0; i < IBFT_BR_COUNT; i++) before[i] = g_branch[i].load();
+  bool r = f();
+  for (int i = 0; i < IBFT_BR_COUNT; i++) g_branch[IBFT_BR_COUNT + i] += g_branch[i].load() - before[i];
+  return r;
+}
 
 extern "C" {
 
@@ -182,7 +198,7 @@ int emul_verify_item_split(const ibft_sig_item* it, const uint8_t* arena, size_t
   fe y, gx, gy;
   bool g_inf = false;
   if (!split_helper_point(ri, dg, G, y, g_inf, gx, gy)) return 0;  // helper phase 2
-  if (!split_chain_finish(acc, fe_mul(y, gz), g_inf, gx, gy, addr)) return 0;   // chain: map back, + u1 G, address
+  if (!count_final_add([&] { return split_chain_finish(acc, fe_mul(y, gz), g_inf, gx, gy, addr); })) return 0;  // chain: map back, + u1 G, address
   memcpy(recovered20, addr, 20);
   return memcmp(addr, ri.signer, 20) == 0;
 }
@@ -210,7 +226,7 @@ int emul_verify_item_qsplit(const ibft_sig_item* it, const uint8_t* arena, size_
   fe y, gx, gy;
   bool g_inf = false;
   if (!split_helper_point(ri, dg, G, y, g_inf, gx, gy)) return 0;
-  if (!split_chain_finish_x(ex, acc, c, y, g_inf, gx, gy, addr)) return 0;
+  if (!count_final_add([&] { return split_chain_finish_x(ex, acc, c, y, g_inf, gx, gy, addr); })) return 0;
   memcpy(recovered20, addr, 20);
   return memcmp(addr, ri.signer, 20) == 0;
 }
@@ -256,7 +272,7 @@ int emul_verify_item_known(const ibft_sig_item* it, const uint8_t* arena, size_t
     bool g_inf = false;
     fe gx, gy;
     known_helper_u1g(ri, w, G, g_inf, gx, gy);
-    cut = known_chain_finish(acc, g_inf, gx, gy, ri) ? 1 : 0;
+    cut = count_final_add([&] { return known_chain_finish(acc, g_inf, gx, gy, ri); }) ? 1 : 0;
   }
   if (cut != whole) return -2;
   return whole;
@@ -283,6 +299,16 @@ int emul_keytab_positions() { return IBFT_KEYTAB_POSITIONS; }
 
 #endif
 void emul_keccak256(const uint8_t* d, uint32_t n, uint8_t* out) { keccak256_bytes(d, n, out); }
+
+// branch counters: out[i] = times branch IBFT_BR_i was taken since the last reset; returns IBFT_BR_COUNT
+// out[IBFT_BR_COUNT + i] = those of them taken in a split pipeline's final add (emul_verify_item_split / _qsplit)
+int emul_branch_counts(unsigned long long* out /* 2 * IBFT_BR_COUNT */) {
+  for (int i = 0; i < 2 * IBFT_BR_COUNT; i++) out[i] = g_branch[i].load();
+  return IBFT_BR_COUNT;
+}
+void emul_branch_reset() {
+  for (auto& c : g_branch) c.store(0);
+}
 
 // op codes = IBFT_DBG_* of include/ibft_verify.h
 int emul_debug_op(int op, const uint8_t* a, const uint8_t* b, const uint8_t* c, uint8_t* out) {

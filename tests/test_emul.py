@@ -8,10 +8,13 @@ import os
 import random
 
 import numpy as np
+import pytest
 
 from oracle import coracle as co
 from oracle import secp256k1 as ec
 from oracle.keccak import keccak256
+
+import adversarial as A
 
 P, N = ec.P, ec.N
 LAM = 0x5363AD4CC05C30E0A5261C028812645A122E22EA20816678DF02967C1B23BD72
@@ -367,61 +370,31 @@ def test_verify_known_key_is_equivalent_to_recovering_that_key(emul):
         assert run(wl.make_item(sg, bytes(20), 0, keccak256(b"x")), ec.G)[0] == 0
 
 
+def run_known(E, item, key):
+    """(verdict of ecdsa_verify_known against `key`, 1 when the recover path yields exactly that key); -2 = the chain / helper
+    cut of k_verify_split disagreed with the one-thread verification"""
+    zero = np.zeros(1, np.uint8)
+    rk = ctypes.c_int(0)
+    key64 = key[0].to_bytes(32, "big") + key[1].to_bytes(32, "big")
+    ok = E.emul_verify_item_known(item.ctypes.data_as(ctypes.c_void_p), zero.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(0), B(key64),
+                                  ctypes.byref(rk))
+    return ok, rk.value
+
+
 def test_verify_known_comb_edge_digits_and_colliding_points(emul):
-    """The comb walk of ecdsa_verify_known on CONSTRUCTED scalars: half-scalars whose 8-bit Booth digits sit on the window edges
-    (0, +-1, 127, 128, 129, all-0x80 bytes, 2^127, 2^128 - 1), u1 = 0 (zero digest), and keys that make the generator stream and
-    the key stream meet in the adder (Q = G, -G, lambda*G, -lambda*G, 2G: P + P, P - P and a running sum at infinity).
-    A signature (r, s, z) is built FOR the chosen u1 = z/s, u2 = r/s: R = u1*G + u2*Q, r = R.x, s = r/u2, z = u1*s; it is valid by
+    """The comb walk of ecdsa_verify_known on CONSTRUCTED scalars (tests/adversarial.py known_vectors): half-scalars whose 8-bit
+    Booth digits sit on the window edges, u1 = 0 (zero digest), and keys that make the generator stream and the key stream meet
+    in the adder (Q = G, -G, lambda*G, -lambda*G, 2G: P + P, P - P and a running sum at infinity).  Every signature is valid by
     construction, so the verification must accept and the recover path must yield exactly Q."""
     import workloads as wl
-    lam = 0x5363AD4CC05C30E0A5261C028812645A122E22EA20816678DF02967C1B23BD72
-    zero = np.zeros(1, np.uint8)
-
-    def run(item, key):
-        rk = ctypes.c_int(0)
-        key64 = key[0].to_bytes(32, "big") + key[1].to_bytes(32, "big")
-        ok = emul.emul_verify_item_known(item.ctypes.data_as(ctypes.c_void_p), zero.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(0), B(key64),
-                                         ctypes.byref(rk))
-        return ok, rk.value
-
-    def craft(u1, u2, Q):
-        R = ec.point_add(ec.point_mul(u1, ec.G) if u1 else ec.INF, ec.point_mul(u2, Q))
-        if R == ec.INF or R[0] >= N or R[0] == 0:
-            return None
-        r = R[0]
-        s = r * pow(u2, -1, N) % N
-        z = u1 * s % N
-        if s == 0:
-            return None
-        return r.to_bytes(32, "big") + s.to_bytes(32, "big") + bytes([R[1] & 1]), z.to_bytes(32, "big")
-
-    all80 = int.from_bytes(b"\x80" * 16, "big")
-    halves = [0, 1, -1, 127, 128, -128, 129, 255, 256, 0x8000, all80, -all80, 2**127, 2**128 - 1, -(2**127) - 5, 0x7F80 << 64]
-    keys = [1, N - 1, lam, N - lam, 2, 0xC0FFEE]
     built = 0
-    for i, d in enumerate(keys):
-        Q = ec.point_mul(d, ec.G)
-        addr = ec.pubkey_to_address(Q) if hasattr(ec, "pubkey_to_address") else None
-        for j in range(len(halves)):
-            k1, k2 = halves[j], halves[(j * 5 + i) % len(halves)]
-            g1, g2 = halves[(j * 3 + 1) % len(halves)], halves[(j * 7 + i + 2) % len(halves)]
-            u2 = (k1 + k2 * lam) % N
-            u1 = (g1 + g2 * lam) % N
-            if j % 4 == 0:
-                u1 = u2                      # with Q = +-G / +-lambda*G the two streams add the same (or opposite) points
-            if j % 4 == 1:
-                u1 = 0                       # zero digest: no generator term at all
-            if u2 == 0:
-                continue
-            c = craft(u1, u2, Q)
-            if c is None:
-                continue
-            sig, z = c
-            item = wl.make_item(sig, addr if addr else bytes(20), 0, z)
-            assert run(item, Q) == (1, 1), (d, j)
-            # the same signature against ANOTHER key never verifies, and agrees with "does recovery yield that key"
-            assert run(item, ec.point_mul(d + 7, ec.G)) == (0, 0), (d, j)
-            built += 1
+    for v in A.known_vectors():
+        Q = A.known_key(v.key_index)
+        item = wl.make_item(v.sig, A.known_addr(v.key_index), 0, v.digest)
+        assert run_known(emul, item, Q) == (1, 1), v
+        # the same signature against ANOTHER key never verifies, and agrees with "does recovery yield that key"
+        assert run_known(emul, item, ec.point_mul(A.KNOWN_KEYS[v.key_index] + 7, ec.G)) == (0, 0), v
+        built += 1
     assert built >= 60
 
 
@@ -441,3 +414,79 @@ def test_key_comb_table_entries_are_the_stated_multiples(emul):
             e = out.raw[64 * (m - 1): 64 * m]
             assert (int.from_bytes(e[:32], "big"), int.from_bytes(e[32:], "big")) == P, (pos, m)
             P = ec.point_add(P, base)
+
+
+# ------------------------------------------------- crafted exceptional-case vectors (tests/adversarial.py), every pipeline
+BR = dict(ADD_DBL=0, ADD_NEG=1, ADD_INF=2, XADD_DBL=3, XADD_NEG=4, XADD_INF=5)  # IBFT_BR_* of secp_fe.cuh
+FINAL = 6  # counters of the split pipelines' final "+ u1 G" follow the overall ones
+
+
+def branch_counts(E):
+    out = (ctypes.c_ulonglong * 12)()
+    assert E.emul_branch_counts(out) == FINAL
+    return list(out)
+
+
+def test_crafted_vectors_agree_with_the_c_oracle():
+    """the expected values of tests/adversarial.py (big-int oracle) against the C oracle, once"""
+    for v in A.recover_vectors():
+        assert co.ecrecover_address(v.digest, v.sig) == v.addr, v.tag
+        if v.key is not None:  # the vector computes what it was built for: u1 G + u2 R
+            R = ec.lift_x(int.from_bytes(v.sig[:32], "big"), v.sig[64] ^ 0)
+            if int.from_bytes(v.digest, "big") < N and "high-s" not in v.tag:
+                assert v.key == ec.point_add(ec.point_mul(v.u[0], ec.G), ec.point_mul(v.u[1], R)), v.tag
+    for v in A.known_vectors():
+        Q = A.known_key(v.key_index)
+        assert co.ecrecover_pubkey(v.digest, v.sig) == Q[0].to_bytes(32, "big") + Q[1].to_bytes(32, "big")
+    for v in A.known_cancelling():
+        assert co.ecrecover_address(v.digest, v.sig) != A.known_addr(v.key_index)
+    tags = [v.tag for v in A.recover_vectors()]
+    assert sum(t.startswith("final-add inf") for t in tags) >= 10 and sum("z=n" in t for t in tags) >= 4
+
+
+PIPELINES = {  # entry point -> (branch counters that must show the crafted collisions)
+    "emul_verify_item": ("ADD_DBL", "ADD_NEG", "ADD_INF"),
+    "emul_verify_item_levels": ("XADD_DBL", "XADD_NEG", "XADD_INF"),
+    "emul_verify_item_split": ("ADD_DBL", "ADD_NEG", "ADD_INF"),
+    "emul_verify_item_qsplit": ("XADD_DBL", "XADD_NEG", "XADD_INF"),
+}
+
+
+@pytest.mark.parametrize("fn", sorted(PIPELINES))
+def test_crafted_recover_vectors_on_every_pipeline(emul, fn):
+    """Every crafted recover vector gives the oracle's verdict and recovered address (zero when recovery fails, e.g. Q = infinity)
+    on the one-thread, level-structured (four-lane), split and four-lane split pipelines -- and the branch counters prove that the
+    set reaches P + P, P - P and the accumulator at infinity, in the split pipelines' final add too."""
+    zero = np.zeros(1, np.uint8)
+    emul.emul_branch_reset()
+    vecs = A.recover_vectors()
+    for v in vecs:
+        item = A.recover_items([v])
+        out = (ctypes.c_uint8 * 20)()
+        rc = getattr(emul, fn)(item.ctypes.data_as(ctypes.c_void_p), zero.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(0), out)
+        assert (rc, bytes(out)) == (int(v.key is not None), v.addr or bytes(20)), v.tag
+    c = branch_counts(emul)
+    for name in PIPELINES[fn]:
+        assert c[BR[name]] >= 1, (name, c)
+    if "split" in fn:  # (the accumulator u2 R of the final add is never at infinity: 0 < u2 < n)
+        for name in PIPELINES[fn][:2]:
+            assert c[FINAL + BR[name]] >= 1, ("final add", name, c)
+
+
+def test_crafted_known_key_vectors_and_variants(emul):
+    """ecdsa_verify_known and its chain / helper cut on the crafted known-key set: every valid vector accepted (recovery yields Q),
+    a misattributed one (key i presented as validator i + 1), a flipped recovery id and a cancelling u1 G + u2 Q rejected; the
+    counters show P + P and P - P in the walk and P + P / infinity in the cut's final add."""
+    import workloads as wl
+    emul.emul_branch_reset()
+    for v in A.known_vectors():
+        Q = A.known_key(v.key_index)
+        assert run_known(emul, wl.make_item(v.sig, A.known_addr(v.key_index), 0, v.digest), Q) == (1, 1)
+        sig, j = A.misattributed(v)
+        assert run_known(emul, wl.make_item(sig, A.known_addr(j), 0, v.digest), A.known_key(j)) == (0, 0)
+        assert run_known(emul, wl.make_item(A.flipped(v), A.known_addr(v.key_index), 0, v.digest), Q) == (0, 0)
+    for v in A.known_cancelling():
+        assert run_known(emul, wl.make_item(v.sig, A.known_addr(v.key_index), 0, v.digest), A.known_key(v.key_index)) == (0, 0)
+    c = branch_counts(emul)
+    assert c[BR["ADD_DBL"]] >= 1 and c[BR["ADD_NEG"]] >= 1 and c[BR["ADD_INF"]] >= 1, c
+    assert c[FINAL + BR["ADD_DBL"]] >= 1 and c[FINAL + BR["ADD_NEG"]] >= 1, c

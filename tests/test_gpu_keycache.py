@@ -9,6 +9,7 @@ import ibft_b200 as ib
 import workloads as wl
 from oracle import coracle as co
 from oracle import secp256k1 as ec
+from test_gpu_adversarial import bits, expected_handed_back
 from test_gpu_verify import expected_groups, groups_for, load_fixture
 
 pytestmark = pytest.mark.gpu
@@ -37,6 +38,10 @@ def test_learn_then_verify_gives_the_golden_bitmap(name):
         assert np.array_equal(bm2, d["bitmap"])
         assert res1.tobytes() == res2.tobytes()
         assert eng.launch_count() - launches == 3                           # k_verify_known + worklist k_recover + k_quorum_reduce: no table rebuild
+        # every valid signer's key is known now: the known-key pass hands back exactly the member items it cannot accept
+        members = {bytes(a) for a in d["addrs"]}
+        handed = expected_handed_back(items, len(d["arena"]), members, bits(d["bitmap"], len(items)), signers_ok)
+        assert eng.known_handed_back() == handed > 0
         # recovered addresses requested: the recover path must be taken (and give the same answers as a plain engine)
         bm3, _, rec3 = eng.verify_batch(items[:500], d["arena"], groups, want_recovered=True)
         plain = make_engine()
@@ -130,10 +135,16 @@ def test_known_key_latency_path_on_a_10k_round():
         assert np.array_equal(bm2, bm1) and res1.tobytes() == res2.tobytes()
         # four pieces x (k_verify_known + worklist k_recover_qsplit) + k_quorum_reduce; no table rebuild
         assert eng.launch_count() - launches == 9
+        members = {bytes(a) for a in d["addrs"]}
+        known = {bytes(seals[i]["signer"]) for i in range(len(seals)) if gold_bits[i]}
+        gold = gold_bits.astype(bool)
+        assert eng.known_handed_back() == expected_handed_back(seals, 0, members, gold, known) > 0
         for path in (ib.Engine.PATH_SPLIT, ib.Engine.PATH_THREAD):           # k_verify_split / one chunk of k_verify_known
             eng.set_recover_path(path)
             bm3, res3, _ = eng.verify_batch(seals, b"", groups)
             assert np.array_equal(bm3, bm1) and res1.tobytes() == res3.tobytes()
+            split = path == ib.Engine.PATH_SPLIT                             # the chain + helper form settles out-of-range (r, s, v)
+            assert eng.known_handed_back() == expected_handed_back(seals, 0, members, gold, known, split=split) > 0
         eng.set_recover_path(ib.Engine.PATH_AUTO)
         bmp, resp, _ = plain.verify_batch(seals, b"", groups)
         assert np.array_equal(bm2, bmp) and res2.tobytes() == resp.tobytes()
@@ -154,10 +165,13 @@ def test_known_key_latency_path_on_a_10k_round():
             fresh.append(wl.make_item(sig, signer, 2, ph, seal_group))
         fresh = np.concatenate(fresh * 80)[:8000]                           # 8,000 tuples: the chain + helper kernel's range
         a, ra, _ = eng.verify_batch(fresh, b"", groups)
+        handed = eng.known_handed_back()
         b, rb, _ = plain.verify_batch(fresh, b"", groups)
         assert np.array_equal(a, b) and ra.tobytes() == rb.tobytes()
         want = co.verify_batch(fresh, b"", tables=[d["addrs"]], group_table=[0] * len(groups), n_threads=8)
         assert np.array_equal(a, want)
+        # the corrupted and the misattributed copies (and signers whose key round 1 could not learn) go to the recover pass
+        assert handed == expected_handed_back(fresh, 0, members, bits(want, len(fresh)), known) >= 2 * 8000 // len(vs_keys)
     finally:
         eng.close()
         plain.close()
@@ -191,10 +205,14 @@ def test_keys_carry_over_to_the_next_height():
         launches = eng.launch_count()
         a, ra, _ = eng.verify_batch(items, d["arena"], g2)
         assert eng.launch_count() - launches == 3          # known-key pass + worklist pass + quorum: nothing to learn, nothing to build
+        handed = eng.known_handed_back()
         b, rb, _ = plain.verify_batch(items, d["arena"], groups_for(plain, len(d["groups"]), slot=1))
         assert np.array_equal(a, b) and ra.tobytes() == rb.tobytes()
         want = co.verify_batch(items, d["arena"].tobytes(), tables=[addrs2], group_table=[0] * len(d["groups"]), n_threads=8)
         assert np.array_equal(a, want)
+        # carried keys are verified: only the new table's member items that cannot be accepted reach the recover pass
+        members2 = {bytes(x) for x in addrs2}
+        assert handed == expected_handed_back(items, len(d["arena"]), members2, bits(want, len(items)), ok_signers & members2) > 0
         for g in range(len(g2)):
             assert np.array_equal(eng.voted_bitmap(g, len(addrs2)), plain.voted_bitmap(g, len(addrs2)))
         # the same slot re-used for the height after that: the donor is the slot's own previous content

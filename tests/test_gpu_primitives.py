@@ -77,19 +77,27 @@ def test_ecmult(engine):
 
 
 def test_combined_generator_table_entries(engine):
-    """Entries of the device-built combined table (d1*G + d2*lambda*G) against the oracle's scalar multiplication."""
+    """Entries of the device-built generator comb tables against the oracle's scalar multiplication, at EVERY comb position p
+    (position 0 = the combined table d1*G + d2*lambda*G of the window loop; positions 1..16 feed the split kernels' u1*G and the
+    known-key walk): entry (d1, d2) of position p = (d1 + d2*lambda) * 2^(wc*p) * G, edge digits and random ones."""
     wc, n = engine.combined_table_info()
     if wc == 0:
         pytest.skip("library built without a combined generator table")
     half, d2n = 1 << (wc - 1), (1 << wc) + 1
     assert n == (half + 1) * d2n
+    positions = -(-132 // wc)  # comb positions covering the 132 window bits
     rnd = random.Random(26)
-    picks = [(0, 1), (0, -1), (1, 0), (1, 1), (1, -1), (half, half), (half, -half), (0, half), (half, 0), (3, -7)]
-    picks += [(rnd.randint(0, half), rnd.randint(-half, half)) for _ in range(60)]
-    for d1, d2 in picks:
-        e = engine.combined_table_entries(d1 * d2n + d2 + half, 1)[0]
-        x = sum(int(e[i]) << (32 * i) for i in range(8))
-        y = sum(int(e[8 + i]) << (32 * i) for i in range(8))
-        want = co.ecmult2((d1 + d2 * LAM) % N, 0, None)
-        assert (x.to_bytes(32, "big") + y.to_bytes(32, "big")) == want, (d1, d2)
-    assert not engine.combined_table_entries(half, 1)[0].any()        # (0, 0) = infinity: zeros, never looked up
+    edges = [(d1, d2) for d1 in (0, 1, 2, half - 1, half) for d2 in (-half, -half + 1, -1, 0, 1, half - 1, half)]
+    for p in range(positions):
+        picks = edges + [(rnd.randint(0, half), rnd.randint(-half, half)) for _ in range(50)]
+        for d1, d2 in picks:
+            e = engine.combined_table_entries(p * n + d1 * d2n + d2 + half, 1)[0]
+            if (d1, d2) == (0, 0):
+                assert not e.any(), p                                     # infinity: zeros, never looked up
+                continue
+            x = sum(int(e[i]) << (32 * i) for i in range(8))
+            y = sum(int(e[8 + i]) << (32 * i) for i in range(8))
+            want = co.ecmult2((d1 + d2 * LAM) * (1 << (wc * p)) % N, 0, None)
+            assert (x.to_bytes(32, "big") + y.to_bytes(32, "big")) == want, (p, d1, d2)
+    with pytest.raises(Exception):
+        engine.combined_table_entries(positions * n - 1, 2)             # one past the last position
