@@ -79,11 +79,14 @@ struct wire_frame {
   bool has_view;
 };
 
-IBFT_HD bool wire_varint(const uint8_t* w, uint32_t len, uint32_t& pos, uint64_t& v) {  // minimal encoding required
+// minimal encoding required.  The 10th byte carries only bit 63: protobuf-go's protowire.ConsumeVarint rejects a 10th byte
+// above 1 ("variable length integer overflow"), so such a frame never decodes on a Go node and must not be accepted here.
+IBFT_HD bool wire_varint(const uint8_t* w, uint32_t len, uint32_t& pos, uint64_t& v) {
   v = 0;
   for (int shift = 0; shift < 64; shift += 7) {
     if (pos >= len) return false;
     uint8_t b = w[pos++];
+    if (shift == 63 && b > 1) return false;
     v |= (uint64_t)(b & 0x7F) << shift;
     if (!(b & 0x80)) return !(b == 0 && shift > 0);  // a trailing zero group is a non-minimal encoding
   }
@@ -174,9 +177,12 @@ IBFT_HD bool parse_wire_frame(const uint8_t* w, uint32_t len, wire_frame& f) {
     if (k == 1) {
       uint64_t v;
       if (wt != 0 || !wire_varint(w, end, pos, v) || v == 0) return false;  // zero scalars are omitted
-      if (depth == 0 && field == 4) {
-        if (v > 0xFFFFFFFFull) return false;
-        f.type = (uint32_t)v;
+      if (msg == WT_IBFT && field == 4) {
+        // IbftMessage.type is an enum: protobuf-go holds int32(v) and re-encodes it sign-extended, so a value above 2^31 - 1 is
+        // not what it would emit.  The canonical form of a NEGATIVE type (10 bytes, v >= 2^63) is handed back too: the host
+        // decides it, which is always allowed.  Checked at every depth: nested certificate messages are part of the signed bytes.
+        if (v > 0x7FFFFFFFull) return false;
+        if (depth == 0) f.type = (uint32_t)v;
       }
       continue;
     }

@@ -58,7 +58,7 @@ enum PayloadKind : uint8_t { PAYLOAD_NONE = 0, PAYLOAD_PREPREPARE = 5, PAYLOAD_P
 struct IbftMessage {  // messages.proto:24-44
   std::shared_ptr<View> view;  // nullptr == nil view
   Bytes from, signature;
-  uint32_t type = PREPREPARE;
+  uint32_t type = PREPREPARE;  // an int32 enum in protobuf-go: the bit pattern of int32(varint); encoded sign-extended
   PayloadKind payload_kind = PAYLOAD_NONE;  // which oneof member is set (independent of `type`, as in Go)
   // Where this message sits in the gossip frame it was decoded from: [wire_off, wire_off + wire_len) of *root_wire.  Set for the
   // top-level message AND for every message nested in its certificates (they share the root's bytes), so that the GPU verifier can
@@ -134,7 +134,7 @@ inline Bytes encode_message(const IbftMessage& m, bool with_signature) {
   }
   wire::f_bytes(o, 2, m.from);
   if (with_signature) wire::f_bytes(o, 3, m.signature);
-  wire::f_varint(o, 4, m.type);
+  wire::f_varint(o, 4, (uint64_t)(int64_t)(int32_t)m.type);  // protobuf-go: uint64(int64(int32 enum)), 10 bytes when negative
   switch (m.payload_kind) {
     case PAYLOAD_PREPREPARE: {
       Bytes b;
@@ -191,6 +191,8 @@ struct Reader {
     for (;;) {
       if (p >= end || shift > 63) throw DecodeError("truncated/overlong varint");
       uint8_t b = *p++;
+      // protowire.ConsumeVarint: the 10th byte holds bit 63 only; anything above 1 overflows 64 bits
+      if (shift == 63 && b > 1) throw DecodeError("variable length integer overflow");
       v |= (uint64_t)(b & 0x7F) << shift;
       shift += 7;
       if (!(b & 0x80)) return v;
@@ -461,7 +463,7 @@ inline void tree_parse_into(TreeNode& node, TreeType type, Reader r) {
         if (other != num) node.fields.erase(other);
     TreeNode::Field& f = node.fields[num];
     f.kind = kind;
-    if (kind == 1) f.scalar = val;
+    if (kind == 1) f.scalar = (type == T_IBFT && num == 4) ? (uint64_t)(int64_t)(int32_t)val : val;  // the enum `type` is int32
     else if (kind == 2) f.bytes = sub.bytes();
     else if (kind == 4) {
       f.subs.push_back(std::make_unique<TreeNode>());

@@ -71,7 +71,7 @@ class IbftMessage:  # messages.proto:24-44
     view: Optional[View] = None
     from_: bytes = b""
     signature: bytes = b""
-    type: int = PREPREPARE
+    type: int = PREPREPARE  # an int32 enum, as in protobuf-go: decoded as int32(varint), encoded sign-extended
     payload: Payload = None
 
     # set by the decoder for a message that arrived in a NON-canonical encoding (unknown fields, duplicates, ...): the exact bytes,
@@ -172,6 +172,12 @@ class DecodeError(ValueError):
     pass
 
 
+def _int32(v: int) -> int:
+    """protobuf-go's int32(v) of a decoded enum varint (IbftMessage.type)"""
+    v &= 0xFFFFFFFF
+    return v - (1 << 32) if v & 0x80000000 else v
+
+
 def _read_varint(buf: bytes, pos: int):
     shift = 0
     val = 0
@@ -180,6 +186,8 @@ def _read_varint(buf: bytes, pos: int):
             raise DecodeError("truncated/overlong varint")
         b = buf[pos]
         pos += 1
+        if shift == 63 and b > 1:  # protowire.ConsumeVarint: the 10th byte holds bit 63 only
+            raise DecodeError("variable length integer overflow")
         val |= (b & 0x7F) << shift
         shift += 7
         if not b & 0x80:
@@ -298,9 +306,12 @@ def decode_ibft_message(buf: bytes) -> IbftMessage:
 #   * a singular sub-message that appears several times is MERGED field by field (the same rule, recursively);
 #   * a oneof: a different member replaces the one set before, the same member again is merged;
 #   * repeated sub-messages accumulate;
+#   * an enum (IbftMessage.type) is int32: decoding keeps the low 32 bits as a signed value, encoding sign-extends it to 64 bits
+#     (a negative type takes 10 bytes) and omits it when it is 0;
+#   * a varint whose 10th byte is above 1 overflows 64 bits: a decode error (protowire.ConsumeVarint), wherever it appears;
 #   * on output: fields in field-number order, zero scalars and empty bytes omitted, minimal varints.
 _SCHEMA = {
-    "IbftMessage": {1: ("msg", "View"), 2: ("bytes",), 3: ("bytes",), 4: ("varint",), 5: ("oneof", "PrePrepareMessage"),
+    "IbftMessage": {1: ("msg", "View"), 2: ("bytes",), 3: ("bytes",), 4: ("enum",), 5: ("oneof", "PrePrepareMessage"),
                     6: ("oneof", "PrepareMessage"), 7: ("oneof", "CommitMessage"), 8: ("oneof", "RoundChangeMessage")},
     "View": {1: ("varint",), 2: ("varint",)},
     "PrePrepareMessage": {1: ("msg", "Proposal"), 2: ("bytes",), 3: ("msg", "RoundChangeCertificate")},
@@ -382,13 +393,15 @@ def _parse_into(node: _Node, buf: bytes, type_name: str, depth: int = 0) -> None
         if pos > len(buf):
             raise DecodeError("truncated field")
         spec = schema.get(num)
-        want = None if spec is None else (0 if spec[0] == "varint" else 2)
+        want = None if spec is None else (0 if spec[0] in ("varint", "enum") else 2)
         if spec is None or wt != want:
             node.unknown += buf[start:pos]
             continue
         kind = spec[0]
         if kind == "varint":
             node.fields[num] = val
+        elif kind == "enum":
+            node.fields[num] = _int32(val)
         elif kind == "bytes":
             node.fields[num] = bytes(val)
         elif kind == "rep":
@@ -416,7 +429,7 @@ def _emit(node: _Node, type_name: str, skip: tuple = ()) -> bytes:
         if num in skip:
             continue
         spec, v = schema[num], node.fields[num]
-        if spec[0] == "varint":
+        if spec[0] in ("varint", "enum"):
             out += _f_varint(num, v)
         elif spec[0] == "bytes":
             out += _f_bytes(num, v)

@@ -15,10 +15,12 @@ import re
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), "..", ".."))
+sys.path.insert(0, os.path.join(os.path.dirname(__file__), ".."))
 
 from google.protobuf import descriptor_pb2, descriptor_pool, message_factory  # noqa: E402
 
 from oracle import ibft_proto as ip  # noqa: E402
+from edge_frames import EDGE_SEED, EDGE_VALIDATORS, EdgeFrames, sig_tlv, signed_variants  # noqa: E402
 
 REF = "/root/reference/messages/proto/messages.pb.go"
 
@@ -203,6 +205,142 @@ def noncanonical_cases(cls):
     return recs
 
 
+# ----------------------------------------------------------------------------------------------------------- edge frames
+# The frames of tests/edge_frames.py, each recorded by name and Keccak-256 with what protobuf answers for it: whether it decodes,
+# whether decode + encode reproduces it (go_canonical), the Keccak-256 of its re-marshal and of its PayloadNoSig, its nesting
+# levels, every `type` in it, and whether a Go node accepts its sender signature and committed seal.  upb (google.protobuf) and
+# protobuf-go disagree in two places.  protowire.ConsumeVarint rejects a varint whose 10th byte is above 1 ("variable length
+# integer overflow"), while upb masks such a VALUE varint to 64 bits and decodes the frame: for those rows go_parses is false by
+# the protowire rule and the upb_* digests keep what upb did, so the difference stays visible.  The other way round,
+# protobuf-go reads a TAG with ConsumeVarint (up to 10 bytes, field number at most 2^29 - 1) where upb refuses a tag longer than
+# 5 bytes: for such a frame the go_* fields are upb's answers for the same frame with its tags re-encoded minimally, which
+# protobuf-go reads identically, and upb_parses stays false.
+def _pb_levels(pb):
+    """nesting levels of a parsed message (the root is level 1; every present sub-message one more)"""
+    subs = []
+    for fd, v in pb.ListFields():
+        if fd.message_type is None:
+            continue
+        subs += list(v) if fd.is_repeated else [v]
+    return 1 + max((_pb_levels(s) for s in subs), default=0)
+
+
+def _pb_types(pb):
+    """IbftMessage.type of the message and of every IbftMessage nested in it"""
+    out = [pb.type] if pb.DESCRIPTOR.name == "IbftMessage" else []
+    for fd, v in pb.ListFields():
+        if fd.message_type is not None:
+            for s in (list(v) if fd.is_repeated else [v]):
+                out += _pb_types(s)
+    return out
+
+
+class _Overflow(Exception):
+    pass
+
+
+def _protowire_read(buf: bytes, desc):
+    """protobuf-go's reading of buf as `desc`: buf with every tag re-encoded minimally (sub-message length prefixes follow), which
+    upb reads the way protobuf-go reads buf; None when buf is malformed.  Raises _Overflow where protowire.ConsumeVarint reports
+    an overflow (a 10th byte above 1)."""
+    out, pos = bytearray(), 0
+
+    def rv():
+        nonlocal pos
+        v, shift, start = 0, 0, pos
+        while True:
+            b = buf[pos]
+            pos += 1
+            if shift == 63 and b > 1:
+                raise _Overflow
+            v |= (b & 0x7F) << shift
+            shift += 7
+            if not b & 0x80:
+                return v, buf[start:pos]
+    try:
+        while pos < len(buf):
+            key, _ = rv()
+            out += ip._varint(key)
+            num, wt = key >> 3, key & 7
+            if wt == 0:
+                out += rv()[1]
+            elif wt in (1, 5):
+                n = 8 if wt == 1 else 4
+                out += buf[pos:pos + n]
+                pos += n
+            elif wt == 2:
+                ln, raw = rv()
+                body = buf[pos:pos + ln]
+                pos += ln
+                fd = desc.fields_by_number.get(num)
+                inner = _protowire_read(body, fd.message_type) if fd is not None and fd.message_type is not None else body
+                if inner is None:
+                    return None
+                out += (raw if inner == body else ip._varint(len(inner))) + inner
+            else:
+                return None
+        return bytes(out) if pos == len(buf) else None
+    except IndexError:
+        return None
+
+
+def edge_cases(cls):
+    import workloads as wl
+    from oracle import coracle as co
+    M = cls["IbftMessage"]
+    E = EdgeFrames()
+    key = E.vs.keys[0]
+
+    def keccak_hex(b):
+        return co.keccak256(b).hex()
+
+    def answers(wire):
+        rec = {"upb_parses": False, "go_parses": False}
+        try:
+            go_src = _protowire_read(wire, M.DESCRIPTOR)  # None: protobuf-go cannot decode the frame
+        except _Overflow:
+            go_src = None
+        try:
+            pb, src = M.FromString(wire), wire
+            rec.update(upb_parses=True)
+        except Exception:
+            if go_src is None or go_src == wire:
+                return rec, None
+            try:
+                pb, src = M.FromString(go_src), go_src    # over-long tags: protobuf-go reads them, upb does not
+            except Exception:
+                return rec, None
+        full = pb.SerializeToString(deterministic=True)
+        nosig = M.FromString(src)
+        nosig.signature = b""
+        nosig = nosig.SerializeToString(deterministic=True)
+        if go_src is None:
+            rec.update(upb_remarshal_keccak=keccak_hex(full), upb_payload_no_sig_keccak=keccak_hex(nosig))  # upb's answer, not Go's
+            return rec, None
+        rec.update(go_parses=True, go_canonical=full == wire, go_remarshal_keccak=keccak_hex(full), go_payload_no_sig_keccak=keccak_hex(nosig),
+                   go_levels=_pb_levels(pb), go_types=_pb_types(pb))
+        # IsValidValidator (core/backend.go:41-45) and IsValidCommittedSeal on the frame, as a Go node decides them
+        frm = getattr(pb, "from")
+        sender = pb.HasField("view") and len(frm) == 20 and len(pb.signature) == 65 and \
+            co.ecrecover_address(co.keccak256(nosig), pb.signature) == frm
+        cd = pb.commitData
+        seal = pb.type == ip.COMMIT and pb.WhichOneof("payload") == "commitData" and len(frm) == 20 and len(cd.proposalHash) == 32 and \
+            len(cd.committedSeal) == 65 and co.ecrecover_address(wl.seal_digest(cd.proposalHash), cd.committedSeal) == frm
+        rec.update(go_sender_valid=bool(sender), go_seal_valid=bool(seal))
+        return rec, nosig
+
+    recs, seen = [], set()
+    for name, body in E.bases():
+        _, go_nosig = answers(body(sig_tlv(b"\x00" * 65)))
+        for vlab, wire in signed_variants(body, key, None if go_nosig is None else co.keccak256(go_nosig)):
+            if wire in seen:      # the same bytes reached through two edges are recorded once
+                continue
+            seen.add(wire)
+            rec, _ = answers(wire)
+            recs.append({"name": "%s/%s" % (name, vlab), "wire_keccak": keccak_hex(wire), **rec})
+    return recs
+
+
 def main():
     cls = load_reference_classes()
     recs = []
@@ -213,10 +351,14 @@ def main():
         nosig = pb.SerializeToString(deterministic=True)
         recs.append({"name": name, "model": repr(m), "wire": wire.hex(), "payload_no_sig": nosig.hex()})
     path = os.path.join(os.path.dirname(__file__), "proto_wire.json")
-    json.dump({"generator": "tests/golden/make_proto_golden.py",
-               "source": "descriptor embedded in reference messages/proto/messages.pb.go (protoc-gen-go v1.28.1)",
-               "cases": recs, "noncanonical": noncanonical_cases(cls)}, open(path, "w"), indent=1)
-    print("wrote", path, len(recs), "cases")
+    edges = edge_cases(cls)
+    text = json.dumps({"generator": "tests/golden/make_proto_golden.py",
+                       "source": "descriptor embedded in reference messages/proto/messages.pb.go (protoc-gen-go v1.28.1)",
+                       "cases": recs, "noncanonical": noncanonical_cases(cls), "edge_validators": [EDGE_SEED, EDGE_VALIDATORS],
+                       "edges": "EDGES"}, indent=1)
+    rows = ",\n  ".join(json.dumps(r, separators=(",", ":")) for r in edges)   # one edge frame per line
+    open(path, "w").write(text.replace('"EDGES"', "[\n  " + rows + "\n ]"))
+    print("wrote", path, len(recs), "cases", len(edges), "edge frames")
 
 
 if __name__ == "__main__":

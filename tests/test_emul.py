@@ -117,9 +117,43 @@ def test_config2_fixture_bit_exact(emul):
 
 
 # ----------------------------------------------------------------------------------------------- raw gossip frames
+WIRE_MAX_DEPTH = 12  # IBFT_WIRE_MAX_DEPTH of csrc/verify_core.cuh: nesting levels the device walks
+
+
+def frame_shape(m, level: int = 1):
+    """(nesting levels, [type of every IbftMessage]) of a decoded frame; the root is level 1, every present sub-message one more"""
+    from oracle import ibft_proto as ip
+    depth, types = level + (m.view is not None), [m.type]
+    p = m.payload
+    if p is None:
+        return depth, types
+    depth = max(depth, level + 1)
+    inner = []
+    if isinstance(p, ip.PrePrepareMessage):
+        if p.proposal is not None:
+            depth = max(depth, level + 2)
+        if p.certificate is not None:
+            depth = max(depth, level + 2)
+            inner = p.certificate.round_change_messages
+    elif isinstance(p, ip.RoundChangeMessage):
+        if p.last_prepared_proposal is not None:
+            depth = max(depth, level + 2)
+        pc = p.latest_prepared_certificate
+        if pc is not None:
+            depth = max(depth, level + 2)
+            inner = ([pc.proposal_message] if pc.proposal_message is not None else []) + list(pc.prepare_messages or [])
+    for x in inner:
+        d, t = frame_shape(x, level + 3)
+        depth, types = max(depth, d), types + t
+    return depth, types
+
+
 def wire_expectation(wire: bytes, kind: int, members):
-    """(status, verdict) the device must produce for a KIND_WIRE / KIND_WIRE_SEAL item, derived from the oracle codec
-    (canonical <=> decode+encode reproduces the frame) and the oracle verifier."""
+    """(status, verdict) the device must produce for a KIND_WIRE / KIND_WIRE_SEAL item, derived from the oracle codec, which
+    decodes the way protobuf-go does (canonical <=> decode + encode reproduces the frame), and the oracle verifier.  A frame
+    protobuf-go cannot decode, or one it would re-encode differently, comes back NEEDS_HOST.  So do exactly two kinds of
+    canonical frames, which the device hands back on purpose: one nested deeper than IBFT_WIRE_MAX_DEPTH, and one with a
+    negative `type` anywhere in it (the canonical 10-byte form of an int32 enum below zero)."""
     import workloads as wl
     from oracle import ibft_proto as ip
     try:
@@ -128,6 +162,9 @@ def wire_expectation(wire: bytes, kind: int, members):
         return 1, False
     if ip.encode_ibft_message(m) != wire:
         return 1, False           # not canonical: the device hands the frame back, it never guesses
+    levels, types = frame_shape(m)
+    if levels > WIRE_MAX_DEPTH or min(types) < 0:
+        return 1, False           # canonical, but one of the two allowed conservative hand-backs
     if len(m.from_) != 20:
         return 0, False
     if kind == 3:
