@@ -54,13 +54,39 @@ IBFT_HD fe fe_beta() {
 #define DSQR PSQR
 #endif
 
+// The doubling's first three products in ONE out-of-line call (each with its own inlined squarer body) instead of three calls
+// and their operand copies, and the rarely taken P + P case of the mixed addition out of the window loop's code.  Nothing more is
+// fused: the window loop and the routines it calls must stay within about 27 KB of SASS.  Larger groups (the front of the
+// mixed addition, pairs of independent products) remove more FMA-pipe instructions but ran slower on an H100 (DESIGN.md §3.1),
+// the same instruction-cache wall that whole inlined point routines hit (IBFT_POINT_BYVAL, IBFT_POINT_INLINE).
+#if !defined(IBFT_POINT_INLINE) && !defined(IBFT_DBL_INLINE)
+#define IBFT_DBL_FRONT 1
+#endif
+struct dbl_abc {
+  fe a, b, c;
+};
+// doubling: A = X^2, B = Y^2, C = B^2
+IBFT_FN dbl_abc jac_dbl_front(fe x, fe y) {
+  IBFT_OPCOUNT(IBFT_OP_DBL_FRONT);
+  dbl_abc r;
+  r.a = fe_sqr_i(x);
+  r.b = fe_sqr_i(y);
+  r.c = fe_sqr_i(r.b);
+  return r;
+}
+
 // dbl-2009-l: 2M + 5S
 IBFT_PT jac jac_double_body(const jac& p) {
   jac r;
   // Y = 0 never happens on secp256k1 (no points of order 2), so no exceptional case besides infinity.
+#if defined(IBFT_DBL_FRONT)
+  const dbl_abc abc = jac_dbl_front(p.x, p.y);
+  const fe a = abc.a, b = abc.b, c = abc.c;
+#else
   fe a = DSQR(p.x);
   fe b = DSQR(p.y);
   fe c = DSQR(b);
+#endif
   fe t = fe_add(p.x, b);
   t = DSQR(t);
   t = fe_sub(t, a);
@@ -75,6 +101,36 @@ IBFT_PT jac jac_double_body(const jac& p) {
   r.inf = p.inf;
   return r;
 }
+
+#if defined(IBFT_DBL_FRONT) && !(defined(IBFT_POINT_BYVAL) && defined(__CUDA_ARCH__))
+// P + P inside the mixed addition, out of line (the point travels by value, in registers): inlined, this doubling sat in the
+// window loop's code -- 440 instructions, 7 KB -- for a branch that only crafted signatures take.
+struct jac_words {
+  uint32_t w[24];
+};
+IBFT_FN jac_words jac_double_rare(jac_words in) {
+  jac p;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { p.x.v[i] = in.w[i]; p.y.v[i] = in.w[8 + i]; p.z.v[i] = in.w[16 + i]; }
+  p.inf = false;
+  const jac r = jac_double_body(p);
+  jac_words o;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { o.w[i] = r.x.v[i]; o.w[8 + i] = r.y.v[i]; o.w[16 + i] = r.z.v[i]; }
+  return o;
+}
+IBFT_HD jac jac_double_ool(const jac& p) {
+  jac_words in;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { in.w[i] = p.x.v[i]; in.w[8 + i] = p.y.v[i]; in.w[16 + i] = p.z.v[i]; }
+  const jac_words o = jac_double_rare(in);
+  jac r;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { r.x.v[i] = o.w[i]; r.y.v[i] = o.w[8 + i]; r.z.v[i] = o.w[16 + i]; }
+  r.inf = p.inf;
+  return r;
+}
+#endif
 
 #if defined(IBFT_POINT_BYVAL) && defined(__CUDA_ARCH__)
 // IBFT_POINT_BYVAL: the two hot group-law routines are out-of-line functions taking the point BY VALUE (the whole accumulator
@@ -129,6 +185,9 @@ IBFT_PT jac jac_double(const jac& p) { return jac_double_body(p); }
 #endif
 
 // p + (qx, qy) with q affine (never infinity): 8M + 3S.  h_out (optional): Z3 / Z1 of the generic case (= H), 1 otherwise.
+// OPT-IN -DIBFT_MADD_7M4S: madd-2007-bl, 7M + 4S -- Z3 = (Z1 + H)^2 - Z1Z1 - HH = 2 Z1 H trades the multiplication Z1 H for a
+// squaring, and X3, Y3 carry the matching factors 4 and 8 (I = 4 HH, r = 2 (S2 - Y1)); h_out is then 2H.  Slower on an H100
+// (DESIGN.md §3.1): the seven extra additions cost more issue slots and code than the 28 wide MACs it saves.
 #if defined(IBFT_POINT_BYVAL) && defined(__CUDA_ARCH__)
 // generic case only; *flag = 0 generic result, 1 = P + P (caller doubles), 2 = P + (-P) (infinity)
 struct jac33 { uint32_t w[33]; };
@@ -144,14 +203,26 @@ __device__ __noinline__ jac33 jac_madd_v(jac24 in, fe qx, fe qy) {
   uint32_t flag = 0;
   if (fe_is_zero(h)) flag = fe_is_zero(rr) ? 1u : 2u;
   fe hh = PSQR(h);
+#if defined(IBFT_MADD_7M4S)
+  fe i4 = fe_dbl(fe_dbl(hh));
+  fe j = PMUL(h, i4);
+  fe r2 = fe_dbl(rr);
+  fe v = PMUL(p.x, i4);
+  fe rx = fe_sub(fe_sub(PSQR(r2), j), fe_dbl(v));
+  fe ry = fe_sub(PMUL(r2, fe_sub(v, rx)), fe_dbl(PMUL(p.y, j)));
+  fe rz = fe_sub(fe_sub(PSQR(fe_add(p.z, h)), z1z1), hh);
+  fe h2 = fe_dbl(h);
+#else
   fe hhh = PMUL(h, hh);
   fe v = PMUL(p.x, hh);
   fe rx = fe_sub(fe_sub(PSQR(rr), hhh), fe_dbl(v));
   fe ry = fe_sub(PMUL(rr, fe_sub(v, rx)), PMUL(p.y, hhh));
   fe rz = PMUL(p.z, h);
+  fe h2 = h;
+#endif
   jac33 o;
 #pragma unroll
-  for (int i = 0; i < 8; i++) { o.w[i] = rx.v[i]; o.w[8 + i] = ry.v[i]; o.w[16 + i] = rz.v[i]; o.w[24 + i] = h.v[i]; }
+  for (int i = 0; i < 8; i++) { o.w[i] = rx.v[i]; o.w[8 + i] = ry.v[i]; o.w[16 + i] = rz.v[i]; o.w[24 + i] = h2.v[i]; }
   o.w[32] = flag;
   return o;
 }
@@ -204,7 +275,11 @@ IBFT_PT jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, fe* h_out =
   if (fe_is_zero(h)) {
     if (fe_is_zero(rr)) {
       IBFT_BRANCH(IBFT_BR_ADD_DBL);
+#if defined(IBFT_DBL_FRONT)
+      return jac_double_ool(p);  // P + P (rare)
+#else
       return jac_double(p);  // P + P (rare; kept inline so that `p` never has its address taken)
+#endif
     }
     IBFT_BRANCH(IBFT_BR_ADD_NEG);
     r = p;
@@ -212,6 +287,17 @@ IBFT_PT jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, fe* h_out =
     return r;
   }
   fe hh = PSQR(h);
+#if defined(IBFT_MADD_7M4S)
+  fe i4 = fe_dbl(fe_dbl(hh));  // I = (2H)^2
+  fe j = PMUL(h, i4);          // J = H I
+  fe r2 = fe_dbl(rr);          // r = 2 (S2 - Y1)
+  fe v = PMUL(p.x, i4);        // V = X1 I
+  r.x = fe_sub(fe_sub(PSQR(r2), j), fe_dbl(v));
+  r.y = fe_sub(PMUL(r2, fe_sub(v, r.x)), fe_dbl(PMUL(p.y, j)));
+  r.z = fe_sub(fe_sub(PSQR(fe_add(p.z, h)), z1z1), hh);
+  r.inf = false;
+  if (h_out) *h_out = fe_dbl(h);
+#else
   fe hhh = PMUL(h, hh);
   fe v = PMUL(p.x, hh);
   r.x = fe_sub(fe_sub(PSQR(rr), hhh), fe_dbl(v));
@@ -219,6 +305,7 @@ IBFT_PT jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, fe* h_out =
   r.z = PMUL(p.z, h);
   r.inf = false;
   if (h_out) *h_out = h;
+#endif
   return r;
 }
 #endif
@@ -613,9 +700,13 @@ IBFT_HD jac ecmult_streams(const ecmult_digits& dg, const gtab_view& G, const rt
   acc.inf = true;
   IBFT_ROLLED
   for (int j = IBFT_NWIN_R - 1; j >= 0; j--) {
+    IBFT_OPCOUNT(IBFT_OP_WIN);
     if (!acc.inf) {
       IBFT_ROLLED
-      for (int t = 0; t < IBFT_WR; t++) acc = jac_double(acc);
+      for (int t = 0; t < IBFT_WR; t++) {
+        IBFT_OPCOUNT(IBFT_OP_WIN_DBL);
+        acc = jac_double(acc);
+      }
     }
     // streams 0,1: R and lambda*R every window; streams 2,3: G and lambda*G every (WG/WR)-th window -- or, with a combined
     // table, ONE stream for both generator halves every (WC/WR)-th window
@@ -652,6 +743,7 @@ IBFT_HD jac ecmult_streams(const ecmult_digits& dg, const gtab_view& G, const rt
       }
       if (use_beta) x = fe_mul(x, beta);  // lambda * (x, y) = (beta x, y)
       if (neg) y = fe_neg(y);
+      IBFT_OPCOUNT(IBFT_OP_WIN_ADD);
       acc = jac_add_affine(acc, x, y);
     }
   }

@@ -63,6 +63,27 @@ __device__ unsigned long long g_stage_clk[16];
 #define IBFT_BRANCH(i) do { } while (0)
 #endif
 
+// Test instrumentation (tests/emul/opcount.cpp, read by tools/fma_budget.py): dynamic operation counts of one recovery
+// (IBFT_OP_*), which the FMA-pipe ledger multiplies by the per-routine instruction counts of the SASS.  Expands to nothing
+// everywhere else, the plain host emulation (tests/emul/emul.cpp) included.
+#define IBFT_OP_MUL_BODY 0     // field multiplications (inlined multiplier bodies, wherever they run)
+#define IBFT_OP_SQR_BODY 1     // field squarings (inlined squarer bodies, wherever they run)
+#define IBFT_OP_MUL_CALL 2     // calls of the out-of-line multiplier fe_mul
+#define IBFT_OP_SQR_CALL 3     // calls of the out-of-line squarer fe_sqr
+#define IBFT_OP_SQRN_CALL 4    // calls of fe_sqrn
+#define IBFT_OP_SQRN_ITER 5    // squarings inside fe_sqrn
+#define IBFT_OP_DBL_FRONT 6    // calls of jac_dbl_front (doubling: A, B, C)
+#define IBFT_OP_FE_INV 7       // field inversions (safegcd)
+#define IBFT_OP_SC_INV 8       // scalar inversions (safegcd)
+#define IBFT_OP_INV_ITER 9     // safegcd iterations (30 divsteps each), both kinds
+#define IBFT_OP_WIN 10         // window-loop iterations
+#define IBFT_OP_WIN_DBL 11     // doublings inside the window loop
+#define IBFT_OP_WIN_ADD 12     // mixed additions inside the window loop
+#define IBFT_OP_COUNT 13
+#ifndef IBFT_OPCOUNT
+#define IBFT_OPCOUNT(k) do { } while (0)
+#endif
+
 #if defined(__CUDA_ARCH__) && !defined(IBFT_PORTABLE_FE)
 #define IBFT_PTX 1
 #else
@@ -289,19 +310,8 @@ __device__ __forceinline__ void mad_chain4_nc(uint32_t& p0, uint32_t& p1, uint32
       : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "+r"(p4), "+r"(p5), "+r"(p6), "+r"(p7)
       : "r"(x0), "r"(x1), "r"(x2), "r"(x3), "r"(y));
 }
-// the top pair is (carry register, FRESH): the fresh half is written with a literal-zero addend, so no register has to be
-// zero-initialised beforehand (saves 16 moves per multiplication on the FMA pipe, which is the busy one)
-__device__ __forceinline__ void mad_chain4_ncz(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t& p4,
-                                               uint32_t& p5, uint32_t& p6, uint32_t& p7_out, uint32_t x0, uint32_t x1,
-                                               uint32_t x2, uint32_t x3, uint32_t y) {
-  asm("mad.lo.cc.u32 %0,%8,%12,%0;\n\tmadc.hi.cc.u32 %1,%8,%12,%1;\n\t"
-      "madc.lo.cc.u32 %2,%9,%12,%2;\n\tmadc.hi.cc.u32 %3,%9,%12,%3;\n\t"
-      "madc.lo.cc.u32 %4,%10,%12,%4;\n\tmadc.hi.cc.u32 %5,%10,%12,%5;\n\t"
-      "madc.lo.cc.u32 %6,%11,%12,%6;\n\tmadc.hi.u32 %7,%11,%12,0;"
-      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "+r"(p4), "+r"(p5), "+r"(p6), "=r"(p7_out)
-      : "r"(x0), "r"(x1), "r"(x2), "r"(x3), "r"(y));
-}
-// both halves of the top pair are fresh
+// both halves of the top pair are fresh: they are written with literal-zero addends, so no register has to be
+// zero-initialised beforehand (moves on the FMA pipe, which is the busy one)
 __device__ __forceinline__ void mad_chain4_nczz(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t& p4,
                                                 uint32_t& p5, uint32_t& p6_out, uint32_t& p7_out, uint32_t x0, uint32_t x1,
                                                 uint32_t x2, uint32_t x3, uint32_t y) {
@@ -310,6 +320,20 @@ __device__ __forceinline__ void mad_chain4_nczz(uint32_t& p0, uint32_t& p1, uint
       "madc.lo.cc.u32 %4,%10,%12,%4;\n\tmadc.hi.cc.u32 %5,%10,%12,%5;\n\t"
       "madc.lo.cc.u32 %6,%11,%12,0;\n\tmadc.hi.u32 %7,%11,%12,0;"
       : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "+r"(p4), "+r"(p5), "=r"(p6_out), "=r"(p7_out)
+      : "r"(x0), "r"(x1), "r"(x2), "r"(x3), "r"(y));
+}
+// acc pairs (p0,p1),(p2,p3),(p4,p5),(p6,p7) += x0*y, x1*y, x2*y, x3*y, the carry out rippled into (p8, p9), which the caller
+// guarantees cannot carry out.  Used where the pair above the chain has already been written by a later row: a carry never
+// has to sit in a register pair whose other half is a materialised zero (an IMAD.MOV on the FMA pipe).
+__device__ __forceinline__ void mad_chain4_r2(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t& p4, uint32_t& p5,
+                                              uint32_t& p6, uint32_t& p7, uint32_t& p8, uint32_t& p9, uint32_t x0, uint32_t x1,
+                                              uint32_t x2, uint32_t x3, uint32_t y) {
+  asm("mad.lo.cc.u32 %0,%10,%14,%0;\n\tmadc.hi.cc.u32 %1,%10,%14,%1;\n\t"
+      "madc.lo.cc.u32 %2,%11,%14,%2;\n\tmadc.hi.cc.u32 %3,%11,%14,%3;\n\t"
+      "madc.lo.cc.u32 %4,%12,%14,%4;\n\tmadc.hi.cc.u32 %5,%12,%14,%5;\n\t"
+      "madc.lo.cc.u32 %6,%13,%14,%6;\n\tmadc.hi.cc.u32 %7,%13,%14,%7;\n\t"
+      "addc.cc.u32 %8,%8,0;\n\taddc.u32 %9,%9,0;"
+      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "+r"(p4), "+r"(p5), "+r"(p6), "+r"(p7), "+r"(p8), "+r"(p9)
       : "r"(x0), "r"(x1), "r"(x2), "r"(x3), "r"(y));
 }
 __device__ __forceinline__ void mulw(uint32_t& lo, uint32_t& hi, uint32_t x, uint32_t y) {
@@ -409,23 +433,28 @@ IBFT_HD void mul_wide_8x8(uint32_t* R, const uint32_t* a, const uint32_t* b) {
         "r"(z1[8]));
 #elif IBFT_PTX
   // E[k] sits at limb position k, O[k] at position k+1 (see DESIGN.md "field multiplier").  No accumulator is ever
-  // zero-initialised: fresh halves are produced by literal-zero addends, carries by addc.
+  // zero-initialised: fresh halves are produced by literal-zero addends, carries by addc.  Rows are taken in pairs so that no
+  // carry word is ever paired with a materialised zero either: the LATER row's chain runs first and writes the top pair fresh,
+  // then the earlier row's chain ripples its carry into that pair (every partial sum is a partial product: nothing overflows).
   uint32_t E[16], O[15];
   mulw(E[0], E[1], a[0], b[0]); mulw(E[2], E[3], a[2], b[0]); mulw(E[4], E[5], a[4], b[0]); mulw(E[6], E[7], a[6], b[0]);
   mulw(O[0], O[1], a[1], b[0]); mulw(O[2], O[3], a[3], b[0]); mulw(O[4], O[5], a[5], b[0]); mulw(O[6], O[7], a[7], b[0]);
-  // row 1: O indices 0..6 carry out -> O[8]; E indices 2..8 where (E[8], E[9]) are both fresh
-  O[8] = mad_chain4(O[0], O[1], O[2], O[3], O[4], O[5], O[6], O[7], a[0], a[2], a[4], a[6], b[1]);
+  // row 1, E: indices 2..9 where (E[8], E[9]) are both fresh
   mad_chain4_nczz(E[2], E[3], E[4], E[5], E[6], E[7], E[8], E[9], a[1], a[3], a[5], a[7], b[1]);
 #pragma unroll
-  for (int i = 2; i < 8; i++) {
-    if (i & 1) {
-      O[i + 7] = mad_chain4(O[i - 1], O[i], O[i + 1], O[i + 2], O[i + 3], O[i + 4], O[i + 5], O[i + 6], a[0], a[2], a[4], a[6], b[i]);
-      mad_chain4_ncz(E[i + 1], E[i + 2], E[i + 3], E[i + 4], E[i + 5], E[i + 6], E[i + 7], E[i + 8], a[1], a[3], a[5], a[7], b[i]);
-    } else {
-      E[i + 8] = mad_chain4(E[i], E[i + 1], E[i + 2], E[i + 3], E[i + 4], E[i + 5], E[i + 6], E[i + 7], a[0], a[2], a[4], a[6], b[i]);
-      mad_chain4_ncz(O[i], O[i + 1], O[i + 2], O[i + 3], O[i + 4], O[i + 5], O[i + 6], O[i + 7], a[1], a[3], a[5], a[7], b[i]);
+  for (int i = 1; i < 7; i++) {
+    if (i & 1) {  // O: row i+1 with (O[i+7], O[i+8]) fresh, then row i rippling into them
+      mad_chain4_nczz(O[i + 1], O[i + 2], O[i + 3], O[i + 4], O[i + 5], O[i + 6], O[i + 7], O[i + 8], a[1], a[3], a[5], a[7], b[i + 1]);
+      mad_chain4_r2(O[i - 1], O[i], O[i + 1], O[i + 2], O[i + 3], O[i + 4], O[i + 5], O[i + 6], O[i + 7], O[i + 8], a[0], a[2], a[4],
+                    a[6], b[i]);
+    } else {      // E: row i+1 with (E[i+8], E[i+9]) fresh, then row i rippling into them
+      mad_chain4_nczz(E[i + 2], E[i + 3], E[i + 4], E[i + 5], E[i + 6], E[i + 7], E[i + 8], E[i + 9], a[1], a[3], a[5], a[7], b[i + 1]);
+      mad_chain4_r2(E[i], E[i + 1], E[i + 2], E[i + 3], E[i + 4], E[i + 5], E[i + 6], E[i + 7], E[i + 8], E[i + 9], a[0], a[2], a[4],
+                    a[6], b[i]);
     }
   }
+  // row 7, O: indices 6..13, carry out -> O[14]
+  O[14] = mad_chain4(O[6], O[7], O[8], O[9], O[10], O[11], O[12], O[13], a[0], a[2], a[4], a[6], b[7]);
   // R = E + (O << 32)
   R[0] = E[0];
   asm("add.cc.u32 %0,%15,%30;\n\taddc.cc.u32 %1,%16,%31;\n\taddc.cc.u32 %2,%17,%32;\n\taddc.cc.u32 %3,%18,%33;\n\t"
@@ -497,30 +526,30 @@ IBFT_HD fe fe_reduce512(const uint32_t* R) {
           "r"(U[3]), "r"(U[4]), "r"(U[5]), "r"(U[6]), "r"(U[7]), "r"(U[8]));
     s9 = 0;
   }
-#else
-  uint32_t t0, t1, t2, t3, t4, t5, t6, t7, u0, u1, u2, u3, u4, u5, u6, u7;
-  mulw(t0, t1, R[8], IBFT_PC); mulw(t2, t3, R[10], IBFT_PC); mulw(t4, t5, R[12], IBFT_PC); mulw(t6, t7, R[14], IBFT_PC);
-  mulw(u0, u1, R[9], IBFT_PC); mulw(u2, u3, R[11], IBFT_PC); mulw(u4, u5, R[13], IBFT_PC); mulw(u6, u7, R[15], IBFT_PC);
-  // S = L + Te
-  asm("add.cc.u32 %0,%9,%17;\n\taddc.cc.u32 %1,%10,%18;\n\taddc.cc.u32 %2,%11,%19;\n\taddc.cc.u32 %3,%12,%20;\n\t"
-      "addc.cc.u32 %4,%13,%21;\n\taddc.cc.u32 %5,%14,%22;\n\taddc.cc.u32 %6,%15,%23;\n\taddc.cc.u32 %7,%16,%24;\n\t"
-      "addc.u32 %8,0,0;"
-      : "=r"(S[0]), "=r"(S[1]), "=r"(S[2]), "=r"(S[3]), "=r"(S[4]), "=r"(S[5]), "=r"(S[6]), "=r"(S[7]), "=r"(s8)
-      : "r"(R[0]), "r"(R[1]), "r"(R[2]), "r"(R[3]), "r"(R[4]), "r"(R[5]), "r"(R[6]), "r"(R[7]), "r"(t0), "r"(t1), "r"(t2),
-        "r"(t3), "r"(t4), "r"(t5), "r"(t6), "r"(t7));
-  // S[1..8] += To ; S[9] = carry
-  asm("add.cc.u32 %0,%0,%9;\n\taddc.cc.u32 %1,%1,%10;\n\taddc.cc.u32 %2,%2,%11;\n\taddc.cc.u32 %3,%3,%12;\n\t"
-      "addc.cc.u32 %4,%4,%13;\n\taddc.cc.u32 %5,%5,%14;\n\taddc.cc.u32 %6,%6,%15;\n\taddc.cc.u32 %7,%7,%16;\n\t"
-      "addc.u32 %8,0,0;"
-      : "+r"(S[1]), "+r"(S[2]), "+r"(S[3]), "+r"(S[4]), "+r"(S[5]), "+r"(S[6]), "+r"(S[7]), "+r"(s8), "=r"(s9)
-      : "r"(u0), "r"(u1), "r"(u2), "r"(u3), "r"(u4), "r"(u5), "r"(u6), "r"(u7));
-#endif
   // S[1..8] += H ; S[9] += carry
   asm("add.cc.u32 %0,%0,%9;\n\taddc.cc.u32 %1,%1,%10;\n\taddc.cc.u32 %2,%2,%11;\n\taddc.cc.u32 %3,%3,%12;\n\t"
       "addc.cc.u32 %4,%4,%13;\n\taddc.cc.u32 %5,%5,%14;\n\taddc.cc.u32 %6,%6,%15;\n\taddc.cc.u32 %7,%7,%16;\n\t"
       "addc.u32 %8,%8,0;"
       : "+r"(S[1]), "+r"(S[2]), "+r"(S[3]), "+r"(S[4]), "+r"(S[5]), "+r"(S[6]), "+r"(S[7]), "+r"(s8), "+r"(s9)
       : "r"(R[8]), "r"(R[9]), "r"(R[10]), "r"(R[11]), "r"(R[12]), "r"(R[13]), "r"(R[14]), "r"(R[15]));
+#else
+  // S = L + H*977 + (H << 32) in two accumulators whose 64-bit addends are exactly the limb pairs the product leaves behind,
+  // (L0,L1), (L2,L3), ... and (H0,H1), (H2,H3), ..., so that no limb is re-paired (copied) between chains:
+  //   even: (L0,L1) += H0*977, (L2,L3) += H2*977, ...   limbs 0..7, carry -> e8
+  //   odd:  (H0,H1) += H1*977, (H2,H3) += H3*977, ...   limbs 1..8, carry -> o9
+  // and one add chain S = even + (odd << 32).  Each accumulator is < 978 * 2^256, so s9:s8 < 2^34 as before.
+  uint32_t e0 = R[0], e1 = R[1], e2 = R[2], e3 = R[3], e4 = R[4], e5 = R[5], e6 = R[6], e7 = R[7], e8;
+  uint32_t o1 = R[8], o2 = R[9], o3 = R[10], o4 = R[11], o5 = R[12], o6 = R[13], o7 = R[14], o8 = R[15], o9;
+  e8 = mad_chain4(e0, e1, e2, e3, e4, e5, e6, e7, R[8], R[10], R[12], R[14], IBFT_PC);
+  o9 = mad_chain4(o1, o2, o3, o4, o5, o6, o7, o8, R[9], R[11], R[13], R[15], IBFT_PC);
+  S[0] = e0;
+  asm("add.cc.u32 %0,%9,%17;\n\taddc.cc.u32 %1,%10,%18;\n\taddc.cc.u32 %2,%11,%19;\n\taddc.cc.u32 %3,%12,%20;\n\t"
+      "addc.cc.u32 %4,%13,%21;\n\taddc.cc.u32 %5,%14,%22;\n\taddc.cc.u32 %6,%15,%23;\n\taddc.cc.u32 %7,%16,%24;\n\t"
+      "addc.u32 %8,%25,0;"
+      : "=r"(S[1]), "=r"(S[2]), "=r"(S[3]), "=r"(S[4]), "=r"(S[5]), "=r"(S[6]), "=r"(S[7]), "=r"(s8), "=r"(s9)
+      : "r"(e1), "r"(e2), "r"(e3), "r"(e4), "r"(e5), "r"(e6), "r"(e7), "r"(e8), "r"(o1), "r"(o2), "r"(o3), "r"(o4), "r"(o5),
+        "r"(o6), "r"(o7), "r"(o8), "r"(o9));
+#endif
   // e = s9:s8 (< 2^34); g = e * (2^32 + 977) (< 2^67) as three limbs
   uint64_t m = (uint64_t)s8 * IBFT_PC + (((uint64_t)(s9 * IBFT_PC)) << 32);
   uint64_t mid = (m >> 32) + s8;
@@ -589,6 +618,7 @@ IBFT_HD fe fe_reduce512(const uint32_t* R) {
 
 // always-inline body (used inside the out-of-line point routines) and the out-of-line entry point (everything else)
 IBFT_HD fe fe_mul_i(const fe& a, const fe& b) {
+  IBFT_OPCOUNT(IBFT_OP_MUL_BODY);
   uint32_t R[16];
   mul_wide_8x8(R, a.v, b.v);
   return fe_reduce512(R);
@@ -617,85 +647,80 @@ __device__ __forceinline__ fe fe_mul(const fe& a, const fe& b) {
 #endif
 }
 #else
-IBFT_FN fe fe_mul(fe a, fe b) { return fe_mul_i(a, b); }
+IBFT_FN fe fe_mul(fe a, fe b) {
+  IBFT_OPCOUNT(IBFT_OP_MUL_CALL);
+  return fe_mul_i(a, b);
+}
 #endif
 
 #if IBFT_PTX
-// shorter carry chains for the squaring triangle
-__device__ __forceinline__ uint32_t mad_chain3(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t& p4,
-                                               uint32_t& p5, uint32_t x0, uint32_t x1, uint32_t x2, uint32_t y) {
-  uint32_t co;
-  asm("mad.lo.cc.u32 %0,%7,%10,%0;\n\tmadc.hi.cc.u32 %1,%7,%10,%1;\n\t"
-      "madc.lo.cc.u32 %2,%8,%10,%2;\n\tmadc.hi.cc.u32 %3,%8,%10,%3;\n\t"
-      "madc.lo.cc.u32 %4,%9,%10,%4;\n\tmadc.hi.cc.u32 %5,%9,%10,%5;\n\t"
-      "addc.u32 %6,0,0;"
-      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "+r"(p4), "+r"(p5), "=r"(co)
-      : "r"(x0), "r"(x1), "r"(x2), "r"(y));
-  return co;
-}
-__device__ __forceinline__ void mad_chain3_nc(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t& p4,
-                                              uint32_t& p5, uint32_t x0, uint32_t x1, uint32_t x2, uint32_t y) {
+// shorter carry chains for the squaring triangle, in the two shapes of mul_wide_8x8: "_nczz" writes its top pair fresh
+// (literal-zero addends), "_r2" ripples its carry out into the pair above it, which a later row has already written
+__device__ __forceinline__ void mad_chain3_nczz(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t& p4_out,
+                                                uint32_t& p5_out, uint32_t x0, uint32_t x1, uint32_t x2, uint32_t y) {
   asm("mad.lo.cc.u32 %0,%6,%9,%0;\n\tmadc.hi.cc.u32 %1,%6,%9,%1;\n\t"
       "madc.lo.cc.u32 %2,%7,%9,%2;\n\tmadc.hi.cc.u32 %3,%7,%9,%3;\n\t"
-      "madc.lo.cc.u32 %4,%8,%9,%4;\n\tmadc.hi.u32 %5,%8,%9,%5;"
-      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "+r"(p4), "+r"(p5)
+      "madc.lo.cc.u32 %4,%8,%9,0;\n\tmadc.hi.u32 %5,%8,%9,0;"
+      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "=r"(p4_out), "=r"(p5_out)
       : "r"(x0), "r"(x1), "r"(x2), "r"(y));
 }
-__device__ __forceinline__ uint32_t mad_chain2(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t x0,
-                                               uint32_t x1, uint32_t y) {
-  uint32_t co;
-  asm("mad.lo.cc.u32 %0,%5,%7,%0;\n\tmadc.hi.cc.u32 %1,%5,%7,%1;\n\t"
-      "madc.lo.cc.u32 %2,%6,%7,%2;\n\tmadc.hi.cc.u32 %3,%6,%7,%3;\n\t"
-      "addc.u32 %4,0,0;"
-      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "=r"(co)
-      : "r"(x0), "r"(x1), "r"(y));
-  return co;
+__device__ __forceinline__ void mad_chain3_r2(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t& p4, uint32_t& p5,
+                                              uint32_t& p6, uint32_t& p7, uint32_t x0, uint32_t x1, uint32_t x2, uint32_t y) {
+  asm("mad.lo.cc.u32 %0,%8,%11,%0;\n\tmadc.hi.cc.u32 %1,%8,%11,%1;\n\t"
+      "madc.lo.cc.u32 %2,%9,%11,%2;\n\tmadc.hi.cc.u32 %3,%9,%11,%3;\n\t"
+      "madc.lo.cc.u32 %4,%10,%11,%4;\n\tmadc.hi.cc.u32 %5,%10,%11,%5;\n\t"
+      "addc.cc.u32 %6,%6,0;\n\taddc.u32 %7,%7,0;"
+      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "+r"(p4), "+r"(p5), "+r"(p6), "+r"(p7)
+      : "r"(x0), "r"(x1), "r"(x2), "r"(y));
 }
-__device__ __forceinline__ void mad_chain2_nc(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t x0,
-                                              uint32_t x1, uint32_t y) {
+__device__ __forceinline__ void mad_chain2_nczz(uint32_t& p0, uint32_t& p1, uint32_t& p2_out, uint32_t& p3_out, uint32_t x0,
+                                                uint32_t x1, uint32_t y) {
   asm("mad.lo.cc.u32 %0,%4,%6,%0;\n\tmadc.hi.cc.u32 %1,%4,%6,%1;\n\t"
-      "madc.lo.cc.u32 %2,%5,%6,%2;\n\tmadc.hi.u32 %3,%5,%6,%3;"
-      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3)
+      "madc.lo.cc.u32 %2,%5,%6,0;\n\tmadc.hi.u32 %3,%5,%6,0;"
+      : "+r"(p0), "+r"(p1), "=r"(p2_out), "=r"(p3_out)
       : "r"(x0), "r"(x1), "r"(y));
 }
-__device__ __forceinline__ uint32_t mad_chain1(uint32_t& p0, uint32_t& p1, uint32_t x0, uint32_t y) {
-  uint32_t co;
-  asm("mad.lo.cc.u32 %0,%3,%4,%0;\n\tmadc.hi.cc.u32 %1,%3,%4,%1;\n\taddc.u32 %2,0,0;"
-      : "+r"(p0), "+r"(p1), "=r"(co)
-      : "r"(x0), "r"(y));
-  return co;
+__device__ __forceinline__ void mad_chain2_r2(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t& p4, uint32_t& p5,
+                                              uint32_t x0, uint32_t x1, uint32_t y) {
+  asm("mad.lo.cc.u32 %0,%6,%8,%0;\n\tmadc.hi.cc.u32 %1,%6,%8,%1;\n\t"
+      "madc.lo.cc.u32 %2,%7,%8,%2;\n\tmadc.hi.cc.u32 %3,%7,%8,%3;\n\t"
+      "addc.cc.u32 %4,%4,0;\n\taddc.u32 %5,%5,0;"
+      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3), "+r"(p4), "+r"(p5)
+      : "r"(x0), "r"(x1), "r"(y));
 }
-__device__ __forceinline__ void mad_chain1_nc(uint32_t& p0, uint32_t& p1, uint32_t x0, uint32_t y) {
-  asm("mad.lo.cc.u32 %0,%2,%3,%0;\n\tmadc.hi.u32 %1,%2,%3,%1;" : "+r"(p0), "+r"(p1) : "r"(x0), "r"(y));
+__device__ __forceinline__ void mad_chain1_r2(uint32_t& p0, uint32_t& p1, uint32_t& p2, uint32_t& p3, uint32_t x0, uint32_t y) {
+  asm("mad.lo.cc.u32 %0,%4,%5,%0;\n\tmadc.hi.cc.u32 %1,%4,%5,%1;\n\taddc.cc.u32 %2,%2,0;\n\taddc.u32 %3,%3,0;"
+      : "+r"(p0), "+r"(p1), "+r"(p2), "+r"(p3)
+      : "r"(x0), "r"(y));
 }
 #endif
 
 // R[0..15] = a^2 : 28 off-diagonal wide MACs (E/O carry chains, as in mul_wide_8x8), doubled, + 8 diagonal MACs
 IBFT_HD void sqr_wide_8(uint32_t* R, const uint32_t* a) {
 #if IBFT_PTX && !defined(IBFT_SQR_VIA_MUL)
+  // Same row pairing as mul_wide_8x8: the later row of each pair writes the top pair fresh, the earlier one ripples into it.
   uint32_t E[14], O[14];
-#pragma unroll
-  for (int i = 0; i < 14; i++) { E[i] = 0; O[i] = 0; }
+  E[0] = 0; E[1] = 0;
   // row 0
   mulw(E[2], E[3], a[2], a[0]); mulw(E[4], E[5], a[4], a[0]); mulw(E[6], E[7], a[6], a[0]);
   mulw(O[0], O[1], a[1], a[0]); mulw(O[2], O[3], a[3], a[0]); mulw(O[4], O[5], a[5], a[0]); mulw(O[6], O[7], a[7], a[0]);
-  // row 1
-  O[8] = mad_chain3(O[2], O[3], O[4], O[5], O[6], O[7], a[2], a[4], a[6], a[1]);
-  mad_chain3_nc(E[4], E[5], E[6], E[7], E[8], E[9], a[3], a[5], a[7], a[1]);
-  // row 2
-  E[10] = mad_chain2(E[6], E[7], E[8], E[9], a[4], a[6], a[2]);
-  mad_chain3_nc(O[4], O[5], O[6], O[7], O[8], O[9], a[3], a[5], a[7], a[2]);
-  // row 3
-  O[10] = mad_chain2(O[6], O[7], O[8], O[9], a[4], a[6], a[3]);
-  mad_chain2_nc(E[8], E[9], E[10], E[11], a[5], a[7], a[3]);
-  // row 4
-  E[12] = mad_chain1(E[10], E[11], a[6], a[4]);
-  mad_chain2_nc(O[8], O[9], O[10], O[11], a[5], a[7], a[4]);
-  // row 5
-  O[12] = mad_chain1(O[10], O[11], a[6], a[5]);
-  mad_chain1_nc(E[12], E[13], a[7], a[5]);
-  // row 6
-  mad_chain1_nc(O[12], O[13], a[7], a[6]);
+  // row 1, E: (E[8], E[9]) fresh
+  mad_chain3_nczz(E[4], E[5], E[6], E[7], E[8], E[9], a[3], a[5], a[7], a[1]);
+  // rows 2 then 1, O: (O[8], O[9])
+  mad_chain3_nczz(O[4], O[5], O[6], O[7], O[8], O[9], a[3], a[5], a[7], a[2]);
+  mad_chain3_r2(O[2], O[3], O[4], O[5], O[6], O[7], O[8], O[9], a[2], a[4], a[6], a[1]);
+  // rows 3 then 2, E: (E[10], E[11])
+  mad_chain2_nczz(E[8], E[9], E[10], E[11], a[5], a[7], a[3]);
+  mad_chain2_r2(E[6], E[7], E[8], E[9], E[10], E[11], a[4], a[6], a[2]);
+  // rows 4 then 3, O: (O[10], O[11])
+  mad_chain2_nczz(O[8], O[9], O[10], O[11], a[5], a[7], a[4]);
+  mad_chain2_r2(O[6], O[7], O[8], O[9], O[10], O[11], a[4], a[6], a[3]);
+  // rows 5 then 4, E: (E[12], E[13])
+  mulw(E[12], E[13], a[7], a[5]);
+  mad_chain1_r2(E[10], E[11], E[12], E[13], a[6], a[4]);
+  // rows 6 then 5, O: (O[12], O[13])
+  mulw(O[12], O[13], a[7], a[6]);
+  mad_chain1_r2(O[10], O[11], O[12], O[13], a[6], a[5]);
   // T = E + (O << 32)   (T[0] = 0, T[15] = 0)
   uint32_t T[16];
   T[0] = 0;
@@ -735,6 +760,7 @@ IBFT_HD void sqr_wide_8(uint32_t* R, const uint32_t* a) {
 }
 
 IBFT_HD fe fe_sqr_i(const fe& a) {
+  IBFT_OPCOUNT(IBFT_OP_SQR_BODY);
   uint32_t R[16];
   sqr_wide_8(R, a.v);
   return fe_reduce512(R);
@@ -749,15 +775,22 @@ __device__ __forceinline__ fe fe_sqr(const fe& a) {
 #endif
 }
 #else
-IBFT_FN fe fe_sqr(fe a) { return fe_sqr_i(a); }
+IBFT_FN fe fe_sqr(fe a) {
+  IBFT_OPCOUNT(IBFT_OP_SQR_CALL);
+  return fe_sqr_i(a);
+}
 #endif
 
 // a^(2^n): out of line, with the squarer inlined in the loop (no per-iteration call marshalling)
 IBFT_FN fe fe_sqrn(fe a, int n) {
+  IBFT_OPCOUNT(IBFT_OP_SQRN_CALL);
 #if IBFT_PTX
 #pragma unroll 1
 #endif
-  for (int i = 0; i < n; i++) a = fe_sqr_i(a);
+  for (int i = 0; i < n; i++) {
+    IBFT_OPCOUNT(IBFT_OP_SQRN_ITER);
+    a = fe_sqr_i(a);
+  }
   return a;
 }
 

@@ -214,6 +214,7 @@ IBFT_HD void modinv30_var(uint32_t* out8, const uint32_t* x8, const modinfo30& m
 #pragma unroll 1
 #endif
   for (int it = 0; it < 40; it++) {  // 25 iterations suffice for 256-bit inputs; the bound only guards against misuse
+    IBFT_OPCOUNT(IBFT_OP_INV_ITER);
     trans2x2 t;
     eta = divsteps_30_var(eta, (uint32_t)f.v[0], (uint32_t)g.v[0], t);
     update_de_30(d, e, t, mi);
@@ -230,11 +231,13 @@ IBFT_HD void modinv30_var(uint32_t* out8, const uint32_t* x8, const modinfo30& m
 }
 
 IBFT_FN fe fe_inv_safegcd(fe a) {
+  IBFT_OPCOUNT(IBFT_OP_FE_INV);
   fe n = fe_normalize(a), r;
   modinv30_var(r.v, n.v, modinfo_p());
   return r;
 }
 IBFT_FN sc sc_inv_safegcd(sc a) {  // a in [0, n)
+  IBFT_OPCOUNT(IBFT_OP_SC_INV);
   sc r;
   modinv30_var(r.v, a.v, modinfo_n());
   return r;
