@@ -5,8 +5,9 @@
 //                    derivation + compare with msg.From / seal.Signer, validator-set membership, warp-ballot of the
 //                    32 verdicts of a warp into one word of the pass/fail bitmap.
 //   k_quorum_mark /  K3: resolve every passing item's signer to its validator index and OR it into the group's voted
-//   k_quorum_reduce  set; then per group: distinct count, 320-bit weighted voting-power sum, >= quorum threshold
-//                    (reference core/validator_manager.go:77-96, :130-135).
+//   k_quorum_reduce  set; then per group: distinct count, 320-bit weighted voting-power sum, and the decision of the group's
+//                    quorum rule: HasQuorum, HasPrepareQuorum or "one valid PREPREPARE" (reference core/ibft.go:1273-1284,
+//                    core/validator_manager.go:77-135).
 //   k_keccak_batch   hash-only batch for IsValidProposalHash (reference core/backend.go:50-51).
 // There is no CPU fallback anywhere in this file: without a CUDA device ibft_engine_create fails.
 #include <cuda_runtime.h>
@@ -1179,7 +1180,40 @@ __global__ void k_quorum_exchange(peer_bufs peers, uint32_t world, uint32_t rank
   }
 }
 
-// one CTA per group: 320-bit sum of the voting power of the voted validators, compared with the threshold
+// The group's decision (hasQuorumByMsgType, reference core/ibft.go:1273-1284) from what the CTA that summed the group's power
+// holds: the quorum rule and proposer of the descriptor, the voted set, the summed power (updated in place: under the PREPARE
+// rule the proposer's power joins the sum), the valid count and the slot's threshold.  Rule 0 is HasQuorum.
+__device__ __forceinline__ uint32_t group_decision(uint32_t rule, uint32_t proposer, const uint32_t* __restrict__ voted,
+                                                   const slot_dev& s, uint32_t n_valid, uint64_t power[5]) {
+  if (rule == IBFT_QUORUM_PREPREPARE) return n_valid >= 1 ? 1u : 0u;  // len(msgs) >= 1
+  if (rule == IBFT_QUORUM_PREPARE) {                                    // HasPrepareQuorum (validator_manager.go:99-127)
+    if (proposer == IBFT_PROPOSER_UNSET) return 0u;                     // no proposal message
+    if (proposer != IBFT_PROPOSER_NONE) {
+      if (proposer >= s.n) return 0u;                                   // table replaced since the groups were planned: no verdict
+      if ((voted[proposer >> 5] >> (proposer & 31)) & 1u) return 0u;    // the proposer is among the senders
+      const uint64_t* p = s.powers + 4 * (size_t)proposer;              // the proposer joins the sender set
+      unsigned long long c = 0;
+#pragma unroll
+      for (int k = 0; k < 5; k++) {
+        unsigned long long add = k < 4 ? p[k] : 0ull;
+        unsigned long long t = power[k] + add;
+        unsigned long long c1 = t < add;
+        unsigned long long t2 = t + c;
+        c1 += t2 < c;
+        power[k] = t2;
+        c = c1;
+      }
+    }
+  }
+  int cmp = 0;  // power >= quorum ?
+  for (int k = 4; k >= 0; k--) {
+    uint64_t q = s.quorum[k];
+    if (cmp == 0 && power[k] != q) cmp = power[k] < q ? -1 : 1;
+  }
+  return cmp >= 0 ? 1u : 0u;
+}
+
+// one CTA per group: 320-bit sum of the voting power of the voted validators, then the group's decision (group_decision)
 #define IBFT_REDUCE_THREADS 1024  // one CTA per group; a 10k-validator set is 10 strided passes instead of 40
 __global__ void __launch_bounds__(IBFT_REDUCE_THREADS)
 k_quorum_reduce(const ibft_group_desc* __restrict__ groups, const group_dev* __restrict__ gdev, uint32_t n_groups,
@@ -1243,15 +1277,9 @@ k_quorum_reduce(const ibft_group_desc* __restrict__ groups, const group_dev* __r
     r.n_distinct = s_cnt[0];
     r.has_quorum = 0;
     r.reserved = 0;
-    if (has_table) {
-      // power >= quorum ?
-      int cmp = 0;
-      for (int k = 4; k >= 0; k--) {
-        uint64_t q = slots[slot].quorum[k];
-        if (cmp == 0 && r.power[k] != q) cmp = r.power[k] < q ? -1 : 1;
-      }
-      r.has_quorum = cmp >= 0 ? 1u : 0u;
-    }
+    if (has_table)
+      r.has_quorum = group_decision(groups[g].flags & IBFT_QUORUM_RULE_MASK, groups[g].reserved, voted + gdev[g].voted_off, slots[slot],
+                                    r.n_valid, r.power);
     results[g] = r;
   }
 }
@@ -2118,11 +2146,17 @@ extern "C" int ibft_get_quorum(ibft_engine* e, uint32_t table_slot, uint64_t quo
   return IBFT_OK;
 }
 
-// lay out the voted sets of the call's groups; validates table slots
+// lay out the voted sets of the call's groups; validates table slots and quorum rules (IBFT_QUORUM_*)
 static int plan_groups(ibft_engine* e, lane* L, const ibft_group_desc* groups, uint32_t n_groups, group_dev* gdev, size_t* total_words) {
   size_t off = 0;
   for (uint32_t g = 0; g < n_groups; g++) {
     uint32_t slot = groups[g].table_slot;
+    const uint32_t rule = groups[g].flags & IBFT_QUORUM_RULE_MASK, proposer = groups[g].reserved;
+    if (rule == 3u) { set_err("group %u: quorum rule 3 is reserved", g); return IBFT_ERR_INVALID_ARG; }
+    if (rule != IBFT_QUORUM_DEFAULT && slot == IBFT_NO_TABLE) {
+      set_err("group %u: quorum rule %u needs a validator table", g, rule);
+      return IBFT_ERR_INVALID_ARG;
+    }
     uint32_t nw = 0;
     if (slot != IBFT_NO_TABLE) {
       if (slot >= e->p.max_table_slots || !e->slots[slot].valid) {
@@ -2135,6 +2169,10 @@ static int plan_groups(ibft_engine* e, lane* L, const ibft_group_desc* groups, u
         set_err("group %u is for height %llu but validator-table slot %u holds height %llu", g, (unsigned long long)groups[g].height,
                 slot, (unsigned long long)e->slots[slot].height);
         return IBFT_ERR_NO_TABLE;
+      }
+      if (rule == IBFT_QUORUM_PREPARE && proposer != IBFT_PROPOSER_NONE && proposer != IBFT_PROPOSER_UNSET && proposer >= e->slots[slot].n) {
+        set_err("group %u: proposer index %u is outside the %u-validator table of slot %u", g, proposer, e->slots[slot].n, slot);
+        return IBFT_ERR_INVALID_ARG;
       }
       nw = (e->slots[slot].n + 31) / 32;
     }

@@ -17,6 +17,9 @@ IBFT_OK, ERR_INVALID_ARG, ERR_NO_DEVICE, ERR_CUDA, ERR_CAPACITY, ERR_VOTING_POWE
 KIND_DIGEST, KIND_PAYLOAD, KIND_SEAL, KIND_WIRE, KIND_WIRE_SEAL, KIND_PAYLOAD2, KIND_INVALID = 0, 1, 2, 3, 4, 5, 255
 ITEM_OK, ITEM_NEEDS_HOST = 0, 1
 NO_TABLE = 0xFFFF
+# quorum rule of a group (ibft_group_desc.flags bits 0-1) and the proposer markers of the PREPARE rule (ibft_group_desc.reserved)
+QUORUM_DEFAULT, QUORUM_PREPREPARE, QUORUM_PREPARE = 0, 1, 2
+PROPOSER_NONE, PROPOSER_UNSET = 0xFFFFFFFF, 0xFFFFFFFE
 DBG = dict(FE_MUL=1, FE_SQR=2, FE_INV=3, FE_SQRT=4, SC_MUL=5, SC_INV=6, ECMULT=7, FE_ADD=8, FE_SUB=9, GLV=10)
 
 # numpy mirrors of the ABI structs
@@ -115,6 +118,24 @@ def _ptr(a: np.ndarray | None):
     return None if a is None else a.ctypes.data_as(c_void_p)
 
 
+def group_descs(n_groups: int, slot=0, rule=QUORUM_DEFAULT, proposer=0, slot_height: dict | None = None) -> np.ndarray:
+    """n ibft_group_desc records.  `slot`, `rule` (QUORUM_*) and `proposer` are each one value for all groups or a sequence of
+    n.  The proposer (its index in the slot's validator table, or PROPOSER_NONE / PROPOSER_UNSET) is stored only for
+    QUORUM_PREPARE groups.  `height` is slot_height[slot] (0 for NO_TABLE groups and unknown slots)."""
+    g = np.zeros(n_groups, dtype=GROUP_DTYPE)
+    per_group = lambda v: [v] * n_groups if np.isscalar(v) else list(v)  # noqa: E731
+    slots, rules, proposers = per_group(slot), per_group(rule), per_group(proposer)
+    if not len(slots) == len(rules) == len(proposers) == n_groups:
+        raise ValueError("slot, rule and proposer need one value or one per group")
+    heights = slot_height or {}
+    for i, (sl, ru, pr) in enumerate(zip(slots, rules, proposers)):
+        g[i]["table_slot"] = sl
+        g[i]["height"] = heights.get(int(sl), 0) if sl != NO_TABLE else 0
+        g[i]["flags"] = ru
+        g[i]["reserved"] = pr if ru == QUORUM_PREPARE else 0
+    return g
+
+
 class Engine:
     """One engine per process per GPU (one process per GPU is the deployment model)."""
 
@@ -181,15 +202,11 @@ class Engine:
                                                  _ptr(powers_be), len(addrs)))
         self.slot_height[slot] = height
 
-    def groups(self, n_groups: int, slot=0) -> np.ndarray:
+    def groups(self, n_groups: int, slot=0, rule=QUORUM_DEFAULT, proposer=0) -> np.ndarray:
         """n group descriptors; `slot` is one slot for all groups or a sequence of slots.  Each group carries the height of the
-        table resident in its slot (ibft_group_desc.height: a group for another height is refused with ERR_NO_TABLE)."""
-        g = np.zeros(n_groups, dtype=GROUP_DTYPE)
-        slots = [slot] * n_groups if np.isscalar(slot) else list(slot)
-        for i, sl in enumerate(slots):
-            g[i]["table_slot"] = sl
-            g[i]["height"] = self.slot_height.get(int(sl), 0) if sl != NO_TABLE else 0
-        return g
+        table resident in its slot (ibft_group_desc.height: a group for another height is refused with ERR_NO_TABLE).
+        `rule` and `proposer`: see group_descs."""
+        return group_descs(n_groups, slot, rule, proposer, self.slot_height)
 
     def get_quorum(self, slot: int):
         q = (c_uint64 * 5)()

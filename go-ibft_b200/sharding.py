@@ -100,6 +100,9 @@ class ShardedVerifier:
 
         sv = ShardedVerifier(engine, n_global, groups, world, rank, local_items, local_arena)
         results, bitmap = sv.run()        # host arrays, identical on every rank
+
+    The descriptors are bound as given, quorum rule and proposer included (Engine.groups(..., rule=, proposer=)): both exchanges
+    return go-ibft's per-message-type decision (HasPrepareQuorum for PREPARE groups, one valid message for PREPREPARE groups).
     """
 
     def __init__(self, engine, n_global: int, groups: np.ndarray, world: int, rank: int, local_items: np.ndarray,

@@ -126,6 +126,28 @@ type Item struct {
 	Hash    []byte // KIND_SEAL: proposal hash
 	Payload []byte // KIND_PAYLOAD: IbftMessage.PayloadNoSig() (messages/proto/helper.go:13-27)
 	Height  uint64
+	Group   uint16 // VerifyGroups only: index into its groups (VerifyBatch groups items by Height)
+}
+
+// packItem marshals one item into its packed tuple (payload bytes appended to *arena); false for a malformed item, which is
+// packed as IBFT_KIND_INVALID.
+func packItem(p *C.ibft_sig_item, it Item, arena *[]byte) bool {
+	if len(it.Sig) != 65 || len(it.Signer) != 20 || (it.Kind == C.IBFT_KIND_SEAL && len(it.Hash) != 32) {
+		p.kind = C.IBFT_KIND_INVALID // malformed => false (messages/helpers.go:38-42 nil seal etc.)
+		return false
+	}
+	C.memcpy(unsafe.Pointer(&p.r[0]), unsafe.Pointer(&it.Sig[0]), 32)
+	C.memcpy(unsafe.Pointer(&p.s[0]), unsafe.Pointer(&it.Sig[32]), 32)
+	p.v = C.uint8_t(it.Sig[64])
+	C.memcpy(unsafe.Pointer(&p.signer[0]), unsafe.Pointer(&it.Signer[0]), 20)
+	p.kind = C.uint8_t(it.Kind)
+	if it.Kind == C.IBFT_KIND_SEAL {
+		C.memcpy(unsafe.Pointer(&p.digest[0]), unsafe.Pointer(&it.Hash[0]), 32)
+	} else {
+		p.payload_off, p.payload_len = C.uint32_t(len(*arena)), C.uint32_t(len(it.Payload))
+		*arena = append(*arena, it.Payload...)
+	}
+	return true
 }
 
 // VerifyBatch runs ONE device call for all items and returns one verdict per item.  A failed launch returns an error and
@@ -144,8 +166,7 @@ func (e *Engine) VerifyBatch(items []Item) ([]bool, error) {
 	e.mu.RLock()
 	for i, it := range items {
 		p := &packed[i]
-		if len(it.Sig) != 65 || len(it.Signer) != 20 || (it.Kind == C.IBFT_KIND_SEAL && len(it.Hash) != 32) {
-			p.kind = C.IBFT_KIND_INVALID // malformed => false (messages/helpers.go:38-42 nil seal etc.)
+		if !packItem(p, it, &arena) {
 			continue
 		}
 		g, ok := groupOf[it.Height]
@@ -162,18 +183,7 @@ func (e *Engine) VerifyBatch(items []Item) ([]bool, error) {
 			}
 			groups = append(groups, d)
 		}
-		C.memcpy(unsafe.Pointer(&p.r[0]), unsafe.Pointer(&it.Sig[0]), 32)
-		C.memcpy(unsafe.Pointer(&p.s[0]), unsafe.Pointer(&it.Sig[32]), 32)
-		p.v = C.uint8_t(it.Sig[64])
-		C.memcpy(unsafe.Pointer(&p.signer[0]), unsafe.Pointer(&it.Signer[0]), 20)
-		p.kind = C.uint8_t(it.Kind)
 		p.group = C.uint16_t(g)
-		if it.Kind == C.IBFT_KIND_SEAL {
-			C.memcpy(unsafe.Pointer(&p.digest[0]), unsafe.Pointer(&it.Hash[0]), 32)
-		} else {
-			p.payload_off, p.payload_len = C.uint32_t(len(arena)), C.uint32_t(len(it.Payload))
-			arena = append(arena, it.Payload...)
-		}
 	}
 	e.mu.RUnlock()
 	bitmap := make([]uint32, (n+31)/32)
@@ -197,6 +207,88 @@ func (e *Engine) VerifyBatch(items []Item) ([]bool, error) {
 		out[i] = bitmap[i/32]>>(uint(i)%32)&1 == 1 && !noTable[uint16(packed[i].group)]
 	}
 	return out, nil
+}
+
+// Quorum rules of a Group (include/ibft_verify.h IBFT_QUORUM_*): which of go-ibft's per-message-type decisions
+// (hasQuorumByMsgType, core/ibft.go:1273-1284) the engine returns as the group's HasQuorum.
+const (
+	QuorumDefault    = uint16(C.IBFT_QUORUM_DEFAULT)    // HasQuorum: COMMIT, ROUND_CHANGE, validPC's PREPREPARE + PREPARE senders
+	QuorumPrePrepare = uint16(C.IBFT_QUORUM_PREPREPARE) // at least one valid message
+	QuorumPrepare    = uint16(C.IBFT_QUORUM_PREPARE)    // HasPrepareQuorum (core/validator_manager.go:99-127); needs Proposer
+	ProposerNone     = uint32(C.IBFT_PROPOSER_NONE)     // the proposer is not a validator of the group's table
+	ProposerUnset    = uint32(C.IBFT_PROPOSER_UNSET)    // there is no proposal message: HasQuorum is false
+)
+
+// Group is one quorum domain of VerifyGroups: the items of one (height, round, message type).
+type Group struct {
+	Height uint64
+	Rule   uint16 // QuorumDefault, QuorumPrePrepare or QuorumPrepare
+	// QuorumPrepare: the proposer's index in the validator table of Height (the order given to SetValidators, without the
+	// entries it skipped), ProposerNone or ProposerUnset.  The caller decides who the proposer is (IsProposer).
+	Proposer uint32
+}
+
+// GroupResult is the engine's quorum result of one Group (ibft_group_result).
+type GroupResult struct {
+	HasQuorum         bool
+	NValid, NDistinct uint32
+	Power             *big.Int // voting power of the distinct valid senders; under QuorumPrepare the proposer's is included
+}
+
+// VerifyGroups runs ONE device call for all items, each in groups[item.Group], and returns the verdicts and every group's
+// quorum decision under its rule.  A group whose height has no resident validator table fails the call (IBFT_ERR_NO_TABLE).
+func (e *Engine) VerifyGroups(items []Item, groups []Group) ([]bool, []GroupResult, error) {
+	n := len(items)
+	if n == 0 || len(groups) == 0 {
+		return nil, nil, errors.New("VerifyGroups needs items and groups")
+	}
+	descs := make([]C.ibft_group_desc, len(groups))
+	e.mu.RLock()
+	for g, gr := range groups {
+		slot := uint32(gr.Height % uint64(e.params.max_table_slots))
+		if h, set := e.slotHeight[slot]; !set || h != gr.Height {
+			e.mu.RUnlock()
+			return nil, nil, fmt.Errorf("group %d: no validator table for height %d", g, gr.Height)
+		}
+		descs[g] = C.ibft_group_desc{table_slot: C.uint16_t(slot), flags: C.uint16_t(gr.Rule), height: C.uint64_t(gr.Height)}
+		if gr.Rule == QuorumPrepare {
+			descs[g].reserved = C.uint32_t(gr.Proposer)
+		}
+	}
+	e.mu.RUnlock()
+	packed := make([]C.ibft_sig_item, n)
+	var arena []byte
+	for i, it := range items {
+		if int(it.Group) >= len(groups) {
+			return nil, nil, fmt.Errorf("item %d: group %d out of range", i, it.Group)
+		}
+		packed[i].group = C.uint16_t(it.Group)
+		packItem(&packed[i], it, &arena)
+	}
+	bitmap := make([]uint32, (n+31)/32)
+	results := make([]C.ibft_group_result, len(groups))
+	var ap *C.uint8_t
+	if len(arena) > 0 {
+		ap = (*C.uint8_t)(unsafe.Pointer(&arena[0]))
+	}
+	rc := C.ibft_verify_batch_ex(e.h, &packed[0], C.uint32_t(n), ap, C.size_t(len(arena)), &descs[0], C.uint32_t(len(descs)),
+		(*C.uint32_t)(unsafe.Pointer(&bitmap[0])), &results[0], nil, nil, nil, 0)
+	if rc != C.IBFT_OK {
+		return nil, nil, fmt.Errorf("ibft_verify_batch_ex: %w", lastError())
+	}
+	out := make([]bool, n)
+	for i := range out {
+		out[i] = bitmap[i/32]>>(uint(i)%32)&1 == 1
+	}
+	res := make([]GroupResult, len(groups))
+	for g, r := range results {
+		p := new(big.Int)
+		for k := 4; k >= 0; k-- {
+			p.Lsh(p, 64).Or(p, new(big.Int).SetUint64(uint64(r.power[k])))
+		}
+		res[g] = GroupResult{HasQuorum: r.has_quorum != 0, NValid: uint32(r.n_valid), NDistinct: uint32(r.n_distinct), Power: p}
+	}
+	return out, res, nil
 }
 
 // ProposalHash = Keccak-256(Keccak-256(raw) || u64_be(round)), both sponges in one device launch (IsValidProposalHash,

@@ -86,15 +86,42 @@ typedef struct ibft_sig_item {
  * answered from the wrong validator set. */
 typedef struct ibft_group_desc {
   uint16_t table_slot; /* slot given to ibft_set_validators, or IBFT_NO_TABLE */
-  uint16_t flags;      /* reserved, 0 */
-  uint32_t reserved;   /* 0 */
+  uint16_t flags;      /* bits 0-1: quorum rule (IBFT_QUORUM_*); bits 2-15 reserved, ignored */
+  uint32_t reserved;   /* IBFT_QUORUM_PREPARE: the proposer (see below); ignored under the other rules */
   uint64_t height;     /* height of the group's messages; must equal the height the slot was set with (ignored for IBFT_NO_TABLE) */
 } ibft_group_desc;     /* sizeof == 16 */
 
+/* Quorum rule of a group: ibft_group_desc.flags & IBFT_QUORUM_RULE_MASK.  go-ibft decides quorum per message type
+ * (hasQuorumByMsgType, core/ibft.go:1273-1284); the rule tells every reduce path which decision a group's has_quorum is.
+ *   IBFT_QUORUM_DEFAULT    HasQuorum over the senders' address set (core/validator_manager.go:77-96): COMMIT, ROUND_CHANGE,
+ *                          and the PREPREPARE + PREPARE sender set of validPC (core/ibft.go:1162-1231).
+ *   IBFT_QUORUM_PREPREPARE has_quorum = n_valid >= 1 (len(msgs) >= 1).
+ *   IBFT_QUORUM_PREPARE    HasPrepareQuorum (core/validator_manager.go:99-127).  ibft_group_desc.reserved = the proposer's
+ *                          index in the slot's validator table, or
+ *                            IBFT_PROPOSER_NONE   the proposer is not a validator of this table: it adds no power (and can
+ *                                                 never be among the valid senders);
+ *                            IBFT_PROPOSER_UNSET  there is no proposal message: has_quorum = 0.
+ *                          The proposer is added to the sender set: power = the voted validators' power plus the proposer's
+ *                          when it is a validator outside the voted set (the sum HasQuorum compares with the quorum), and
+ *                          has_quorum = 0 when the proposer's own PREPARE is among the valid items (its bit is set in the voted
+ *                          set).  n_valid and n_distinct count the senders only, as under the other rules.
+ *   3                      reserved.
+ * With rule 0 (and the reserved field ignored) every result is what it was before rules existed.  Validated on the host by
+ * every call that takes groups (the host-buffer calls and ibft_bind_groups): a rule of 3, a proposer index >= the table's n, or
+ * a rule other than 0 on an IBFT_NO_TABLE group fails with IBFT_ERR_INVALID_ARG and nothing is launched. */
+#define IBFT_QUORUM_RULE_MASK 3u
+#define IBFT_QUORUM_DEFAULT 0u
+#define IBFT_QUORUM_PREPREPARE 1u
+#define IBFT_QUORUM_PREPARE 2u
+#define IBFT_PROPOSER_NONE 0xFFFFFFFFu
+#define IBFT_PROPOSER_UNSET 0xFFFFFFFEu
+
 /* Per-group result of the on-device quorum reduction.
  * power[] is the little-endian 320-bit sum of votingPower over the DISTINCT validators with >= 1 valid
- * item in the group (HasQuorum sums over an address *set*: validator_manager.go:88-92, :147-155).
- * has_quorum = power >= floor(2*total/3)+1 (validator_manager.go:95, :130-135). */
+ * item in the group (HasQuorum sums over an address *set*: validator_manager.go:88-92, :147-155); under IBFT_QUORUM_PREPARE
+ * the proposer's power is part of the sum.
+ * has_quorum = the group's quorum rule (IBFT_QUORUM_*); under the default rule power >= floor(2*total/3)+1
+ * (validator_manager.go:95, :130-135). */
 typedef struct ibft_group_result {
   uint64_t power[5];
   uint32_t n_valid;     /* items of the group with verdict 1 */
@@ -207,7 +234,9 @@ int ibft_verify_batch_device(ibft_engine* e, const void* d_items, uint32_t n, co
 
 /* Device-resident quorum reduction over a complete (all-gathered) bitmap: resolves each item's signer to its
  * validator index, ORs the per-group voted sets and reduces voting power against the threshold.
- * d_groups: ibft_group_desc[n_groups]; d_results: ibft_group_result[n_groups] (device). */
+ * d_groups: ibft_group_desc[n_groups]; d_results: ibft_group_result[n_groups] (device).
+ * has_quorum follows each bound group's quorum rule (IBFT_QUORUM_*, validated by ibft_bind_groups): a PREPARE group gets
+ * HasPrepareQuorum and a PREPREPARE group "at least one valid message" without a return to the host. */
 int ibft_quorum_reduce_device(ibft_engine* e, const void* d_items, uint32_t n, const void* d_bitmap,
                               const void* d_groups, uint32_t n_groups, void* d_results, void* stream);
 
@@ -216,7 +245,8 @@ int ibft_quorum_reduce_device(ibft_engine* e, const void* d_items, uint32_t n, c
  *                                 count per group); depends only on the bound groups, identical on every rank
  *   ibft_quorum_mark_device    -> marks items [shard_lo, shard_hi) with a set bitmap bit into d_partial (W words, device)
  *   (all-gather the partials -- they can ride in the same collective as the bitmap words)
- *   ibft_quorum_merge_device   -> ORs / sums n_parts partials (part_stride_words apart) and reduces against the thresholds */
+ *   ibft_quorum_merge_device   -> ORs / sums n_parts partials (part_stride_words apart) and reduces against the thresholds,
+ *                                 applying each bound group's quorum rule (IBFT_QUORUM_*) to the merged voted sets and counts */
 int ibft_quorum_partial_words(ibft_engine* e, uint32_t* words_out);
 int ibft_quorum_mark_device(ibft_engine* e, const void* d_items, uint32_t n, uint32_t shard_lo, uint32_t shard_hi,
                             const void* d_bitmap, void* d_partial, void* stream);
@@ -230,7 +260,8 @@ int ibft_quorum_merge_device(ibft_engine* e, const void* d_partials, uint32_t n_
  *   into parity (epoch & 1) of ITS buffer and marks its votes behind the bitmap words of that parity (ibft_quorum_mark_device),
  *   then calls this: ONE kernel publishes the rank's flag, waits (bounded) for the peers' flags, reads their words out of peer
  *   memory -- OR-ing voted sets, summing counts, assembling the complete bitmap in d_bitmap_full (world x bitmap_words_per_rank
- *   words) -- and the weighted reduce follows.  peer_bufs[r] = device address of rank r's buffer as mapped in THIS process.
+ *   words) -- and the weighted reduce follows, under each bound group's quorum rule (IBFT_QUORUM_*).  peer_bufs[r] = device
+ *   address of rank r's buffer as mapped in THIS process.
  *   *d_timeout_flag (device uint32, zeroed by the caller) becomes 1 when a peer did not publish in time: results are then
  *   meaningless and the device is NOT left spinning. */
 /* Exchange buffers.  The engine allocates one (zeroed, `words` uint32 words = 2 * words_per_rank + 2 flags, rounded up) and
