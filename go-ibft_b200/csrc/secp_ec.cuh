@@ -650,7 +650,8 @@ IBFT_HD void ecmult_build_rtable(const aff& R, const rtab_view& T) {
 // addition); scale every entry up to the LAST entry's Z with those ratios -- (X f^2, Y f^3), f = Z_8 / Z_m -- and read the
 // table as AFFINE points of the isomorphic curve Y^2 = X^3 + 7 Z_8^6.  The caller runs the window loop on that curve (the a = 0
 // law never uses b) and multiplies the accumulator's Z by the returned Z_8 at the end.  Only usable when nothing else (no
-// generator point of the original curve) is added inside the loop: the chain warps of k_recover_split.
+// generator point of the original curve) is added inside the loop: the chain warps of k_recover_split and the one-thread
+// recovery (verify_core.cuh recover_key), which add u1*G after the loop.
 // 1 dbl + 6 madd + 6 M + 7 (1S + 3M), against 4 dbl + 3 madd + inversion + 6 M + 7 (1S + 5M) for ecmult_build_rtable.
 IBFT_HD fe ecmult_build_rtable_globalz(const aff& R, const rtab_view& T) {
   fe zr[8];  // zr[m] = Z of entry m / Z of entry m-1
@@ -845,9 +846,31 @@ IBFT_HD jac ecmult_gen_comb(const ecmult_digits& dg, const gtab_view& G) {
     fe x, y;
     G.load_comb_pos(jg, d1, d2, x, y);
     if (neg) y = fe_neg(y);
+    IBFT_OPCOUNT(IBFT_OP_COMB_ADD);
     acc = jac_add_affine(acc, x, y);
   }
   return acc;
+}
+
+// L2 prefetch of the comb entries ecmult_gen_comb is about to read: the 17 gathers are issued together instead of one per
+// dependent addition (the per-position tables are 36 MB, so a random entry is rarely in L2 already)
+IBFT_HD void ecmult_gen_comb_prefetch(const ecmult_digits& dg, const gtab_view& G) {
+#if defined(__CUDA_ARCH__)
+  IBFT_ROLLED
+  for (int jg = IBFT_CTAB_POSITIONS - 1; jg >= 0; jg--) {
+    int d1 = booth_digit<IBFT_WC>(dg.ks[2], jg), d2 = booth_digit<IBFT_WC>(dg.ks[3], jg);
+    if (dg.kneg[2]) d1 = -d1;
+    if (dg.kneg[3]) d2 = -d2;
+    if (d1 < 0 || (d1 == 0 && d2 < 0)) { d1 = -d1; d2 = -d2; }
+    const uint32_t* e = G.comb + (size_t)jg * IBFT_GTAB_ENTRY_WORDS * (size_t)IBFT_CTAB_ENTRIES +
+                        (size_t)IBFT_GTAB_ENTRY_WORDS * ((size_t)d1 * IBFT_CTAB_D2 + (size_t)(d2 + (1 << (IBFT_WC - 1))));
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(e));
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(e + 8));
+  }
+#else
+  (void)dg;
+  (void)G;
+#endif
 }
 #endif
 

@@ -59,6 +59,12 @@ __device__ unsigned long long g_stage_clk[16];
 #define IBFT_BR_XADD_NEG 4     // xyzz_add_x: P + (-P)
 #define IBFT_BR_XADD_INF 5     // xyzz_add_x: accumulator at infinity
 #define IBFT_BR_COUNT 6
+// the rare cases of the one-thread recovery's final A + B (verify_core.cuh recover_final): ids past the 2 * IBFT_BR_COUNT
+// overall and final-add counters of the emulation
+#define IBFT_BR_REC_DBL 12     // A = B: the sum is a doubling
+#define IBFT_BR_REC_NEG 13     // A = -B: the sum is the point at infinity
+#define IBFT_BR_REC_B_INF 14   // u1 * G is the point at infinity (u1 = 0)
+#define IBFT_BR_REC_NONRES 15  // r^3 + 7 is a non-residue: r is not an abscissa
 #ifndef IBFT_BRANCH
 #define IBFT_BRANCH(i) do { } while (0)
 #endif
@@ -79,7 +85,10 @@ __device__ unsigned long long g_stage_clk[16];
 #define IBFT_OP_WIN 10         // window-loop iterations
 #define IBFT_OP_WIN_DBL 11     // doublings inside the window loop
 #define IBFT_OP_WIN_ADD 12     // mixed additions inside the window loop
-#define IBFT_OP_COUNT 13
+#define IBFT_OP_COUNT 13       // the counters above (emul_op_counts)
+#define IBFT_OP_COMB_ADD 13    // mixed additions of the u1 * G comb (ecmult_gen_comb)
+#define IBFT_OP_REC_FINAL 14   // final steps of the one-thread recovery (A + B, root and inverse, affine)
+#define IBFT_OP_COUNT_ALL 15
 #ifndef IBFT_OPCOUNT
 #define IBFT_OPCOUNT(k) do { } while (0)
 #endif
@@ -864,6 +873,30 @@ IBFT_HD fe fe_sqrt_candidate(const fe& a) {
   t = fe_mul(t, c.x2);
   t = fe_sqrn(t, 2);
   return t;
+}
+
+// The square root of c and the inverse of y V from ONE exponentiation (V != 0):
+//   u = (c V^4)^((p-3)/4) = c^((p-3)/4) V^-2,   y = c V^2 u = c^((p+1)/4),   w = u V = c^((p-3)/4) / V,
+// and y w V = c^((p-1)/2), so w = 1 / (y V) exactly when c is a residue (y^2 = c); the caller checks that.  Negating y negates
+// 1 / (y V): the caller flips w with y.  (p-3)/4 = [223 ones][0][22 ones][0000][1][0][11]: the chain of fe_sqrt_candidate
+// up to its last six bits, one multiplication more.  Out of line: the recovery calls it from its rare branches too.
+struct fe_root_inv {
+  fe y, w;
+};
+IBFT_FN fe_root_inv fe_sqrt_inv(fe c, fe V) {
+  const fe v2 = fe_sqr(V);
+  const fe a = fe_mul(c, fe_sqr(v2));
+  fe_chain ch = fe_chain_223(a);
+  fe t = fe_sqrn(ch.x223, 23);
+  t = fe_mul(t, ch.x22);
+  t = fe_sqrn(t, 5);
+  t = fe_mul(t, a);
+  t = fe_sqrn(t, 3);
+  t = fe_mul(t, ch.x2);
+  fe_root_inv o;
+  o.y = fe_mul(fe_mul(c, v2), t);
+  o.w = fe_mul(t, V);
+  return o;
 }
 
 // a^(p-2) (Fermat inverse; 0 -> 0).  p-2 = [223 ones][0][22 ones][0000][1][0][11][0][1]

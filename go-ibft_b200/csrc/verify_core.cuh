@@ -320,16 +320,11 @@ __device__ __forceinline__ bool ecmult_affine(const exec_quad& ex, const sc& u1,
 }
 #endif
 
-// Recover the signer of (r, s, v) over digest z.  Returns false when the signature is invalid; addr20 then zero.
+// The public key Q = r^-1 (s R - z G) of an in-range (r, s, v): R = lift_x(r, v) by a square root, then u1 G + u2 R by the
+// executor's ecmult_affine.  false: r is not an abscissa, or Q is the point at infinity.
 template <class EX>
-IBFT_HD bool ecrecover_address_x(const EX& ex, const uint8_t* r_be, const uint8_t* s_be, uint8_t v, const uint8_t* z_be,
-                                 const gtab_view& G, const rtab_view& T, uint8_t* addr20, aff* key_out = nullptr) {
-#pragma unroll
-  for (int i = 0; i < 20; i++) addr20[i] = 0;
-  sc r = sc_from_be(r_be), s = sc_from_be(s_be);
-  if (v > 1) return false;
-  if (sc_is_zero(r) || sc_is_zero(s) || sc_ge_n(r) || sc_ge_n(s)) return false;
-  IBFT_STAGE(1);
+IBFT_HD bool recover_key(const EX& ex, const sc& r, const sc& s, uint8_t v, const uint8_t* z_be, const gtab_view& G,
+                         const rtab_view& T, fe& qx, fe& qy) {
   // R = lift_x(r, v)   (r < n < p: always a canonical field element)
   fe x;
 #pragma unroll
@@ -349,8 +344,138 @@ IBFT_HD bool ecrecover_address_x(const EX& ex, const uint8_t* r_be, const uint8_
   sc u1 = sc_neg(sc_mul(z, rinv));
   sc u2 = sc_mul(s, rinv);
   IBFT_STAGE(3);
+  return ecmult_affine(ex, u1, u2, R, G, T, qx, qy);
+}
+
+#if IBFT_WC > 0 && !defined(IBFT_RECOVER_TABLE_INV)
+// ------------------------------------------------------------------------------------------------------------
+// The one-thread recovery (exec_serial: k_recover and the key registry's worklist pass) without a field inversion.
+// -DIBFT_RECOVER_TABLE_INV keeps the composition above (affine table by one inversion, generator streams inside the window
+// loop, inversion of Z at the end) for A/B runs.
+//   1. u2 * R on the isomorphic curve E': phi(R) = (x c, c^2), c = x^3 + 7 = y^2, needs no square root; the table {1..8} phi(R)
+//      is made "effective affine" without an inversion (ecmult_build_rtable_globalz), and the window loop walks the R streams
+//      only.  Its result (X, Y, Z) on E' with the table's Z_8 is the Jacobian point A = (X, Y, W0 y) of E, W0 = Z Z_8: y stays
+//      unknown.
+//   2. u1 * G by the comb over the per-position tables (ecmult_gen_comb, no doubling) into B = (Xb, Yb, Zb).
+//   3. A + B (recover_final): Z_A^2 = W0^2 c needs no root, so H and V = W0 Zb H do not depend on y; ONE exponentiation of
+//      c V^4 gives y = sqrt(c) and 1 / (y V) = 1 / Z3 (fe_sqrt_inv), then S2 and the rest of the addition use y.
+// A = (X, Y, W0) is held with Z = W0 (the factor y kept apart); the rare cases are exact: A = +-B, u1 = 0, a non-residue c.
+// ------------------------------------------------------------------------------------------------------------
+IBFT_HD bool recover_affine(const fe& x, const fe& y, const fe& zi, fe& qx, fe& qy) {
+  const fe zi2 = fe_sqr(zi);
+  qx = fe_normalize(fe_mul(x, zi2));
+  qy = fe_normalize(fe_mul(y, fe_mul(zi2, zi)));
+  return true;
+}
+// y = sqrt(c) with parity v and w = 1 / (y V); false when c is a non-residue
+IBFT_HD bool recover_root(const fe& c, const fe& V, uint8_t v, fe& y, fe& w) {
+  const fe_root_inv o = fe_sqrt_inv(c, V);
+  if (!fe_equal(fe_sqr(o.y), c)) {
+    IBFT_BRANCH(IBFT_BR_REC_NONRES);
+    return false;
+  }
+  y = fe_normalize(o.y);
+  w = o.w;
+  if ((y.v[0] & 1u) != (uint32_t)v) {
+    y = fe_normalize(fe_neg(y));
+    w = fe_neg(w);
+  }
+  return true;
+}
+IBFT_HD bool recover_final(const jac& A, const fe& c, uint8_t v, const jac& B, fe& qx, fe& qy) {
+  IBFT_OPCOUNT(IBFT_OP_REC_FINAL);
+  fe y, w;
+  if (B.inf) {  // u1 = 0: Q = A, Z_A = W0 y
+    IBFT_BRANCH(IBFT_BR_REC_B_INF);
+    if (A.inf || !recover_root(c, A.z, v, y, w)) return false;
+    return recover_affine(A.x, A.y, w, qx, qy);
+  }
+  if (A.inf) {  // u2 R is never infinity (0 < u2 < n); Q = B, and c must still be a residue
+    if (!recover_root(c, B.z, v, y, w)) return false;
+    return recover_affine(B.x, B.y, fe_mul(y, w), qx, qy);  // 1 / Zb = y / (y Zb)
+  }
+  // add-1998-cmo-2 with Z1 = W0 y, Z2 = Zb: Z1Z1 = W0^2 c, S2 = Yb Z1 Z1Z1 = y (Yb W0 Z1Z1), Z3 = Z1 Z2 H = y V
+  const fe z1z1 = fe_mul(fe_sqr(A.z), c);
+  const fe z2z2 = fe_sqr(B.z);
+  const fe u1 = fe_mul(A.x, z2z2);
+  const fe h = fe_sub(fe_mul(B.x, z1z1), u1);
+  const fe s1 = fe_mul(A.y, fe_mul(B.z, z2z2));
+  const fe t2 = fe_mul(B.y, fe_mul(A.z, z1z1));  // S2 / y
+  if (fe_is_zero(h)) {  // A = +-B (crafted signatures only): y first, then the sign of S2 - S1 decides
+    if (!recover_root(c, A.z, v, y, w)) return false;
+    if (!fe_is_zero(fe_sub(fe_mul(t2, y), s1))) {
+      IBFT_BRANCH(IBFT_BR_REC_NEG);
+      return false;  // A = -B: Q is the point at infinity
+    }
+    IBFT_BRANCH(IBFT_BR_REC_DBL);
+    jac P = A;
+    P.z = fe_mul(A.z, y);
+    const jac D = jac_double(P);
+    if (!recover_root(c, D.z, v, y, w)) return false;
+    return recover_affine(D.x, D.y, fe_mul(y, w), qx, qy);
+  }
+  const fe V = fe_mul(fe_mul(A.z, B.z), h);
+  if (!recover_root(c, V, v, y, w)) return false;
+  const fe rr = fe_sub(fe_mul(t2, y), s1);
+  const fe hh = fe_sqr(h);
+  const fe hhh = fe_mul(h, hh);
+  const fe vv = fe_mul(u1, hh);
+  const fe x3 = fe_sub(fe_sub(fe_sqr(rr), hhh), fe_dbl(vv));
+  const fe y3 = fe_sub(fe_mul(rr, fe_sub(vv, x3)), fe_mul(s1, hhh));
+  return recover_affine(x3, y3, w, qx, qy);
+}
+
+IBFT_HD bool recover_key(const exec_serial& ex, const sc& r, const sc& s, uint8_t v, const uint8_t* z_be, const gtab_view& G,
+                         const rtab_view& T, fe& qx, fe& qy) {
+#if !defined(__CUDA_ARCH__)
+  // the host emulation supplies the per-position comb entries through host_pos; without them it runs the composition above
+  if (G.host_pos == nullptr) return recover_key<exec_serial>(ex, r, s, v, z_be, G, T, qx, qy);
+#endif
+  // u1 = -z/r, u2 = s/r  (mod n)
+  sc z = sc_reduce_once(sc_from_be(z_be));
+  sc rinv = IBFT_SC_INV(r);
+  ecmult_digits dg;
+  ecmult_split_into(sc_mul(s, rinv), dg, 0);
+  ecmult_split_into(sc_neg(sc_mul(z, rinv)), dg, 2);
+  IBFT_STAGE(3);
+  // phi(R) on E' and its inversion-free table; c = x^3 + 7
+  fe x;
+#pragma unroll
+  for (int i = 0; i < 8; i++) x.v[i] = r.v[i];
+  fe c = fe_add(fe_mul(fe_sqr(x), x), fe_from_u32(7));
+  aff Rp;
+  Rp.x = fe_mul(x, c);
+  Rp.y = fe_sqr(c);
+  IBFT_STAGE(4);
+  const fe z8 = ecmult_build_rtable_globalz(Rp, T);
+  IBFT_STAGE(7);
+  jac A = ecmult_streams(dg, G, T, false);
+  IBFT_STAGE(8);
+  // park A (and c) in this thread's slice of the table, dead from here on: the comb's accumulator takes their registers
+  const bool a_inf = A.inf;
+  T.store(0, A.x, A.y);
+  T.store(1, fe_mul(A.z, z8), c);
+  ecmult_gen_comb_prefetch(dg, G);
+  const jac B = ecmult_gen_comb(dg, G);
+  T.load(0, A.x, A.y);
+  T.load(1, A.z, c);
+  A.inf = a_inf;
+  return recover_final(A, c, v, B, qx, qy);
+}
+#endif
+
+// Recover the signer of (r, s, v) over digest z.  Returns false when the signature is invalid; addr20 then zero.
+template <class EX>
+IBFT_HD bool ecrecover_address_x(const EX& ex, const uint8_t* r_be, const uint8_t* s_be, uint8_t v, const uint8_t* z_be,
+                                 const gtab_view& G, const rtab_view& T, uint8_t* addr20, aff* key_out = nullptr) {
+#pragma unroll
+  for (int i = 0; i < 20; i++) addr20[i] = 0;
+  sc r = sc_from_be(r_be), s = sc_from_be(s_be);
+  if (v > 1) return false;
+  if (sc_is_zero(r) || sc_is_zero(s) || sc_ge_n(r) || sc_ge_n(s)) return false;
+  IBFT_STAGE(1);
   fe qx, qy;
-  if (!ecmult_affine(ex, u1, u2, R, G, T, qx, qy)) return false;
+  if (!recover_key(ex, r, s, v, z_be, G, T, qx, qy)) return false;
   if (key_out) { key_out->x = qx; key_out->y = qy; }
   IBFT_STAGE(9);
   keccak256_xy_address(qx, qy, addr20);

@@ -6,15 +6,17 @@ instruction, every other IMAD-class instruction (IMAD.MOV, IMAD.X, IMAD.HI, ...)
 pipe's work per recovery without a GPU:
 
   static   the SASS of k_recover<128> (cuobjdump): every out-of-line routine it calls (fe_mul, fe_sqr, fe_sqrn, the doubling's
-           fused front end, the safegcd inversions) and the window loop, found by its back branches;
+           fused front end, the safegcd inversion, the root-and-inverse exponentiation fe_sqrt_inv), the window loop and the
+           u1*G comb loop after it, found by their back branches;
   dynamic  how often each of them runs per recovery, counted by the host emulation of the same sources (IBFT_OPCOUNT,
-           tests/emul) over the config-3 items (tests/golden/config3.npz).
+           tests/emul/recover_comb.cpp: the product's one-thread composition) over the config-3 items (tests/golden/config3.npz).
 
 It prints per-routine instruction counts, then estimated FMA-pipe cycles, IMAD.WIDE and products per recovery and the
 hot-loop code size (window loop + every routine it calls outside the P + P block).  The estimate covers the field routines, the inversions and the
-window loop.  The addition body is charged whole to every addition except its P + P block (listed apart, never taken by the
-config-3 items); its other short branches (beta, negation, zero digits) are counted as taken, so that term is an upper
-bound.  Keccak, range checks and the inline code around the square root are not modelled.
+window loop and the comb loop.  The addition body is charged whole to every addition except its P + P block (listed apart,
+never taken by the config-3 items); its other short branches (beta, negation, zero digits) are counted as taken, so that term
+is an upper bound.  Keccak, range checks and the inline code of the final addition (its products are calls, counted above) are
+not modelled.
 
   python tools/fma_budget.py                 # builds go-ibft_b200/libibftverify.so if stale
   IBFT_LIB=/path/libibftverify.so python tools/fma_budget.py --items 2000
@@ -38,10 +40,10 @@ CUOBJDUMP = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", 
 
 # IBFT_OP_* of csrc/secp_fe.cuh
 OPS = ["mul_body", "sqr_body", "mul_call", "sqr_call", "sqrn_call", "sqrn_iter", "dbl_front", "fe_inv", "sc_inv", "inv_iter",
-       "win", "win_dbl", "win_add"]
+       "win", "win_dbl", "win_add", "comb_add", "rec_final"]
 # demangled-name fragment of an out-of-line routine -> its call counter
 ROUTINES = [("fe_mul", "mul_call"), ("fe_sqrn", "sqrn_call"), ("fe_sqr", "sqr_call"), ("jac_dbl_front", "dbl_front"),
-            ("fe_inv_safegcd", "fe_inv"), ("sc_inv_safegcd", "sc_inv")]
+            ("fe_inv_safegcd", "fe_inv"), ("sc_inv_safegcd", "sc_inv"), ("fe_sqrt_inv", "rec_final")]
 # routines with an inner loop: the counter of that loop's iterations
 LOOPS = {"fe_sqrn": "sqrn_iter", "fe_inv_safegcd": "inv_iter", "sc_inv_safegcd": "inv_iter"}
 
@@ -152,12 +154,20 @@ def cold_block(add_loop, bounds, names):
     return best or []
 
 
+def comb_loop(body, window_tail):
+    """the u1*G comb loop: the first loop after the window loop that makes calls (the prefetch loop before it makes none)"""
+    after = sorted((h, t) for h, t in loops(body) if h > window_tail and tally(span(body, h, t))["call"])
+    if not after:
+        raise SystemExit("comb loop not found in the SASS")
+    return after[0]
+
+
 def counting_emulation(out_dir: str) -> ctypes.CDLL:
-    """the host emulation built with its operation counters (tests/emul/opcount.cpp) into out_dir"""
+    """the host emulation of the product's one-thread composition with its operation counters (tests/emul/recover_comb.cpp)"""
     emul = os.path.join(ROOT, "tests", "emul")
-    so = os.path.join(out_dir, "libibft_opcount.so")
+    so = os.path.join(out_dir, "libibft_recover_comb.so")
     subprocess.check_call([os.environ.get("CXX", "g++"), "-O2", "-fPIC", "-std=c++17", '-DEMUL_DIR="%s"' % emul, "-shared", "-o",
-                           so, os.path.join(emul, "opcount.cpp"), "-lpthread"])
+                           so, os.path.join(emul, "recover_comb.cpp"), "-lpthread"])
     return ctypes.CDLL(so)
 
 
@@ -171,12 +181,12 @@ def op_counts(items_limit: int):
         items = items[:items_limit]
     out = (ctypes.c_uint8 * 20)()
     ap = arena.ctypes.data_as(ctypes.c_void_p)
-    E.emul_verify_item(items[0].ctypes.data_as(ctypes.c_void_p), ap, ctypes.c_size_t(len(arena)), out)  # builds the emulation's tables
+    E.emul_verify_item_comb(items[0].ctypes.data_as(ctypes.c_void_p), ap, ctypes.c_size_t(len(arena)), out)  # builds the emulation's tables
     E.emul_op_reset()
     for i in range(len(items)):
-        E.emul_verify_item(items[i].ctypes.data_as(ctypes.c_void_p), ap, ctypes.c_size_t(len(arena)), out)
+        E.emul_verify_item_comb(items[i].ctypes.data_as(ctypes.c_void_p), ap, ctypes.c_size_t(len(arena)), out)
     buf = (ctypes.c_ulonglong * 32)()
-    n = E.emul_op_counts(buf)
+    n = E.emul_op_counts_all(buf)
     assert n <= len(OPS), "IBFT_OP_* of secp_fe.cuh and OPS of this tool disagree"
     return {k: (buf[i] if i < n else 0) for i, k in enumerate(OPS)}, len(items)
 
@@ -220,6 +230,8 @@ def main():
     rows.append(("window loop: doubling", tally(dbl_loop), per["win_dbl"]))
     rows.append(("window loop: stream/addition", tally([x for x in add_loop if x not in cold]), per["win_add"]))
     rows.append(("window loop: P + P block (rare)", tally(cold), 0.0))
+    ch, ct = comb_loop(body, wt)
+    rows.append(("comb loop: per addition", tally(span(body, ch, ct)), per["comb_add"]))
 
     print(f"library: {lib}")
     print(f"dynamic counts: host emulation of {n_items} config-3 items, {recoveries:.0f} double-scalar multiplications")
