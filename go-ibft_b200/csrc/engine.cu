@@ -23,6 +23,7 @@
 
 #include "../../include/ibft_verify.h"
 #include "verify_core.cuh"
+#include "debug_arith.cuh"
 
 #include "secp_gtable.inc"
 
@@ -1534,7 +1535,7 @@ __global__ void k_debug_op(int op, const uint8_t* a, const uint8_t* b, const uin
       }
       break;
     }
-    default: break;
+    default: debug_arith_op(op, pa, pb, o); break;
   }
 }
 

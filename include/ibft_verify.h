@@ -345,6 +345,22 @@ int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* wide_mac_per
 #define IBFT_DBG_FE_ADD 8   /* out = a+b mod p */
 #define IBFT_DBG_FE_SUB 9   /* out = a-b mod p */
 #define IBFT_DBG_GLV 10     /* out(64) = |k1| (16B BE) || |k2| (16B BE) || sign1 || sign2 padded -- see tests */
+/* Arithmetic at the reduction edges (csrc/debug_arith.cuh).  "Raw" results are the routine's weakly reduced limbs (< 2^256, not
+ * necessarily < p), exactly what the kernels chain into the next operation. */
+#define IBFT_DBG_FE_MUL_RAW 11     /* out = fe_mul(a, b), raw */
+#define IBFT_DBG_FE_SQR_RAW 12     /* out = fe_sqr(a), raw */
+#define IBFT_DBG_FE_ADD_RAW 13     /* out = fe_add(a, b), raw */
+#define IBFT_DBG_FE_SUB_RAW 14     /* out = fe_sub(a, b), raw */
+#define IBFT_DBG_FE_NORMALIZE 15   /* out = fe_normalize(a) */
+#define IBFT_DBG_FE_EQUAL 16       /* out[0] = fe_equal(a, b) (1 byte) */
+#define IBFT_DBG_FE_SQRN 17        /* out = fe_sqrn(a, k), k = low byte of b, raw */
+#define IBFT_DBG_FE_SQRT_INV 18    /* out(64) = y || w of fe_sqrt_inv(c = a, V = b), raw */
+#define IBFT_DBG_SC_ADD 19         /* out = sc_add(a, b) */
+#define IBFT_DBG_SC_NEG 20         /* out = sc_neg(a) */
+#define IBFT_DBG_SC_REDUCE_ONCE 21 /* out = sc_reduce_once(a) */
+#define IBFT_DBG_SC_DIGITS 22      /* out(256): ecmult_split_into(a), a in [0, n), and the Booth digits of both halves: half h at
+                                    * 128 h = magnitude (6 words, little-endian) || sign byte at 24 || 33 int8 4-bit digits at 32
+                                    * || 17 int16 (little-endian) 8-bit digits at 72 */
 /* Generator comb tables (builds with IBFT_WC > 0): *wc = window (0 when absent), *entries = entries of one comb position;
  * copies `count` 64-byte entries (x, y as 8 little-endian words each) starting at `first`, positions laid out one after the
  * other: entry p * entries + d1 * (2^wc + 1) + d2 + 2^(wc-1) holds (d1 + d2*lambda) * 2^(wc*p) * G, p = 0..16 (position 0 is

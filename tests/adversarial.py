@@ -11,10 +11,12 @@ Known-key vectors: pick the key Q and u1 = z/s, u2 = r/s of the verification u1 
 from __future__ import annotations
 
 import functools
+import random
 from dataclasses import dataclass
 
 import numpy as np
 
+from arith_edges import fold4_signature_targets
 from oracle import secp256k1 as ec
 
 N = ec.N
@@ -96,6 +98,15 @@ def recover_vectors() -> tuple[Vector, ...]:
     for u2 in (1, 7, LAM, 0xDEADBEEF):
         out.append(recover_vector(f"u1=0 z=0 u2={u2:#x}", R, 0, u2))
         out.append(recover_vector(f"u1=0 z=n u2={u2:#x}", R, 0, u2, z_override=N.to_bytes(32, "big")))  # digest >= n, reduces to 0
+    # the mod-n products s r^-1 (u2) and z r^-1 (u1) carry into sc_reduce512's fold 4 (tests/arith_edges.py)
+    # (the 512-bit product must exceed about 0.62 * 2^512, so r^-1 has to be large: R = c G for the first such c)
+    rnd = random.Random(0xF014)
+    fold4 = [c for c in range(2, 200) if pow(mul(c)[0], -1, N) > 7 * N // 8][:5]
+    for c in fold4:
+        R = mul(c)
+        t_u2, t_u1 = fold4_signature_targets(rnd, R[0], 2)
+        out.append(recover_vector(f"fold4 u2 c={c:#x}", R, rnd.randrange(1, N), t_u2))
+        out.append(recover_vector(f"fold4 u1 c={c:#x}", R, -t_u1, rnd.randrange(1, N)))
     twins = [high_s_twin(v) for v in out if 0 < int.from_bytes(v.sig[32:64], "big") < N]
     return tuple(out + twins)
 

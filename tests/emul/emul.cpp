@@ -14,6 +14,7 @@ static std::atomic<unsigned long long> g_branch[16];
 #define IBFT_BRANCH(i) g_branch[i].fetch_add(1, std::memory_order_relaxed)
 
 #include "../../go-ibft_b200/csrc/verify_core.cuh"
+#include "../../go-ibft_b200/csrc/debug_arith.cuh"
 #include "../../go-ibft_b200/csrc/secp_gtable.inc"
 
 #include <cstdio>
@@ -349,7 +350,7 @@ int emul_debug_op(int op, const uint8_t* a, const uint8_t* b, const uint8_t* c, 
       fe_to_be(fe_normalize(fe_mul(Q.y, fe_mul(zi2, zi))), out + 32);
       return 0;
     }
-    default: return -1;
+    default: return debug_arith_op(op, a, b, out) ? 0 : -1;
   }
 }
 }
