@@ -103,6 +103,11 @@ class ShardedVerifier:
 
     The descriptors are bound as given, quorum rule and proposer included (Engine.groups(..., rule=, proposer=)): both exchanges
     return go-ibft's per-message-type decision (HasPrepareQuorum for PREPARE groups, one valid message for PREPREPARE groups).
+
+    Peer-memory exchange: when a peer does not publish its round within the kernel's bounded wait, finish() raises RuntimeError,
+    and so does every later round of this verifier -- the timeout flag is never cleared.  Rebuild the verifiers of all ranks
+    after a timeout: the parity alternation only guarantees that a peer has finished reading this rank's buffer of round e when
+    this rank has seen the peer's flag of round e + 1, and a timed-out round skipped that check.
     """
 
     def __init__(self, engine, n_global: int, groups: np.ndarray, world: int, rank: int, local_items: np.ndarray,
