@@ -19,6 +19,7 @@
 #include <cstring>
 #include <mutex>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/ibft_verify.h"
@@ -50,16 +51,29 @@ struct slot_dev {
   uint64_t quorum[5];      // floor(2*total/3) + 1
   uint32_t n;
   uint32_t valid;
-  // key registry (engine flag IBFT_FLAG_KEY_CACHE; all nullptr otherwise), validator-index order:
-  uint32_t* key_state;     // 0 = unknown, 1 = key learned from a successful recovery, 3 = table being built, 2 = comb table built
-  uint32_t* key_xy;        // n x 16 words: affine public key
-  uint32_t* key_tab;       // n x IBFT_KEYTAB_WORDS: per validator 17 comb positions x 128 entries x 16 words, affine (build_keytab_pos)
-  uint32_t* learn_count;   // number of keys learned so far (the host compares it with the number of tables built)
+  // key registry (engine flag IBFT_FLAG_KEY_CACHE; all nullptr otherwise).  One registry per ENGINE, one entry per distinct
+  // address of the resident tables: a key belongs to an address, not to a height, so every slot that lists the address reads
+  // the same entry.  key_ref maps this table's validator index to its entry; the other pointers are the engine's registry
+  // (the same in every slot).
+  const uint32_t* key_ref;     // n words, validator-index order: registry entry of the validator's address
+  uint32_t* key_state;         // per entry: 0 = unknown, 1 = key learned from a successful recovery, 3 = table being built,
+                               // 2 = comb table built
+  uint32_t* key_xy;            // 16 words per entry: affine public key
+  uint32_t* const* key_chunks; // comb tables, IBFT_KEY_CHUNK entries per chunk of IBFT_KEY_CHUNK x IBFT_KEYTAB_WORDS words; per
+                               // entry 17 comb positions x 128 entries x 16 words, affine (build_keytab_pos)
+  uint32_t* learn_count;       // number of keys learned so far, engine-wide (the host compares it with the number it built)
 };
 #define IBFT_KEY_UNKNOWN 0u
 #define IBFT_KEY_LEARNED 1u
 #define IBFT_KEY_READY 2u
 #define IBFT_KEY_BUILDING 3u  // claimed by a table-build pass (refresh_key_tables_locked)
+#define IBFT_KEY_CHUNK 256u   // registry entries per comb-table chunk (34 MiB): the pool grows by whole chunks, never by copying
+#define IBFT_KEY_REF_FRESH 0x80000000u  // key_ref mark of an entry new to its address (k_adopt_entries); entries are < 2^31
+
+// comb table of registry entry r
+__device__ __forceinline__ uint32_t* key_table_of(uint32_t* const* __restrict__ chunks, uint32_t r) {
+  return chunks[r / IBFT_KEY_CHUNK] + (size_t)(r % IBFT_KEY_CHUNK) * IBFT_KEYTAB_WORDS;
+}
 
 __device__ __forceinline__ uint32_t bswap32(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
 
@@ -136,19 +150,22 @@ __device__ __forceinline__ bool member_and_vote(const ibft_group_desc* __restric
   if (ok && record) record_vote(sink, groups, group, v);
   return ok;
 }
-// key registry: remember the public key a successful recovery produced for validator v (first writer wins; concurrent
-// writers store the same key)
+// key registry: remember the public key a successful recovery produced for validator v of `slot`, in the registry entry of
+// its address -- every other resident table that lists the address sees it too (first writer wins; concurrent writers store
+// the same key)
 __device__ __forceinline__ void learn_key(const slot_dev* __restrict__ slots, uint32_t slot, int v, const aff& K) {
   if (slot == IBFT_NO_TABLE || v < 0) return;
   const slot_dev& s = slots[slot];
-  if (s.key_state == nullptr || s.key_state[v] != IBFT_KEY_UNKNOWN) return;
+  if (s.key_ref == nullptr) return;
+  const uint32_t r = s.key_ref[v];
+  if (s.key_state[r] != IBFT_KEY_UNKNOWN) return;
 #pragma unroll
   for (int i = 0; i < 8; i++) {
-    s.key_xy[16 * (size_t)v + i] = K.x.v[i];
-    s.key_xy[16 * (size_t)v + 8 + i] = K.y.v[i];
+    s.key_xy[16 * (size_t)r + i] = K.x.v[i];
+    s.key_xy[16 * (size_t)r + 8 + i] = K.y.v[i];
   }
   __threadfence();
-  if (atomicCAS(&s.key_state[v], IBFT_KEY_UNKNOWN, IBFT_KEY_LEARNED) == IBFT_KEY_UNKNOWN) atomicAdd(s.learn_count, 1u);
+  if (atomicCAS(&s.key_state[r], IBFT_KEY_UNKNOWN, IBFT_KEY_LEARNED) == IBFT_KEY_UNKNOWN) atomicAdd(s.learn_count, 1u);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -310,11 +327,16 @@ k_verify_known(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
     uint32_t slot = IBFT_NO_TABLE;
     const bool member = have && group_member(groups, n_groups, slots, n_slots, it.group, ri.signer, &v, &slot);
     if (member) {
-      bool ready = v >= 0 && slots[slot].key_state != nullptr && slots[slot].key_state[v] == IBFT_KEY_READY;
+      uint32_t r = 0;  // registry entry of the signer's address
+      bool ready = false;
+      if (v >= 0 && slots[slot].key_ref != nullptr) {
+        r = slots[slot].key_ref[v];
+        ready = slots[slot].key_state[r] == IBFT_KEY_READY;
+      }
       if (ready) {
         gtab_view G{g_gtable};
         G.comb = ctable;
-        gtab_view Qt{slots[slot].key_tab + (size_t)v * IBFT_KEYTAB_WORDS};
+        gtab_view Qt{key_table_of(slots[slot].key_chunks, r)};
         ok = ecdsa_verify_known(ri, G, Qt);
       }
       if (ok) record_vote(sink, groups, it.group, v);
@@ -737,7 +759,7 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
         int v = -1;
         uint32_t slot = IBFT_NO_TABLE;
         if (have && group_member(groups, n_groups, slots, n_slots, it.group, ri.signer, &v, &slot)) {
-          const bool ready = v >= 0 && slots[slot].key_state != nullptr && slots[slot].key_state[v] == IBFT_KEY_READY;
+          const bool ready = v >= 0 && slots[slot].key_ref != nullptr && slots[slot].key_state[slots[slot].key_ref[v]] == IBFT_KEY_READY;
           if (ready) {
             sc r = sc_from_be(ri.r), sv = sc_from_be(ri.s);
 #pragma unroll
@@ -853,7 +875,7 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
     dg.kneg[2] = dg.kneg[3] = false;
     vslot = s_slot[27 * S + i];
     const slot_dev& sd = slots[vslot >> 16];
-    gtab_view Qt{sd.key_tab + (size_t)(vslot & 0xFFFFu) * IBFT_KEYTAB_WORDS};
+    gtab_view Qt{key_table_of(sd.key_chunks, sd.key_ref[vslot & 0xFFFFu])};
     acc = ecmult_streams_known(dg, G, Qt, false);
   }
   named_bar_sync(1 + IBFT_SPLIT_CHAINS + warp, 64);  // u1*G is posted
@@ -1369,75 +1391,43 @@ k_build_ctable(uint32_t* __restrict__ out) {  // blockIdx.y = comb position: ent
 #endif
 
 #if IBFT_WC > 0
-// key registry: comb tables for every validator of `slot` whose key has been learned but whose table is missing.  One thread
-// per (validator, comb position): 8*pos doublings, 128 additions and 128 inversions each -- a whole 10k-validator set
-// (170,000 threads, 21.8 M table entries, 1.39 GB) is built once per validator set; k_keytabs_ready then publishes the tables.
+// key registry: comb tables for every registry entry whose key has been learned but whose table is missing.  One thread per
+// (entry, comb position): 8*pos doublings, 128 additions and 128 inversions each -- a whole 10k-validator set (170,000
+// threads, 21.8 M table entries, 1.39 GB) is built once per engine, whatever the number of resident heights that list it;
+// k_keytabs_step then publishes the tables.
 __global__ void __launch_bounds__(64)
-k_build_keytabs(const slot_dev* __restrict__ slots, uint32_t slot) {
-  const slot_dev& s = slots[slot];
+k_build_keytabs(const uint32_t* __restrict__ state, const uint32_t* __restrict__ key_xy, uint32_t* const* __restrict__ chunks,
+                uint32_t n_entries) {
   const uint32_t t = blockIdx.x * 64 + threadIdx.x;
-  const uint32_t v = t / IBFT_KEYTAB_POSITIONS, pos = t % IBFT_KEYTAB_POSITIONS;
-  if (s.key_state == nullptr || v >= s.n || s.key_state[v] != IBFT_KEY_BUILDING) return;
+  const uint32_t r = t / IBFT_KEYTAB_POSITIONS, pos = t % IBFT_KEYTAB_POSITIONS;
+  if (r >= n_entries || state[r] != IBFT_KEY_BUILDING) return;
   aff Q;
 #pragma unroll
   for (int i = 0; i < 8; i++) {
-    Q.x.v[i] = s.key_xy[16 * (size_t)v + i];
-    Q.y.v[i] = s.key_xy[16 * (size_t)v + 8 + i];
+    Q.x.v[i] = key_xy[16 * (size_t)r + i];
+    Q.y.v[i] = key_xy[16 * (size_t)r + 8 + i];
   }
-  build_keytab_pos(Q, (int)pos, s.key_tab + (size_t)v * IBFT_KEYTAB_WORDS + (size_t)pos * IBFT_KEYTAB_ENTRIES * IBFT_GTAB_ENTRY_WORDS);
+  build_keytab_pos(Q, (int)pos, key_table_of(chunks, r) + (size_t)pos * IBFT_KEYTAB_ENTRIES * IBFT_GTAB_ENTRY_WORDS);
 }
-// state steps around the build, one launch each on the same stream: LEARNED -> BUILDING (claim: the set of validators this pass
+// state steps around the build, one launch each on the same stream: LEARNED -> BUILDING (claim: the set of entries this pass
 // builds is fixed here -- recover kernels of another lane may keep learning keys meanwhile, those wait for the next pass),
 // BUILDING -> READY (publish)
 __global__ void __launch_bounds__(256)
-k_keytabs_step(const slot_dev* __restrict__ slots, uint32_t slot, uint32_t from, uint32_t to) {
-  const slot_dev& s = slots[slot];
-  const uint32_t v = blockIdx.x * 256 + threadIdx.x;
-  if (s.key_state != nullptr && v < s.n && s.key_state[v] == from) s.key_state[v] = to;
+k_keytabs_step(uint32_t* __restrict__ state, uint32_t n_entries, uint32_t from, uint32_t to) {
+  const uint32_t r = blockIdx.x * 256 + threadIdx.x;
+  if (r < n_entries && state[r] == from) state[r] = to;
 }
-#endif
-
-#if IBFT_WC > 0
-// key registry carry-over (ibft_set_validators): consensus moves to the next height with (mostly) the same validators, and a
-// key belongs to an ADDRESS, not to a height.  One CTA per validator of the new table (rank r of its sorted address table):
-// look the address up in the donor table; if the donor holds a finished comb table for it, copy key + table (136 KiB, 16-byte
-// loads) and publish.  A 10k-validator set is 1.39 GB of device-to-device copy, once per height.
+// ibft_set_validators: the new table's key_ref arrives with bit 31 set on the entries just given to an address the registry
+// did not hold -- a fresh or a retired entry, whose state (and key) may still be that of another address.  Reset those to
+// unknown, then clear the mark.  Runs while every lane is held and the device is idle, before the table is published.
 __global__ void __launch_bounds__(256)
-k_carry_keys(slot_dev dst, slot_dev src) {
-  __shared__ int s_src;
-  const uint32_t r = blockIdx.x;
-  const uint32_t* k = dst.keys + 6 * (size_t)r;
-  const uint32_t v = __ldg(k + 5);
-  if (threadIdx.x == 0) {
-    int lo = 0, hi = (int)src.n - 1, found = -1;
-    while (lo <= hi && found < 0) {
-      int mid = (lo + hi) >> 1;
-      const uint32_t* q = src.keys + 6 * (size_t)mid;
-      int cmp = 0;
-#pragma unroll
-      for (int i = 0; i < 5; i++) {
-        uint32_t a = __ldg(q + i), b = __ldg(k + i);
-        if (cmp == 0 && a != b) cmp = a < b ? -1 : 1;
-      }
-      if (cmp == 0) found = (int)__ldg(q + 5);
-      else if (cmp < 0) lo = mid + 1;
-      else hi = mid - 1;
-    }
-    if (found >= 0 && src.key_state[found] != IBFT_KEY_READY) found = -1;
-    s_src = found;
-  }
-  __syncthreads();
-  const int sv = s_src;
-  if (sv < 0) return;
-  const uint4* from = reinterpret_cast<const uint4*>(src.key_tab + (size_t)sv * IBFT_KEYTAB_WORDS);
-  uint4* to = reinterpret_cast<uint4*>(dst.key_tab + (size_t)v * IBFT_KEYTAB_WORDS);
-  for (uint32_t i = threadIdx.x; i < IBFT_KEYTAB_WORDS / 4; i += 256) to[i] = from[i];
-  if (threadIdx.x < 16) dst.key_xy[16 * (size_t)v + threadIdx.x] = src.key_xy[16 * (size_t)sv + threadIdx.x];
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    dst.key_state[v] = IBFT_KEY_READY;
-    atomicAdd(dst.learn_count, 1u);
+k_adopt_entries(uint32_t* __restrict__ key_ref, uint32_t n, uint32_t* __restrict__ state) {
+  const uint32_t v = blockIdx.x * 256 + threadIdx.x;
+  if (v >= n) return;
+  const uint32_t r = key_ref[v];
+  if (r & IBFT_KEY_REF_FRESH) {
+    state[r & ~IBFT_KEY_REF_FRESH] = IBFT_KEY_UNKNOWN;
+    key_ref[v] = r & ~IBFT_KEY_REF_FRESH;
   }
 }
 #endif
@@ -1613,12 +1603,45 @@ struct slot_host {
   uint32_t* d_keys = nullptr;
   uint64_t* d_powers = nullptr;
   uint64_t quorum[5] = {0, 0, 0, 0, 0};
-  // key registry (IBFT_FLAG_KEY_CACHE)
-  uint32_t* d_key_state = nullptr;
-  uint32_t* d_key_xy = nullptr;
-  uint32_t* d_key_tab = nullptr;
-  uint32_t* d_learn_count = nullptr;
-  uint32_t built_count = 0;  // value of *d_learn_count when the tables were last brought up to date
+  // key registry (IBFT_FLAG_KEY_CACHE): registry entry of each validator, on the device and here
+  uint32_t* d_key_ref = nullptr;
+  std::vector<uint32_t> key_ref;
+};
+
+// 20-byte address as a hash-map key
+struct addr20 {
+  uint8_t b[20];
+  bool operator==(const addr20& o) const { return memcmp(b, o.b, 20) == 0; }
+};
+struct addr20_hash {
+  size_t operator()(const addr20& a) const {
+    uint64_t x, y;
+    uint32_t z;
+    memcpy(&x, a.b, 8); memcpy(&y, a.b + 8, 8); memcpy(&z, a.b + 16, 4);
+    return (size_t)((x * 0x9E3779B97F4A7C15ull) ^ (y + 0x632BE59BD9B4E019ull + (x << 6) + (x >> 2)) ^ ((uint64_t)z << 29));
+  }
+};
+
+// The engine's key registry (IBFT_FLAG_KEY_CACHE): one entry per distinct address listed by at least one resident table.
+// Device: state and key of every possible entry (allocated at engine creation), comb tables in chunks of IBFT_KEY_CHUNK
+// entries allocated as the registry grows (only in ibft_set_validators, which holds every lane and drains the device).
+// Host: address -> entry, per-entry reference counts (one per table row that lists the address) and a free list.  An entry
+// whose count drops to 0 is retired: its address is forgotten, and the entry goes to the next new address with its state
+// reset to unknown.
+struct key_registry {
+  uint32_t capacity = 0;                 // entries that state / key_xy / the chunk-pointer array can hold
+  uint32_t* d_state = nullptr;           // capacity words
+  uint32_t* d_key_xy = nullptr;          // capacity x 16 words
+  uint32_t** d_chunks = nullptr;         // capacity / IBFT_KEY_CHUNK (rounded up) chunk base pointers
+  uint32_t* d_learn_count = nullptr;     // keys learned so far (learn_key)
+  uint32_t* h_learn_count = nullptr;     // pinned
+  uint32_t built_count = 0;              // value of *d_learn_count when the tables were last brought up to date
+  std::vector<uint32_t*> chunks;         // host copy of the allocated chunk pointers
+  uint32_t used = 0;                     // entries [0, used) have been handed out at least once (high-water mark)
+  std::unordered_map<addr20, uint32_t, addr20_hash> by_addr;
+  std::vector<addr20> addr_of;           // address of each entry in use
+  std::vector<uint32_t> refs;            // reference count of each entry
+  std::vector<uint32_t> free_list;       // retired entries, reused before the high-water mark moves
 };
 
 struct pending_call {
@@ -1692,9 +1715,8 @@ struct ibft_engine {
   std::vector<slot_dev> slots_shadow;
   std::atomic<uint64_t> launches{0};
   std::atomic<int> recover_path{IBFT_PATH_AUTO};
-  std::mutex keys_mu;                  // key registry upkeep (built_count, h_learn_counts)
-  uint32_t* d_learn_counts = nullptr;  // key registry: one "keys learned" counter per table slot (read back in one copy)
-  uint32_t* h_learn_counts = nullptr;  // pinned
+  std::mutex keys_mu;  // key registry upkeep (reg.built_count); ibft_set_validators changes the registry under every lane's lock
+  key_registry reg;
   int sm_count = 132;  // replaced by the device's count at engine creation
   uint32_t* d_ctable = nullptr;  // combined generator table (IBFT_WC > 0)
   cudaFuncAttributes recover_attr{};
@@ -1739,12 +1761,13 @@ static void engine_free(ibft_engine* e) {
   for (auto& s : e->slots) {
     if (s.d_keys) cudaFree(s.d_keys);
     if (s.d_powers) cudaFree(s.d_powers);
-    cudaFree(s.d_key_state); cudaFree(s.d_key_xy); cudaFree(s.d_key_tab);
+    cudaFree(s.d_key_ref);
   }
   for (auto& L : e->lanes) lane_free(&L);
   cudaFree(e->d_ctable);
-  cudaFree(e->d_learn_counts);
-  cudaFreeHost(e->h_learn_counts);
+  for (auto c : e->reg.chunks) cudaFree(c);
+  cudaFree(e->reg.d_state); cudaFree(e->reg.d_key_xy); cudaFree(e->reg.d_chunks); cudaFree(e->reg.d_learn_count);
+  cudaFreeHost(e->reg.h_learn_count);
   cudaFree(e->d_slots);
   if (e->hash_stream) cudaStreamDestroy(e->hash_stream);
   cudaFree(e->hs_arena); cudaFreeHost(e->hs_h_arena); cudaFree(e->hs_meta); cudaFreeHost(e->hs_h_meta);
@@ -1797,9 +1820,20 @@ static int engine_alloc(ibft_engine* e) {
   if (rc != IBFT_OK) return rc;
   lane* L = &e->lanes[0];
   if (p.flags & IBFT_FLAG_KEY_CACHE) {
-    CU(cudaMalloc(&e->d_learn_counts, (size_t)p.max_table_slots * 4));
-    CU(cudaMemset(e->d_learn_counts, 0, (size_t)p.max_table_slots * 4));
-    CU(cudaHostAlloc(&e->h_learn_counts, (size_t)p.max_table_slots * 4, cudaHostAllocDefault));
+    // the most entries there can ever be: every slot full of distinct addresses, plus the table ibft_set_validators is
+    // installing (its references are taken before the slot's previous content lets go of its own)
+    key_registry& R = e->reg;
+    const size_t cap = ((size_t)p.max_table_slots + 1) * p.max_validators;
+    if (cap >= IBFT_KEY_REF_FRESH) { set_err("key registry of %zu entries: at most 2^31 - 1", cap); return IBFT_ERR_INVALID_ARG; }
+    R.capacity = (uint32_t)cap;
+    const size_t n_chunks = (cap + IBFT_KEY_CHUNK - 1) / IBFT_KEY_CHUNK;
+    CU(cudaMalloc(&R.d_state, std::max<size_t>(cap, 1) * 4));
+    CU(cudaMalloc(&R.d_key_xy, std::max<size_t>(cap, 1) * 64));
+    CU(cudaMalloc(&R.d_chunks, std::max<size_t>(n_chunks, 1) * sizeof(uint32_t*)));
+    CU(cudaMemset(R.d_chunks, 0, std::max<size_t>(n_chunks, 1) * sizeof(uint32_t*)));
+    CU(cudaMalloc(&R.d_learn_count, 4));
+    CU(cudaMemset(R.d_learn_count, 0, 4));
+    CU(cudaHostAlloc(&R.h_learn_count, 4, cudaHostAllocDefault));
   }
   CU(cudaMalloc(&e->d_slots, (size_t)p.max_table_slots * sizeof(slot_dev)));
   CU(cudaMemset(e->d_slots, 0, (size_t)p.max_table_slots * sizeof(slot_dev)));
@@ -1855,7 +1889,8 @@ extern "C" int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count,
 
 // test hook: the key registry entry of validator `validator` (validator-index order) of a table slot -- its state
 // (IBFT_KEY_*), the learned affine key (x, y as 8 little-endian words each) and `count` comb entries starting at `first`
-// (entry j * 128 + m - 1 = m * 2^(8j) * Q, same format as ibft_debug_ctable).  Waits for the device.
+// (entry j * 128 + m - 1 = m * 2^(8j) * Q, same format as ibft_debug_ctable).  Read through the slot's key_ref into the
+// engine's registry.  Waits for the device.
 extern "C" int ibft_debug_keytab(ibft_engine* e, uint32_t table_slot, uint32_t validator, uint32_t first, uint32_t count, uint8_t* out,
                                  uint32_t* state_out, uint8_t* key_out) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
@@ -1863,24 +1898,45 @@ extern "C" int ibft_debug_keytab(ibft_engine* e, uint32_t table_slot, uint32_t v
   all_lanes_lock lk(e);
   if (table_slot >= e->p.max_table_slots || !e->slots[table_slot].valid) { set_err("slot %u not set", table_slot); return IBFT_ERR_NO_TABLE; }
   const slot_host& s = e->slots[table_slot];
-  if (!s.d_key_state) { set_err("engine has no key registry"); return IBFT_ERR_INVALID_ARG; }
+  if (!e->reg.d_state) { set_err("engine has no key registry"); return IBFT_ERR_INVALID_ARG; }
   if (validator >= s.n || (count && !out) || (size_t)first + count > (size_t)IBFT_KEYTAB_POSITIONS * IBFT_KEYTAB_ENTRIES) {
     set_err("range");
     return IBFT_ERR_INVALID_ARG;
   }
+  const uint32_t r = s.key_ref[validator];
   CU(cudaSetDevice(e->p.device));
   CU(cudaDeviceSynchronize());
-  if (state_out) CU(cudaMemcpy(state_out, s.d_key_state + validator, 4, cudaMemcpyDeviceToHost));
-  if (key_out) CU(cudaMemcpy(key_out, s.d_key_xy + 16 * (size_t)validator, 64, cudaMemcpyDeviceToHost));
-  if (count)
-    CU(cudaMemcpy(out, s.d_key_tab + (size_t)validator * IBFT_KEYTAB_WORDS + (size_t)first * IBFT_GTAB_ENTRY_WORDS, (size_t)count * 64,
-                  cudaMemcpyDeviceToHost));
+  if (state_out) CU(cudaMemcpy(state_out, e->reg.d_state + r, 4, cudaMemcpyDeviceToHost));
+  if (key_out) CU(cudaMemcpy(key_out, e->reg.d_key_xy + 16 * (size_t)r, 64, cudaMemcpyDeviceToHost));
+  if (count) {
+    const uint32_t* tab = e->reg.chunks[r / IBFT_KEY_CHUNK] + (size_t)(r % IBFT_KEY_CHUNK) * IBFT_KEYTAB_WORDS;
+    CU(cudaMemcpy(out, tab + (size_t)first * IBFT_GTAB_ENTRY_WORDS, (size_t)count * 64, cudaMemcpyDeviceToHost));
+  }
   return IBFT_OK;
 #else
   (void)table_slot; (void)validator; (void)first; (void)count; (void)out; (void)state_out; (void)key_out;
   set_err("library built without a key registry");
   return IBFT_ERR_INVALID_ARG;
 #endif
+}
+
+// test hook: the key registry as a whole -- entries in use (distinct addresses of the resident tables), how many of those have a
+// finished comb table, and the bytes of comb-table chunks allocated so far.  Any output may be NULL.  Waits for the device.
+extern "C" int ibft_debug_key_registry(ibft_engine* e, uint32_t* entries_in_use, uint32_t* entries_ready, uint64_t* bytes_reserved) {
+  if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+  all_lanes_lock lk(e);
+  const key_registry& R = e->reg;
+  if (!R.d_state) { set_err("engine has no key registry"); return IBFT_ERR_INVALID_ARG; }
+  CU(cudaSetDevice(e->p.device));
+  CU(cudaDeviceSynchronize());
+  std::vector<uint32_t> state(R.used);
+  if (R.used) CU(cudaMemcpy(state.data(), R.d_state, (size_t)R.used * 4, cudaMemcpyDeviceToHost));
+  uint32_t ready = 0;
+  for (const auto& kv : R.by_addr) ready += state[kv.second] == IBFT_KEY_READY;
+  if (entries_in_use) *entries_in_use = (uint32_t)R.by_addr.size();
+  if (entries_ready) *entries_ready = ready;
+  if (bytes_reserved) *bytes_reserved = (uint64_t)R.chunks.size() * IBFT_KEY_CHUNK * IBFT_KEYTAB_WORDS * 4;
+  return IBFT_OK;
 }
 
 // test hook: number of items the known-key pass of the most recent completed host-buffer call handed to the recover pass
@@ -1957,6 +2013,71 @@ static void be32_to_limbs(const uint8_t* b, uint64_t l[4]) {
   }
 }
 
+// Key registry (caller holds every lane, device idle): one reference per row of a table being installed.  An address the
+// registry does not hold takes a retired entry, or the next one above the high-water mark; its row of `refs` carries
+// IBFT_KEY_REF_FRESH.  The comb-table pool grows by whole chunks when the high-water mark passes its last one.  On failure
+// (IBFT_ERR_CAPACITY: the pool could not grow) the registry is exactly as it was.
+static int registry_acquire(ibft_engine* e, const uint8_t* addrs, uint32_t n, std::vector<uint32_t>& refs) {
+  key_registry& R = e->reg;
+  const uint32_t used0 = R.used;
+  const size_t chunks0 = R.chunks.size();
+  std::vector<uint32_t> fresh;  // entries given to new addresses, in the order they were taken
+  refs.assign(n, 0);
+  for (uint32_t v = 0; v < n; v++) {
+    addr20 a;
+    memcpy(a.b, addrs + 20 * (size_t)v, 20);
+    auto ins = R.by_addr.emplace(a, 0u);
+    if (ins.second) {
+      uint32_t r;
+      if (!R.free_list.empty()) { r = R.free_list.back(); R.free_list.pop_back(); }
+      else r = R.used++;
+      ins.first->second = r;
+      if (R.addr_of.size() <= r) { R.addr_of.resize((size_t)r + 1); R.refs.resize((size_t)r + 1, 0u); }
+      R.addr_of[r] = a;
+      fresh.push_back(r);
+      refs[v] = r | IBFT_KEY_REF_FRESH;
+    } else {
+      refs[v] = ins.first->second;
+    }
+  }
+  cudaError_t ce = cudaSuccess;
+  const size_t need = ((size_t)R.used + IBFT_KEY_CHUNK - 1) / IBFT_KEY_CHUNK;
+  while (R.used <= R.capacity && R.chunks.size() < need) {
+    uint32_t* c = nullptr;
+    ce = cudaMalloc(&c, (size_t)IBFT_KEY_CHUNK * IBFT_KEYTAB_WORDS * 4);
+    if (ce != cudaSuccess) break;
+    R.chunks.push_back(c);
+  }
+  if (ce == cudaSuccess && R.chunks.size() > chunks0)
+    ce = cudaMemcpy(R.d_chunks + chunks0, R.chunks.data() + chunks0, (R.chunks.size() - chunks0) * sizeof(uint32_t*), cudaMemcpyHostToDevice);
+  if (ce != cudaSuccess || R.used > R.capacity) {
+    set_err("key registry: %zu new addresses do not fit (%u entries in use, %zu chunks of %u): %s", fresh.size(),
+            (uint32_t)(R.by_addr.size() - fresh.size()), chunks0, IBFT_KEY_CHUNK,
+            ce != cudaSuccess ? cudaGetErrorString(ce) : "registry capacity");
+    (void)cudaGetLastError();
+    for (size_t i = fresh.size(); i-- > 0;) {  // forget the new addresses; retired entries go back in the order they left
+      R.by_addr.erase(R.addr_of[fresh[i]]);
+      if (fresh[i] < used0) R.free_list.push_back(fresh[i]);
+    }
+    R.used = used0;
+    while (R.chunks.size() > chunks0) { cudaFree(R.chunks.back()); R.chunks.pop_back(); }
+    refs.clear();
+    return ce == cudaSuccess || ce == cudaErrorMemoryAllocation ? IBFT_ERR_CAPACITY : IBFT_ERR_CUDA;
+  }
+  for (uint32_t v = 0; v < n; v++) R.refs[refs[v] & ~IBFT_KEY_REF_FRESH]++;
+  return IBFT_OK;
+}
+// ... and one reference less per row of a table being dropped; an entry no resident table lists any more is retired
+static void registry_release(ibft_engine* e, const std::vector<uint32_t>& refs) {
+  key_registry& R = e->reg;
+  for (uint32_t r : refs) {
+    if (--R.refs[r] == 0) {
+      R.by_addr.erase(R.addr_of[r]);
+      R.free_list.push_back(r);
+    }
+  }
+}
+
 extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t height, const uint8_t* addrs,
                                    const uint8_t* powers_be, uint32_t n) {
   if (!e || (!addrs && n)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
@@ -2018,38 +2139,52 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
   CU(cudaSetDevice(e->p.device));
   slot_host& s = e->slots[table_slot];
   CU(cudaDeviceSynchronize());
-  // the slot's previous content stays alive until its key registry has been carried over
-  slot_host old = s;
-  slot_dev old_dev = e->slots_shadow[table_slot];
+  // the slot's previous content keeps its registry references until the new table holds its own
+  slot_host old = std::move(s);
   s = slot_host{};
+  const bool registry = (e->p.flags & IBFT_FLAG_KEY_CACHE) && e->reg.d_state && IBFT_WC > 0;
   int rc_alloc = IBFT_OK;
   do {
     cudaError_t ce = cudaMalloc(&s.d_keys, std::max<size_t>(keys.size(), 6) * 4);
     if (ce == cudaSuccess) ce = cudaMalloc(&s.d_powers, std::max<size_t>(powers.size(), 4) * 8);
     if (ce == cudaSuccess && n) ce = cudaMemcpy(s.d_keys, keys.data(), keys.size() * 4, cudaMemcpyHostToDevice);
     if (ce == cudaSuccess && n) ce = cudaMemcpy(s.d_powers, powers.data(), powers.size() * 8, cudaMemcpyHostToDevice);
-#if IBFT_WC > 0
-    if (ce == cudaSuccess && (e->p.flags & IBFT_FLAG_KEY_CACHE) && n) {
-      ce = cudaMalloc(&s.d_key_state, (size_t)n * 4);
-      if (ce == cudaSuccess) ce = cudaMalloc(&s.d_key_xy, (size_t)n * 64);
-      if (ce == cudaSuccess) ce = cudaMalloc(&s.d_key_tab, (size_t)n * IBFT_KEYTAB_WORDS * 4);  // 136 KiB per validator (comb)
-      if (ce == cudaSuccess) ce = cudaMemset(s.d_key_state, 0, (size_t)n * 4);
-      s.d_learn_count = e->d_learn_counts + table_slot;
-    }
-#endif
+    if (ce == cudaSuccess && registry && n) ce = cudaMalloc(&s.d_key_ref, (size_t)n * 4);
     if (ce != cudaSuccess) {
-      set_err("validator table of %u validators%s: %s", n, (e->p.flags & IBFT_FLAG_KEY_CACHE) ? " with its key registry (136 KiB per validator)" : "",
-              cudaGetErrorString(ce));
+      set_err("validator table of %u validators: %s", n, cudaGetErrorString(ce));
       rc_alloc = ce == cudaErrorMemoryAllocation ? IBFT_ERR_CAPACITY : IBFT_ERR_CUDA;
       (void)cudaGetLastError();
     }
   } while (0);
-  if (rc_alloc != IBFT_OK) {  // the slot keeps its previous table
-    cudaFree(s.d_keys); cudaFree(s.d_powers); cudaFree(s.d_key_state); cudaFree(s.d_key_xy); cudaFree(s.d_key_tab);
-    s = old;
+  // one registry entry per address: the addresses the registry already holds keep their entry (and key); new ones get an entry
+  if (rc_alloc == IBFT_OK && registry && n) rc_alloc = registry_acquire(e, addrs, n, s.key_ref);
+  if (rc_alloc != IBFT_OK) {  // the slot keeps its previous table, the registry its previous references
+    cudaFree(s.d_keys); cudaFree(s.d_powers); cudaFree(s.d_key_ref);
+    s = std::move(old);
     return rc_alloc;
   }
-  if (s.d_learn_count) CU(cudaMemset(s.d_learn_count, 0, 4));  // a new validator set starts with an empty registry (then the carry-over)
+#if IBFT_WC > 0
+  if (s.d_key_ref) {
+    // upload key_ref; entries new to their address are reset to unknown before any kernel can read them through this table
+    cudaError_t ce = cudaMemcpy(s.d_key_ref, s.key_ref.data(), (size_t)n * 4, cudaMemcpyHostToDevice);
+    bool adopt = false;
+    for (uint32_t v = 0; v < n && !adopt; v++) adopt = (s.key_ref[v] & IBFT_KEY_REF_FRESH) != 0;
+    if (ce == cudaSuccess && adopt) {
+      k_adopt_entries<<<(n + 255) / 256, 256>>>(s.d_key_ref, n, e->reg.d_state);
+      e->launches++;
+      ce = cudaGetLastError();
+      if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
+    }
+    for (auto& r : s.key_ref) r &= ~IBFT_KEY_REF_FRESH;
+    if (ce != cudaSuccess) {
+      set_err("validator table of %u validators: key registry entries: %s", n, cudaGetErrorString(ce));
+      registry_release(e, s.key_ref);
+      cudaFree(s.d_keys); cudaFree(s.d_powers); cudaFree(s.d_key_ref);
+      s = std::move(old);
+      return IBFT_ERR_CUDA;
+    }
+  }
+#endif
   s.n = n;
   s.height = height;
   memcpy(s.quorum, q, sizeof s.quorum);
@@ -2057,71 +2192,61 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
   slot_dev sd{};
   sd.keys = s.d_keys;
   sd.powers = s.d_powers;
-  sd.key_state = s.d_key_state;
-  sd.key_xy = s.d_key_xy;
-  sd.key_tab = s.d_key_tab;
-  sd.learn_count = s.d_learn_count;
+  if (s.d_key_ref) {
+    sd.key_ref = s.d_key_ref;
+    sd.key_state = e->reg.d_state;
+    sd.key_xy = e->reg.d_key_xy;
+    sd.key_chunks = e->reg.d_chunks;
+    sd.learn_count = e->reg.d_learn_count;
+  }
   memcpy(sd.quorum, q, sizeof sd.quorum);
   sd.n = n;
   sd.valid = 1;
-#if IBFT_WC > 0
-  if (s.d_key_state) {
-    // carry the keys over from the donor table: the resident table of the greatest height that has a registry (the previous
-    // block, normally) -- this slot's previous content included
-    const slot_dev* donor = nullptr;
-    uint64_t best_h = 0;
-    if (old.valid && old.d_key_state && old.n) { donor = &old_dev; best_h = old.height; }
-    for (uint32_t k = 0; k < e->p.max_table_slots; k++) {
-      const slot_host& o = e->slots[k];
-      if (k == table_slot || !o.valid || !o.d_key_state || !o.n) continue;
-      if (donor == nullptr || o.height > best_h) { donor = &e->slots_shadow[k]; best_h = o.height; }
-    }
-    if (donor != nullptr) {
-      k_carry_keys<<<n, 256>>>(sd, *donor);
-      e->launches++;
-      CU(cudaGetLastError());
-      CU(cudaDeviceSynchronize());
-      CU(cudaMemcpy(&s.built_count, s.d_learn_count, 4, cudaMemcpyDeviceToHost));  // carried keys come with finished tables
-    }
-  }
-#endif
+  // the previous content lets go of its entries: an address no resident table lists any more is forgotten
+  registry_release(e, old.key_ref);
   if (old.d_keys) cudaFree(old.d_keys);
   if (old.d_powers) cudaFree(old.d_powers);
-  cudaFree(old.d_key_state); cudaFree(old.d_key_xy); cudaFree(old.d_key_tab);
+  cudaFree(old.d_key_ref);
   e->slots_shadow[table_slot] = sd;
   CU(cudaMemcpy(e->d_slots + table_slot, &sd, sizeof sd, cudaMemcpyHostToDevice));
   return IBFT_OK;
 }
 
-// Key registry upkeep: for every resident validator table, build the tables of multiples of the keys learned since the last
-// call.  Cheap when nothing is new (one 4-byte read per slot).  ibft_verify_batch / ibft_verify_wait call it on their way out;
-// callers of the device-resident entry points call it between rounds.
+// Key registry upkeep: build the comb tables of the keys learned since the last call -- one claim / build / publish pass over
+// the engine's registry, whichever tables the keys were learned through.  Cheap when nothing is new (one 4-byte read).
+// ibft_verify_batch / ibft_verify_wait call it on their way out; callers of the device-resident entry points call it between
+// rounds.  n_ready_out: the members of the resident tables whose key is known, summed over the tables.
 static int refresh_key_tables_locked(ibft_engine* e, lane* L, uint32_t* n_ready_out) {
   uint32_t total = 0;
 #if IBFT_WC > 0
-  if ((e->p.flags & IBFT_FLAG_KEY_CACHE) && e->d_learn_counts) {
+  if ((e->p.flags & IBFT_FLAG_KEY_CACHE) && e->reg.d_state) {
+    key_registry& R = e->reg;
     std::lock_guard<std::mutex> kl(e->keys_mu);
     CU(cudaSetDevice(e->p.device));
-    CU(cudaMemcpyAsync(e->h_learn_counts, e->d_learn_counts, (size_t)e->p.max_table_slots * 4, cudaMemcpyDeviceToHost, L->stream));
+    CU(cudaMemcpyAsync(R.h_learn_count, R.d_learn_count, 4, cudaMemcpyDeviceToHost, L->stream));
     CU(cudaStreamSynchronize(L->stream));
-    bool built = false;
-    for (uint32_t slot = 0; slot < e->p.max_table_slots; slot++) {
-      slot_host& s = e->slots[slot];
-      if (!s.valid || !s.d_learn_count) continue;
-      uint32_t learned = e->h_learn_counts[slot];
-      if (learned > s.built_count) {
-        k_keytabs_step<<<(s.n + 255) / 256, 256, 0, L->stream>>>(e->d_slots, slot, IBFT_KEY_LEARNED, IBFT_KEY_BUILDING);
-        k_build_keytabs<<<(uint32_t)(((size_t)s.n * IBFT_KEYTAB_POSITIONS + 63) / 64), 64, 0, L->stream>>>(e->d_slots, slot);
-        k_keytabs_step<<<(s.n + 255) / 256, 256, 0, L->stream>>>(e->d_slots, slot, IBFT_KEY_BUILDING, IBFT_KEY_READY);
-        e->launches += 3;
-        CU(cudaGetLastError());
-        s.built_count = learned;
-        built = true;
-      }
-      total += learned;
+    const uint32_t learned = *R.h_learn_count;
+    if (learned != R.built_count && R.used) {
+      // the pass covers [0, used), retired entries included: one that was retired while still LEARNED (a table replaced
+      // before any refresh ran) gets its table built once for nothing -- 17 threads -- and is reset when it is reused
+      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, L->stream>>>(R.d_state, R.used, IBFT_KEY_LEARNED, IBFT_KEY_BUILDING);
+      k_build_keytabs<<<(uint32_t)(((size_t)R.used * IBFT_KEYTAB_POSITIONS + 63) / 64), 64, 0, L->stream>>>(R.d_state, R.d_key_xy,
+                                                                                                          R.d_chunks, R.used);
+      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, L->stream>>>(R.d_state, R.used, IBFT_KEY_BUILDING, IBFT_KEY_READY);
+      e->launches += 3;
+      CU(cudaGetLastError());
+      R.built_count = learned;
+      // the tables are complete before anybody can launch the next round on another stream
+      CU(cudaStreamSynchronize(L->stream));
     }
-    // the tables are complete before anybody can launch the next round on another stream
-    if (built) CU(cudaStreamSynchronize(L->stream));
+    if (n_ready_out && R.used) {
+      std::vector<uint32_t> state(R.used);
+      CU(cudaMemcpyAsync(state.data(), R.d_state, (size_t)R.used * 4, cudaMemcpyDeviceToHost, L->stream));
+      CU(cudaStreamSynchronize(L->stream));
+      for (const slot_host& s : e->slots)
+        if (s.valid)
+          for (uint32_t r : s.key_ref) total += state[r] != IBFT_KEY_UNKNOWN;
+    }
   }
 #endif
   if (n_ready_out) *n_ready_out = total;

@@ -39,7 +39,7 @@ EXPORTS = [
     "ibft_verify_wait", "ibft_bind_groups", "ibft_verify_batch_device", "ibft_quorum_reduce_device", "ibft_quorum_partial_words", "ibft_quorum_mark_device", "ibft_quorum_merge_device", "ibft_quorum_exchange_device",
     "ibft_exchange_alloc", "ibft_exchange_open", "ibft_exchange_close", "ibft_exchange_free", "ibft_exchange_clear",
     "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
-    "ibft_debug_keytab", "ibft_debug_known_handed_back",
+    "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
 ]
 
 
@@ -109,6 +109,7 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.ibft_probe_int_peak.argtypes = [c_void_p, POINTER(c_double), POINTER(c_double)]
     lib.ibft_debug_ctable.argtypes = [c_void_p, c_uint32, c_uint32, c_void_p, POINTER(c_int), POINTER(c_uint32)]
     lib.ibft_debug_keytab.argtypes = [c_void_p, c_uint32, c_uint32, c_uint32, c_uint32, c_void_p, POINTER(c_uint32), c_void_p]
+    lib.ibft_debug_key_registry.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32), POINTER(c_uint64)]
     lib.ibft_debug_known_handed_back.argtypes = [c_void_p, POINTER(c_uint32)]
     lib.ibft_debug_op.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_uint32]
     if path is None:
@@ -395,6 +396,13 @@ class Engine:
         self._check(self.lib.ibft_debug_keytab(self.handle, slot, validator, first, count, _ptr(out) if count else None, ctypes.byref(st),
                                                _ptr(key)))
         return int(st.value), key, out
+
+    def key_registry(self) -> tuple[int, int, int]:
+        """The engine's key registry: (entries in use = distinct addresses of the resident tables, entries whose comb table is
+        built, bytes of comb-table chunks allocated)."""
+        used, ready, nbytes = c_uint32(), c_uint32(), c_uint64()
+        self._check(self.lib.ibft_debug_key_registry(self.handle, ctypes.byref(used), ctypes.byref(ready), ctypes.byref(nbytes)))
+        return int(used.value), int(ready.value), int(nbytes.value)
 
     def known_handed_back(self) -> int:
         """items the known-key pass of the most recent completed host-buffer call left to the recover pass"""

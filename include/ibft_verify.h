@@ -144,11 +144,15 @@ typedef struct ibft_engine_params {
  * signature by that validator; once its comb table is built (m * 2^(8j) * Q for 17 positions j and m = 1..128), later signatures
  * by the same validator are VERIFIED against the key -- 51 mixed additions, no doubling, no square root, no per-signature table,
  * no address hash -- instead of recovered.  A signature the verification rejects is re-checked by the recover path, so every
- * verdict is the recover path's verdict.  Costs 136 KiB of device memory per validator and table slot (1.39 GB for a
- * 10,000-validator set; ibft_set_validators fails with IBFT_ERR_CAPACITY when the device cannot hold it, and the slot keeps its
- * previous table).  A key belongs to an address, not to a height: ibft_set_validators carries the finished tables over, by
- * address, from the slot's previous content -- or, when the slot was empty, from the resident table of the greatest height --
- * so a chain that moves to the next height with (mostly) the same validators never recovers their signatures again. */
+ * verdict is the recover path's verdict.  A key belongs to an address, not to a height: the engine keeps ONE registry entry per
+ * distinct address that appears in at least one resident validator table -- 64 bytes of key, a state word and the 136 KiB comb
+ * table (1.39 GB for a 10,000-validator set, however many resident heights list it).  A key learned through any table serves
+ * every table that lists the address, including tables set earlier, so a chain that moves to the next height with (mostly) the
+ * same validators never recovers their signatures again.  An entry is retired when no resident table lists its address any
+ * more: a validator that leaves every table and later rejoins is learned again.  The engine reserves the state and key of
+ * (max_table_slots + 1) x max_validators entries at creation (68 bytes each) and allocates comb tables in chunks of 256
+ * entries (34 MiB) as new addresses arrive; ibft_set_validators fails with IBFT_ERR_CAPACITY when the registry cannot grow to
+ * hold its table's new addresses, and the slot keeps its previous table. */
 #define IBFT_FLAG_KEY_CACHE 1u
 
 typedef struct ibft_device_info {
@@ -322,8 +326,8 @@ int ibft_sign_batch(ibft_engine* e, const uint8_t* privkeys, const uint8_t* dige
 #define IBFT_PATH_QSPLIT 4
 int ibft_set_recover_path(ibft_engine* e, int path);
 
-/* Key registry (IBFT_FLAG_KEY_CACHE): build the tables of the keys learned since the last call; *n_keys_out = keys known
- * over all resident tables.  ibft_verify_batch / ibft_verify_wait do this on their way out; users of the device-resident
+/* Key registry (IBFT_FLAG_KEY_CACHE): build the tables of the keys learned since the last call; *n_keys_out = the members of
+ * the resident tables whose key is known, summed over the tables (an address listed by two tables counts twice).  ibft_verify_batch / ibft_verify_wait do this on their way out; users of the device-resident
  * entry points call it between rounds.  No-op (0 keys) when the flag is off. */
 int ibft_refresh_key_tables(ibft_engine* e, uint32_t* n_keys_out);
 
@@ -369,9 +373,13 @@ int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count, uint8_t* o
 /* Key registry entry of validator `validator` (validator-index order) of a table slot: *state_out = 0 unknown, 1 learned,
  * 2 comb table built; key_out (64 bytes) = the learned affine key, x then y as 8 little-endian words; out = `count` comb
  * entries starting at `first` in the format of ibft_debug_ctable, entry j * 128 + m - 1 = m * 2^(8j) * Q (j = 0..16,
- * m = 1..128).  Any output may be NULL.  Waits for the device. */
+ * m = 1..128).  Read through the table's reference into the engine's registry.  Any output may be NULL.  Waits for the device. */
 int ibft_debug_keytab(ibft_engine* e, uint32_t table_slot, uint32_t validator, uint32_t first, uint32_t count, uint8_t* out,
                       uint32_t* state_out, uint8_t* key_out);
+/* The key registry as a whole: *entries_in_use = distinct addresses of the resident tables, *entries_ready = those of them
+ * whose comb table is built, *bytes_reserved = bytes of comb-table chunks allocated so far (whole chunks of 256 x 136 KiB).
+ * Any output may be NULL.  IBFT_ERR_INVALID_ARG without IBFT_FLAG_KEY_CACHE.  Waits for the device. */
+int ibft_debug_key_registry(ibft_engine* e, uint32_t* entries_in_use, uint32_t* entries_ready, uint64_t* bytes_reserved);
 /* Number of items the known-key pass (IBFT_FLAG_KEY_CACHE) of the most recent completed host-buffer call left to the recover
  * pass -- signatures of member signers whose key is not known yet or that the verification against the key rejected (the
  * chain + helper form also settles out-of-range (r, s, v) itself).  0 when the call took no known-key pass.  Same "most recent
