@@ -25,6 +25,7 @@
 #include "../../include/ibft_verify.h"
 #include "verify_core.cuh"
 #include "debug_arith.cuh"
+#include "key_budget.hpp"
 
 #include "secp_gtable.inc"
 
@@ -62,17 +63,31 @@ struct slot_dev {
   uint32_t* const* key_chunks; // comb tables, IBFT_KEY_CHUNK entries per chunk of IBFT_KEY_CHUNK x IBFT_KEYTAB_WORDS words; per
                                // entry 17 comb positions x 128 entries x 16 words, affine (build_keytab_pos)
   uint32_t* learn_count;       // number of keys learned so far, engine-wide (the host compares it with the number it built)
+  // bounded registry (ibft_set_key_table_budget; both nullptr otherwise): key_chunks is then a pool of table slots
+  const uint32_t* key_tab;     // per entry: its table slot, or IBFT_KEY_NO_TAB (nullptr: entry r's table is slot r)
+  uint8_t* key_used;           // per entry: set by the known-key pass on every lookup; read and cleared at reclaim points
 };
 #define IBFT_KEY_UNKNOWN 0u
 #define IBFT_KEY_LEARNED 1u
 #define IBFT_KEY_READY 2u
 #define IBFT_KEY_BUILDING 3u  // claimed by a table-build pass (refresh_key_tables_locked)
+#define IBFT_KEY_EVICTED 4u   // bounded registry: key known, no table slot (every kernel treats it as LEARNED)
+#define IBFT_KEY_NO_TAB 0xFFFFFFFFu
 #define IBFT_KEY_CHUNK 256u   // registry entries per comb-table chunk (34 MiB): the pool grows by whole chunks, never by copying
 #define IBFT_KEY_REF_FRESH 0x80000000u  // key_ref mark of an entry new to its address (k_adopt_entries); entries are < 2^31
 
-// comb table of registry entry r
-__device__ __forceinline__ uint32_t* key_table_of(uint32_t* const* __restrict__ chunks, uint32_t r) {
-  return chunks[r / IBFT_KEY_CHUNK] + (size_t)(r % IBFT_KEY_CHUNK) * IBFT_KEYTAB_WORDS;
+// comb table in slot t
+__device__ __forceinline__ uint32_t* key_table_of(uint32_t* const* __restrict__ chunks, uint32_t t) {
+  return chunks[t / IBFT_KEY_CHUNK] + (size_t)(t % IBFT_KEY_CHUNK) * IBFT_KEYTAB_WORDS;
+}
+// known-key pass: the table slot of registry entry r, and whether the table can be used.  The state and the slot depend only on
+// r and are loaded side by side; a bounded registry also records the use.
+__device__ __forceinline__ uint32_t key_lookup(const slot_dev& s, uint32_t r, bool* ready) {
+  const uint32_t st = s.key_state[r];
+  const uint32_t t = s.key_tab != nullptr ? s.key_tab[r] : r;
+  if (s.key_used != nullptr) s.key_used[r] = 1;
+  *ready = st == IBFT_KEY_READY && t != IBFT_KEY_NO_TAB;
+  return t;
 }
 
 __device__ __forceinline__ uint32_t bswap32(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
@@ -327,16 +342,13 @@ k_verify_known(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
     uint32_t slot = IBFT_NO_TABLE;
     const bool member = have && group_member(groups, n_groups, slots, n_slots, it.group, ri.signer, &v, &slot);
     if (member) {
-      uint32_t r = 0;  // registry entry of the signer's address
+      uint32_t t = 0;  // table slot of the signer's registry entry
       bool ready = false;
-      if (v >= 0 && slots[slot].key_ref != nullptr) {
-        r = slots[slot].key_ref[v];
-        ready = slots[slot].key_state[r] == IBFT_KEY_READY;
-      }
+      if (v >= 0 && slots[slot].key_ref != nullptr) t = key_lookup(slots[slot], slots[slot].key_ref[v], &ready);
       if (ready) {
         gtab_view G{g_gtable};
         G.comb = ctable;
-        gtab_view Qt{key_table_of(slots[slot].key_chunks, r)};
+        gtab_view Qt{key_table_of(slots[slot].key_chunks, t)};
         ok = ecdsa_verify_known(ri, G, Qt);
       }
       if (ok) record_vote(sink, groups, it.group, v);
@@ -702,7 +714,8 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
 // valid (malformed, out of range, unknown group, signer not in the set) are settled here.  A round in which every signature
 // verifies (the normal case of consensus) never runs a second chain.
 // ------------------------------------------------------------------------------------------------------------
-#define IBFT_VSLOT_WORDS 29   // [0..26] as IBFT_SLOT_WORDS, [27] validator index | slot << 16 of the signer, [28] phase-2 flags
+#define IBFT_VSLOT_WORDS 30   // [0..26] as IBFT_SLOT_WORDS, [27] validator index | slot << 16 of the signer, [28] phase-2 flags,
+                              // [29] table slot of the signer's key
 #define IBFT_VSPLIT_SMEM ((IBFT_SPLIT_SIGS * (IBFT_ITEM_ROW_WORDS + IBFT_VSLOT_WORDS)) * 4)
 #define IBFT_VF_VALID 1u      // digits of u2 posted: the chain runs
 #define IBFT_VF_NEG0 2u
@@ -759,7 +772,9 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
         int v = -1;
         uint32_t slot = IBFT_NO_TABLE;
         if (have && group_member(groups, n_groups, slots, n_slots, it.group, ri.signer, &v, &slot)) {
-          const bool ready = v >= 0 && slots[slot].key_ref != nullptr && slots[slot].key_state[slots[slot].key_ref[v]] == IBFT_KEY_READY;
+          bool ready = false;
+          uint32_t t = 0;
+          if (v >= 0 && slots[slot].key_ref != nullptr) t = key_lookup(slots[slot], slots[slot].key_ref[v], &ready);
           if (ready) {
             sc r = sc_from_be(ri.r), sv = sc_from_be(ri.s);
 #pragma unroll
@@ -768,6 +783,7 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
               s_slot[(19 + k) * S + i] = r.v[k];
             }
             s_slot[27 * S + i] = (uint32_t)v | (slot << 16);
+            s_slot[29 * S + i] = t;
             okmask |= 1u << p;
           } else {
             flags = IBFT_VF_RECOVER;               // member whose key is not known (or no table: v < 0): the recover path decides
@@ -874,8 +890,7 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
     dg.kneg[0] = flags & IBFT_VF_NEG0; dg.kneg[1] = flags & IBFT_VF_NEG1;
     dg.kneg[2] = dg.kneg[3] = false;
     vslot = s_slot[27 * S + i];
-    const slot_dev& sd = slots[vslot >> 16];
-    gtab_view Qt{key_table_of(sd.key_chunks, sd.key_ref[vslot & 0xFFFFu])};
+    gtab_view Qt{key_table_of(slots[vslot >> 16].key_chunks, s_slot[29 * S + i])};
     acc = ecmult_streams_known(dg, G, Qt, false);
   }
   named_bar_sync(1 + IBFT_SPLIT_CHAINS + warp, 64);  // u1*G is posted
@@ -1394,10 +1409,10 @@ k_build_ctable(uint32_t* __restrict__ out) {  // blockIdx.y = comb position: ent
 // key registry: comb tables for every registry entry whose key has been learned but whose table is missing.  One thread per
 // (entry, comb position): 8*pos doublings, 128 additions and 128 inversions each -- a whole 10k-validator set (170,000
 // threads, 21.8 M table entries, 1.39 GB) is built once per engine, whatever the number of resident heights that list it;
-// k_keytabs_step then publishes the tables.
+// k_keytabs_step then publishes the tables.  tab: the bounded registry's table slot of each entry (nullptr: slot r).
 __global__ void __launch_bounds__(64)
-k_build_keytabs(const uint32_t* __restrict__ state, const uint32_t* __restrict__ key_xy, uint32_t* const* __restrict__ chunks,
-                uint32_t n_entries) {
+k_build_keytabs(const uint32_t* __restrict__ state, const uint32_t* __restrict__ key_xy, const uint32_t* __restrict__ tab,
+                uint32_t* const* __restrict__ chunks, uint32_t n_entries) {
   const uint32_t t = blockIdx.x * 64 + threadIdx.x;
   const uint32_t r = t / IBFT_KEYTAB_POSITIONS, pos = t % IBFT_KEYTAB_POSITIONS;
   if (r >= n_entries || state[r] != IBFT_KEY_BUILDING) return;
@@ -1407,26 +1422,29 @@ k_build_keytabs(const uint32_t* __restrict__ state, const uint32_t* __restrict__
     Q.x.v[i] = key_xy[16 * (size_t)r + i];
     Q.y.v[i] = key_xy[16 * (size_t)r + 8 + i];
   }
-  build_keytab_pos(Q, (int)pos, key_table_of(chunks, r) + (size_t)pos * IBFT_KEYTAB_ENTRIES * IBFT_GTAB_ENTRY_WORDS);
+  const uint32_t slot = tab != nullptr ? tab[r] : r;
+  build_keytab_pos(Q, (int)pos, key_table_of(chunks, slot) + (size_t)pos * IBFT_KEYTAB_ENTRIES * IBFT_GTAB_ENTRY_WORDS);
 }
 // state steps around the build, one launch each on the same stream: LEARNED -> BUILDING (claim: the set of entries this pass
 // builds is fixed here -- recover kernels of another lane may keep learning keys meanwhile, those wait for the next pass),
-// BUILDING -> READY (publish)
+// BUILDING -> READY (publish).  A bounded registry (tab != nullptr) claims only the entries that hold a table slot.
 __global__ void __launch_bounds__(256)
-k_keytabs_step(uint32_t* __restrict__ state, uint32_t n_entries, uint32_t from, uint32_t to) {
+k_keytabs_step(uint32_t* __restrict__ state, const uint32_t* __restrict__ tab, uint32_t n_entries, uint32_t from, uint32_t to) {
   const uint32_t r = blockIdx.x * 256 + threadIdx.x;
-  if (r < n_entries && state[r] == from) state[r] = to;
+  if (r < n_entries && state[r] == from && (tab == nullptr || tab[r] != IBFT_KEY_NO_TAB)) state[r] = to;
 }
 // ibft_set_validators: the new table's key_ref arrives with bit 31 set on the entries just given to an address the registry
 // did not hold -- a fresh or a retired entry, whose state (and key) may still be that of another address.  Reset those to
-// unknown, then clear the mark.  Runs while every lane is held and the device is idle, before the table is published.
+// unknown (and, in a bounded registry, without a table slot), then clear the mark.  Runs while every lane is held and the
+// device is idle, before the table is published.
 __global__ void __launch_bounds__(256)
-k_adopt_entries(uint32_t* __restrict__ key_ref, uint32_t n, uint32_t* __restrict__ state) {
+k_adopt_entries(uint32_t* __restrict__ key_ref, uint32_t n, uint32_t* __restrict__ state, uint32_t* __restrict__ tab) {
   const uint32_t v = blockIdx.x * 256 + threadIdx.x;
   if (v >= n) return;
   const uint32_t r = key_ref[v];
   if (r & IBFT_KEY_REF_FRESH) {
     state[r & ~IBFT_KEY_REF_FRESH] = IBFT_KEY_UNKNOWN;
+    if (tab != nullptr) tab[r & ~IBFT_KEY_REF_FRESH] = IBFT_KEY_NO_TAB;
     key_ref[v] = r & ~IBFT_KEY_REF_FRESH;
   }
 }
@@ -1642,6 +1660,16 @@ struct key_registry {
   std::vector<addr20> addr_of;           // address of each entry in use
   std::vector<uint32_t> refs;            // reference count of each entry
   std::vector<uint32_t> free_list;       // retired entries, reused before the high-water mark moves
+  // Bounded registry (ibft_set_key_table_budget, for the rest of the engine's life): `chunks` is a pool of budget.max_tables
+  // table slots, chunk i holding chunk_tables[i] of them (0: not allocated yet; the last one may be partial), and an entry
+  // holds a slot or none (budget.table, mirrored in d_tab).  Slots are taken away only at reclaim points (every lane held,
+  // device drained); the per-call refresh only hands out free ones.
+  bool bounded = false;
+  ibft::key_budget budget;
+  std::vector<uint32_t> chunk_tables;
+  uint32_t* d_tab = nullptr;             // capacity words
+  uint8_t* d_used = nullptr;             // capacity bytes: used flags of the known-key pass
+  bool build_due = false;                // entries admitted at the last reclaim point wait for the next refresh
 };
 
 struct pending_call {
@@ -1766,6 +1794,7 @@ static void engine_free(ibft_engine* e) {
   for (auto& L : e->lanes) lane_free(&L);
   cudaFree(e->d_ctable);
   for (auto c : e->reg.chunks) cudaFree(c);
+  cudaFree(e->reg.d_tab); cudaFree(e->reg.d_used);
   cudaFree(e->reg.d_state); cudaFree(e->reg.d_key_xy); cudaFree(e->reg.d_chunks); cudaFree(e->reg.d_learn_count);
   cudaFreeHost(e->reg.h_learn_count);
   cudaFree(e->d_slots);
@@ -1904,12 +1933,17 @@ extern "C" int ibft_debug_keytab(ibft_engine* e, uint32_t table_slot, uint32_t v
     return IBFT_ERR_INVALID_ARG;
   }
   const uint32_t r = s.key_ref[validator];
+  const uint32_t t = e->reg.bounded ? e->reg.budget.table[r] : r;
   CU(cudaSetDevice(e->p.device));
   CU(cudaDeviceSynchronize());
-  if (state_out) CU(cudaMemcpy(state_out, e->reg.d_state + r, 4, cudaMemcpyDeviceToHost));
+  if (state_out) {
+    CU(cudaMemcpy(state_out, e->reg.d_state + r, 4, cudaMemcpyDeviceToHost));
+    if (*state_out == IBFT_KEY_EVICTED) *state_out = IBFT_KEY_LEARNED;
+  }
   if (key_out) CU(cudaMemcpy(key_out, e->reg.d_key_xy + 16 * (size_t)r, 64, cudaMemcpyDeviceToHost));
   if (count) {
-    const uint32_t* tab = e->reg.chunks[r / IBFT_KEY_CHUNK] + (size_t)(r % IBFT_KEY_CHUNK) * IBFT_KEYTAB_WORDS;
+    if (t == IBFT_KEY_NO_TAB) { set_err("validator %u has no comb table", validator); return IBFT_ERR_INVALID_ARG; }
+    const uint32_t* tab = e->reg.chunks[t / IBFT_KEY_CHUNK] + (size_t)(t % IBFT_KEY_CHUNK) * IBFT_KEYTAB_WORDS;
     CU(cudaMemcpy(out, tab + (size_t)first * IBFT_GTAB_ENTRY_WORDS, (size_t)count * 64, cudaMemcpyDeviceToHost));
   }
   return IBFT_OK;
@@ -1935,7 +1969,9 @@ extern "C" int ibft_debug_key_registry(ibft_engine* e, uint32_t* entries_in_use,
   for (const auto& kv : R.by_addr) ready += state[kv.second] == IBFT_KEY_READY;
   if (entries_in_use) *entries_in_use = (uint32_t)R.by_addr.size();
   if (entries_ready) *entries_ready = ready;
-  if (bytes_reserved) *bytes_reserved = (uint64_t)R.chunks.size() * IBFT_KEY_CHUNK * IBFT_KEYTAB_WORDS * 4;
+  uint64_t tables = (uint64_t)R.chunks.size() * IBFT_KEY_CHUNK;
+  if (R.bounded) { tables = 0; for (uint32_t c : R.chunk_tables) tables += c; }
+  if (bytes_reserved) *bytes_reserved = tables * IBFT_KEYTAB_WORDS * 4;
   return IBFT_OK;
 }
 
@@ -2041,7 +2077,7 @@ static int registry_acquire(ibft_engine* e, const uint8_t* addrs, uint32_t n, st
     }
   }
   cudaError_t ce = cudaSuccess;
-  const size_t need = ((size_t)R.used + IBFT_KEY_CHUNK - 1) / IBFT_KEY_CHUNK;
+  const size_t need = R.bounded ? 0 : ((size_t)R.used + IBFT_KEY_CHUNK - 1) / IBFT_KEY_CHUNK;  // a bounded pool grows lazily
   while (R.used <= R.capacity && R.chunks.size() < need) {
     uint32_t* c = nullptr;
     ce = cudaMalloc(&c, (size_t)IBFT_KEY_CHUNK * IBFT_KEYTAB_WORDS * 4);
@@ -2065,6 +2101,7 @@ static int registry_acquire(ibft_engine* e, const uint8_t* addrs, uint32_t n, st
     return ce == cudaSuccess || ce == cudaErrorMemoryAllocation ? IBFT_ERR_CAPACITY : IBFT_ERR_CUDA;
   }
   for (uint32_t v = 0; v < n; v++) R.refs[refs[v] & ~IBFT_KEY_REF_FRESH]++;
+  if (R.bounded) R.budget.ensure(R.used);
   return IBFT_OK;
 }
 // ... and one reference less per row of a table being dropped; an entry no resident table lists any more is retired
@@ -2077,6 +2114,135 @@ static void registry_release(ibft_engine* e, const std::vector<uint32_t>& refs) 
     }
   }
 }
+
+#if IBFT_WC > 0
+// Bounded registry: tables chunk i holds under a budget of m table slots (the last chunk may be partial)
+static uint32_t pool_chunk_tables(uint32_t m, size_t i) {
+  const size_t lo = i * IBFT_KEY_CHUNK;
+  return lo >= m ? 0u : (uint32_t)std::min<size_t>(IBFT_KEY_CHUNK, m - lo);
+}
+// make sure the chunk of table slot t is allocated (lazily, at its size under the current budget); false when it cannot be
+static bool pool_reserve(key_registry& R, uint32_t t, bool* grew) {
+  const size_t i = t / IBFT_KEY_CHUNK;
+  if (R.chunk_tables[i]) return true;
+  const uint32_t k = pool_chunk_tables(R.budget.max_tables, i);
+  uint32_t* c = nullptr;
+  if (cudaMalloc(&c, (size_t)k * IBFT_KEYTAB_WORDS * 4) != cudaSuccess) { (void)cudaGetLastError(); return false; }
+  R.chunks[i] = c;
+  R.chunk_tables[i] = k;
+  *grew = true;
+  return true;
+}
+static uint32_t* pool_table(key_registry& R, uint32_t t) {
+  return R.chunks[t / IBFT_KEY_CHUNK] + (size_t)(t % IBFT_KEY_CHUNK) * IBFT_KEYTAB_WORDS;
+}
+
+// A reclaim point of the bounded registry (caller holds every lane, device drained): read and clear the used flags, rank the
+// entries with a known key (key_budget.hpp), evict, move the kept tables that sit at or above the (new) budget down, resize or
+// free the chunks the new budget does not cover, and give slots to the admitted entries (built by the next refresh).  A chunk
+// that cannot be allocated costs tables, never an error: the entries concerned keep their key and take the recover path.
+// Invariant: an entry is READY only while its slot holds the comb table of its own current key.
+static int budget_reclaim(ibft_engine* e, uint32_t new_max) {
+  key_registry& R = e->reg;
+  ibft::key_budget& B = R.budget;
+  const uint32_t n = R.used;
+  std::vector<uint32_t> state(n);
+  std::vector<uint8_t> used(n), listed(n), known(n), addr((size_t)n * 20);
+  if (n) {
+    CU(cudaMemcpy(state.data(), R.d_state, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(used.data(), R.d_used, n, cudaMemcpyDeviceToHost));
+    CU(cudaMemset(R.d_used, 0, n));
+  }
+  for (uint32_t r = 0; r < n; r++) {
+    listed[r] = R.refs[r] > 0;
+    known[r] = state[r] == IBFT_KEY_LEARNED || state[r] == IBFT_KEY_READY || state[r] == IBFT_KEY_EVICTED;
+    memcpy(&addr[20 * (size_t)r], R.addr_of[r].b, 20);
+  }
+  const ibft::key_budget::plan p = B.reclaim(n, listed.data(), known.data(), used.data(), addr.data(), new_max);
+  std::vector<uint32_t> lost;  // entries whose table could not be placed
+  bool grew = false;
+  for (const auto& mv : p.moves) {
+    if (!pool_reserve(R, mv.to, &grew)) { lost.push_back(mv.entry); continue; }
+    CU(cudaMemcpy(pool_table(R, mv.to), pool_table(R, mv.from), (size_t)IBFT_KEYTAB_WORDS * 4, cudaMemcpyDeviceToDevice));
+  }
+  for (uint32_t r : lost) B.drop(r);
+  lost.clear();
+  // chunks whose size changes with the budget: freed when it no longer covers them, otherwise reallocated at the new size with
+  // the tables they keep (only tables below the new budget are live by now)
+  const size_t n_chunks = R.chunks.size();
+  for (size_t i = 0; i < n_chunks; i++) {
+    const uint32_t have = R.chunk_tables[i], want = pool_chunk_tables(new_max, i);
+    if (!have || have == want) continue;
+    uint32_t* c = nullptr;
+    if (want && cudaMalloc(&c, (size_t)want * IBFT_KEYTAB_WORDS * 4) == cudaSuccess) {
+      CU(cudaMemcpy(c, R.chunks[i], (size_t)std::min(have, want) * IBFT_KEYTAB_WORDS * 4, cudaMemcpyDeviceToDevice));
+    } else {
+      (void)cudaGetLastError();
+      c = nullptr;
+      for (uint32_t t = (uint32_t)(i * IBFT_KEY_CHUNK); t < i * IBFT_KEY_CHUNK + have && t < B.owner.size(); t++)
+        if (B.owner[t] != ibft::kNoTable) lost.push_back(B.owner[t]);
+    }
+    CU(cudaFree(R.chunks[i]));
+    R.chunks[i] = c;
+    R.chunk_tables[i] = c ? want : 0u;
+  }
+  for (uint32_t r : lost) B.drop(r);
+  for (uint32_t r : p.admitted) {
+    const uint32_t t = B.table[r];
+    if (t != ibft::kNoTable && !pool_reserve(R, t, &grew)) B.drop(r);
+  }
+  // states: a slot that holds the entry's table stays READY, an admitted one is LEARNED (built by the next refresh), and every
+  // other known key of a listed entry is EVICTED -- so LEARNED without a slot means "learned since this reclaim point"
+  R.build_due = false;
+  for (uint32_t r = 0; r < n; r++) {
+    if (!listed[r] || !known[r]) continue;
+    if (B.table[r] == ibft::kNoTable) state[r] = IBFT_KEY_EVICTED;
+    else if (state[r] != IBFT_KEY_READY) { state[r] = IBFT_KEY_LEARNED; R.build_due = true; }
+  }
+  if (n) {
+    CU(cudaMemcpy(R.d_tab, B.table.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(R.d_state, state.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
+  }
+  CU(cudaMemcpy(R.d_chunks, R.chunks.data(), R.chunks.size() * sizeof(uint32_t*), cudaMemcpyHostToDevice));
+  return IBFT_OK;
+}
+
+// Switch the engine to a bounded registry (every lane held, device drained).  The tables built so far stay where they are:
+// entry r's table is slot r of the pool, then the first reclaim point brings the pool to its budget.
+static int budget_enable(ibft_engine* e) {
+  key_registry& R = e->reg;
+  const size_t n_chunks = ((size_t)R.capacity + IBFT_KEY_CHUNK - 1) / IBFT_KEY_CHUNK;
+  uint32_t* d_tab = nullptr;
+  uint8_t* d_used = nullptr;
+  cudaError_t ce = cudaMalloc(&d_tab, std::max<size_t>(R.capacity, 1) * 4);
+  if (ce == cudaSuccess) ce = cudaMalloc(&d_used, std::max<size_t>(R.capacity, 1));
+  if (ce == cudaSuccess) ce = cudaMemset(d_used, 0, std::max<size_t>(R.capacity, 1));
+  if (ce != cudaSuccess) {
+    cudaFree(d_tab); cudaFree(d_used);
+    (void)cudaGetLastError();
+    set_err("key table budget: %s", cudaGetErrorString(ce));
+    return ce == cudaErrorMemoryAllocation ? IBFT_ERR_CAPACITY : IBFT_ERR_CUDA;
+  }
+  R.d_tab = d_tab;
+  R.d_used = d_used;
+  std::vector<uint32_t> state(R.used);
+  if (R.used) CU(cudaMemcpy(state.data(), R.d_state, (size_t)R.used * 4, cudaMemcpyDeviceToHost));
+  std::vector<uint8_t> holds(R.chunks.size() * IBFT_KEY_CHUNK, 0);
+  for (uint32_t r = 0; r < R.used; r++) holds[r] = state[r] == IBFT_KEY_READY && R.refs[r] > 0;
+  R.budget.adopt_identity(R.used, holds);
+  R.chunk_tables.assign(n_chunks, 0);
+  for (size_t i = 0; i < R.chunks.size(); i++) R.chunk_tables[i] = IBFT_KEY_CHUNK;
+  R.chunks.resize(n_chunks, nullptr);
+  R.bounded = true;
+  for (size_t k = 0; k < e->slots.size(); k++) {
+    if (!e->slots[k].d_key_ref) continue;
+    e->slots_shadow[k].key_tab = R.d_tab;
+    e->slots_shadow[k].key_used = R.d_used;
+    CU(cudaMemcpy(e->d_slots + k, &e->slots_shadow[k], sizeof(slot_dev), cudaMemcpyHostToDevice));
+  }
+  return IBFT_OK;
+}
+#endif
 
 extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t height, const uint8_t* addrs,
                                    const uint8_t* powers_be, uint32_t n) {
@@ -2170,7 +2336,7 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
     bool adopt = false;
     for (uint32_t v = 0; v < n && !adopt; v++) adopt = (s.key_ref[v] & IBFT_KEY_REF_FRESH) != 0;
     if (ce == cudaSuccess && adopt) {
-      k_adopt_entries<<<(n + 255) / 256, 256>>>(s.d_key_ref, n, e->reg.d_state);
+      k_adopt_entries<<<(n + 255) / 256, 256>>>(s.d_key_ref, n, e->reg.d_state, e->reg.bounded ? e->reg.d_tab : nullptr);
       e->launches++;
       ce = cudaGetLastError();
       if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
@@ -2198,6 +2364,7 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
     sd.key_xy = e->reg.d_key_xy;
     sd.key_chunks = e->reg.d_chunks;
     sd.learn_count = e->reg.d_learn_count;
+    if (e->reg.bounded) { sd.key_tab = e->reg.d_tab; sd.key_used = e->reg.d_used; }
   }
   memcpy(sd.quorum, q, sizeof sd.quorum);
   sd.n = n;
@@ -2209,6 +2376,9 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
   cudaFree(old.d_key_ref);
   e->slots_shadow[table_slot] = sd;
   CU(cudaMemcpy(e->d_slots + table_slot, &sd, sizeof sd, cudaMemcpyHostToDevice));
+#if IBFT_WC > 0
+  if (e->reg.bounded) return budget_reclaim(e, e->reg.budget.max_tables);  // entries retired here give their slots back
+#endif
   return IBFT_OK;
 }
 
@@ -2226,13 +2396,40 @@ static int refresh_key_tables_locked(ibft_engine* e, lane* L, uint32_t* n_ready_
     CU(cudaMemcpyAsync(R.h_learn_count, R.d_learn_count, 4, cudaMemcpyDeviceToHost, L->stream));
     CU(cudaStreamSynchronize(L->stream));
     const uint32_t learned = *R.h_learn_count;
-    if (learned != R.built_count && R.used) {
+    bool build = learned != R.built_count && R.used;
+    if (R.bounded && build) {
+      // the other lane's kernels may be running: only FREE slots are handed out here, to the keys learned since the last
+      // reclaim point (LEARNED without a slot), in ascending address order
+      std::vector<uint32_t> state(R.used), fresh;
+      CU(cudaMemcpyAsync(state.data(), R.d_state, (size_t)R.used * 4, cudaMemcpyDeviceToHost, L->stream));
+      CU(cudaStreamSynchronize(L->stream));
+      for (uint32_t r = 0; r < R.used; r++)
+        if (state[r] == IBFT_KEY_LEARNED && R.refs[r] > 0 && R.budget.table[r] == ibft::kNoTable) fresh.push_back(r);
+      std::sort(fresh.begin(), fresh.end(), [&](uint32_t a, uint32_t b) { return memcmp(R.addr_of[a].b, R.addr_of[b].b, 20) < 0; });
+      bool grew = false, assigned = false;
+      for (uint32_t r : fresh) {
+        const uint32_t t = R.budget.take_free(r);
+        if (t == ibft::kNoTable) break;
+        if (!pool_reserve(R, t, &grew)) { R.budget.drop(r); break; }  // the pool cannot grow: builds stop at what it holds
+        CU(cudaMemcpyAsync(R.d_tab + r, &R.budget.table[r], 4, cudaMemcpyHostToDevice, L->stream));
+        assigned = true;
+      }
+      if (grew) CU(cudaMemcpyAsync(R.d_chunks, R.chunks.data(), R.chunks.size() * sizeof(uint32_t*), cudaMemcpyHostToDevice, L->stream));
+      CU(cudaStreamSynchronize(L->stream));  // the host copies above read pageable memory that changes on the next call
+      R.built_count = learned;
+      build = assigned;
+    }
+    if (R.bounded && R.build_due) build = true;
+    if (build) {
       // the pass covers [0, used), retired entries included: one that was retired while still LEARNED (a table replaced
-      // before any refresh ran) gets its table built once for nothing -- 17 threads -- and is reset when it is reused
-      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, L->stream>>>(R.d_state, R.used, IBFT_KEY_LEARNED, IBFT_KEY_BUILDING);
+      // before any refresh ran) gets its table built once for nothing -- 17 threads -- and is reset when it is reused.  A
+      // bounded registry builds only the entries that hold a slot.
+      const uint32_t* tab = R.bounded ? R.d_tab : nullptr;
+      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, L->stream>>>(R.d_state, tab, R.used, IBFT_KEY_LEARNED, IBFT_KEY_BUILDING);
       k_build_keytabs<<<(uint32_t)(((size_t)R.used * IBFT_KEYTAB_POSITIONS + 63) / 64), 64, 0, L->stream>>>(R.d_state, R.d_key_xy,
-                                                                                                          R.d_chunks, R.used);
-      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, L->stream>>>(R.d_state, R.used, IBFT_KEY_BUILDING, IBFT_KEY_READY);
+                                                                                                          tab, R.d_chunks, R.used);
+      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, L->stream>>>(R.d_state, tab, R.used, IBFT_KEY_BUILDING, IBFT_KEY_READY);
+      R.build_due = false;
       e->launches += 3;
       CU(cudaGetLastError());
       R.built_count = learned;
@@ -2255,9 +2452,40 @@ static int refresh_key_tables_locked(ibft_engine* e, lane* L, uint32_t* n_ready_
 extern "C" int ibft_refresh_key_tables(ibft_engine* e, uint32_t* n_keys_out) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
-  std::lock_guard<std::mutex> lk(L->mu);
+  std::unique_lock<std::mutex> lk(L->mu), lk1;
   if (L->pending.active) { set_err("a submitted call is still pending"); return IBFT_ERR_INVALID_ARG; }
+#if IBFT_WC > 0
+  if (e->reg.bounded) {  // a reclaim point: every lane (in index order), device drained
+    lk1 = std::unique_lock<std::mutex>(e->lanes[1].mu);
+    CU(cudaSetDevice(e->p.device));
+    CU(cudaDeviceSynchronize());
+    int rc = budget_reclaim(e, e->reg.budget.max_tables);
+    if (rc != IBFT_OK) return rc;
+  }
+#endif
   return refresh_key_tables_locked(e, L, n_keys_out);
+}
+
+extern "C" int ibft_set_key_table_budget(ibft_engine* e, uint32_t max_tables) {
+  if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+#if IBFT_WC > 0
+  if (!(e->p.flags & IBFT_FLAG_KEY_CACHE) || !e->reg.d_state) { set_err("engine has no key registry"); return IBFT_ERR_INVALID_ARG; }
+  all_lanes_lock lk(e);
+  for (auto& L : e->lanes)
+    if (L.pending.active) { set_err("a submitted call is still pending; wait for it first"); return IBFT_ERR_INVALID_ARG; }
+  CU(cudaSetDevice(e->p.device));
+  CU(cudaDeviceSynchronize());
+  if (!e->reg.bounded) {
+    int rc = budget_enable(e);
+    if (rc != IBFT_OK) return rc;
+  }
+  // more slots than the registry can ever have entries would never be used
+  return budget_reclaim(e, std::min(max_tables, e->reg.capacity));
+#else
+  (void)max_tables;
+  set_err("library built without a key registry");
+  return IBFT_ERR_INVALID_ARG;
+#endif
 }
 
 extern "C" int ibft_get_quorum(ibft_engine* e, uint32_t table_slot, uint64_t quorum_out[5], uint64_t* height_out,

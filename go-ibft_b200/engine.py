@@ -38,7 +38,7 @@ EXPORTS = [
     "ibft_set_validators", "ibft_get_quorum", "ibft_verify_batch", "ibft_verify_batch_ex", "ibft_last_item_status", "ibft_verify_submit", "ibft_verify_poll",
     "ibft_verify_wait", "ibft_bind_groups", "ibft_verify_batch_device", "ibft_quorum_reduce_device", "ibft_quorum_partial_words", "ibft_quorum_mark_device", "ibft_quorum_merge_device", "ibft_quorum_exchange_device",
     "ibft_exchange_alloc", "ibft_exchange_open", "ibft_exchange_close", "ibft_exchange_free", "ibft_exchange_clear",
-    "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
+    "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_set_key_table_budget", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
     "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
 ]
 
@@ -73,6 +73,8 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.ibft_last_error.restype = c_char_p
     lib.ibft_refresh_key_tables.restype = c_int
     lib.ibft_refresh_key_tables.argtypes = [c_void_p, POINTER(c_uint32)]
+    lib.ibft_set_key_table_budget.restype = c_int
+    lib.ibft_set_key_table_budget.argtypes = [c_void_p, c_uint32]
     lib.ibft_set_recover_path.restype = c_int
     lib.ibft_set_recover_path.argtypes = [c_void_p, c_int]
     lib.ibft_engine_launch_count.restype = c_uint64
@@ -143,8 +145,10 @@ class Engine:
     """One engine per process per GPU (one process per GPU is the deployment model)."""
 
     def __init__(self, device: int = 0, max_items: int = 1 << 16, max_payload_bytes: int = 1 << 24, max_groups: int = 64,
-                 max_table_slots: int = 16, max_validators: int = 16384, key_cache: bool = False):
-        """key_cache: IBFT_FLAG_KEY_CACHE -- verify (instead of recover) signatures of validators whose key is already known."""
+                 max_table_slots: int = 16, max_validators: int = 16384, key_cache: bool = False,
+                 key_table_budget: int | None = None):
+        """key_cache: IBFT_FLAG_KEY_CACHE -- verify (instead of recover) signatures of validators whose key is already known.
+        key_table_budget: with key_cache, hold at most this many comb tables (136 KiB each; set_key_table_budget)."""
         self.lib = load_library()
         self.params = EngineParams(device, max_items, max_payload_bytes, max_groups, max_table_slots, max_validators, 1 if key_cache else 0)
         self.handle = c_void_p()
@@ -153,6 +157,12 @@ class Engine:
         if rc != IBFT_OK:
             self.handle = None
             raise EngineError(rc, self.lib.ibft_last_error().decode())
+        if key_table_budget is not None:
+            try:
+                self.set_key_table_budget(key_table_budget)
+            except EngineError:
+                self.close()
+                raise
 
     def close(self):
         if getattr(self, "handle", None):
@@ -186,6 +196,11 @@ class Engine:
         n = c_uint32(0)
         self._check(self.lib.ibft_refresh_key_tables(self.handle, ctypes.byref(n)))
         return int(n.value)
+
+    def set_key_table_budget(self, max_tables: int) -> None:
+        """Key registry (engine flag key_cache): keep at most max_tables comb tables, for the keys used most recently (bounded
+        mode from now on; the value may be changed again)."""
+        self._check(self.lib.ibft_set_key_table_budget(self.handle, int(max_tables)))
 
     def launch_count(self) -> int:
         return int(self.lib.ibft_engine_launch_count(self.handle))

@@ -12,6 +12,7 @@
 //                   CUDA kernels.  There is NO CPU fallback: if the engine call fails the answer is `false` (no verdict is
 //                   ever invented) and last_error() says why.
 #pragma once
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -83,12 +84,20 @@ class GpuVerifier : public Verifier {
   uint32_t ingress_linger_us = 0;
   uint32_t ingress_second_min = 32;  // queue length from which a SECOND flush goes up while one is still on the device
 
-  explicit GpuVerifier(const ibft_engine_params& params) {
+  // key_table_budget >= 0 (with IBFT_FLAG_KEY_CACHE): hold at most that many comb tables (ibft_set_key_table_budget)
+  explicit GpuVerifier(const ibft_engine_params& params, int64_t key_table_budget = -1) {
     params_ = params;
     int rc = ibft_engine_create(&params_, &engine_);
+    if (rc == IBFT_OK && key_table_budget >= 0) {
+      rc = ibft_set_key_table_budget(engine_, (uint32_t)std::min<int64_t>(key_table_budget, UINT32_MAX));
+      if (rc != IBFT_OK) {
+        error_ = ibft_last_error();
+        ibft_engine_destroy(engine_);
+      }
+    }
     if (rc != IBFT_OK) {
+      if (error_.empty()) error_ = ibft_last_error();
       engine_ = nullptr;
-      error_ = ibft_last_error();
     }
   }
   ~GpuVerifier() override {

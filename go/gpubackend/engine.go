@@ -43,6 +43,9 @@ type Params struct {
 	// the next height carries the tables over by address, so only newcomers are ever recovered again.  ~2.7x the recover
 	// path's throughput, 0.48 ms instead of 0.8 ms for a 10k-validator COMMIT round (DESIGN.md section 3.1c).
 	KeyCache bool
+	// KeyTableBudget, when non-nil (with KeyCache), bounds the comb tables to that many (ibft_set_key_table_budget): the keys
+	// used most recently keep theirs, the others are verified by recovery, and SetValidators never fails for table memory.
+	KeyTableBudget *uint32
 }
 
 func lastError() error { return errors.New(C.GoString(C.ibft_last_error())) }
@@ -58,6 +61,13 @@ func NewEngine(p Params) (*Engine, error) {
 	}
 	if rc := C.ibft_engine_create(&e.params, &e.h); rc != C.IBFT_OK {
 		return nil, fmt.Errorf("ibft_engine_create: %w", lastError())
+	}
+	if p.KeyTableBudget != nil {
+		if rc := C.ibft_set_key_table_budget(e.h, C.uint32_t(*p.KeyTableBudget)); rc != C.IBFT_OK {
+			err := fmt.Errorf("ibft_set_key_table_budget: %w", lastError())
+			C.ibft_engine_destroy(e.h)
+			return nil, err
+		}
 	}
 	return e, nil
 }

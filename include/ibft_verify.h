@@ -152,7 +152,9 @@ typedef struct ibft_engine_params {
  * more: a validator that leaves every table and later rejoins is learned again.  The engine reserves the state and key of
  * (max_table_slots + 1) x max_validators entries at creation (68 bytes each) and allocates comb tables in chunks of 256
  * entries (34 MiB) as new addresses arrive; ibft_set_validators fails with IBFT_ERR_CAPACITY when the registry cannot grow to
- * hold its table's new addresses, and the slot keeps its previous table. */
+ * hold its table's new addresses, and the slot keeps its previous table.  ibft_set_key_table_budget bounds the comb tables
+ * instead: the engine then keeps at most that many, for the keys used most recently, never allocates them in
+ * ibft_set_validators and never refuses a table for them. */
 #define IBFT_FLAG_KEY_CACHE 1u
 
 typedef struct ibft_device_info {
@@ -331,6 +333,24 @@ int ibft_set_recover_path(ibft_engine* e, int path);
  * entry points call it between rounds.  No-op (0 keys) when the flag is off. */
 int ibft_refresh_key_tables(ibft_engine* e, uint32_t* n_keys_out);
 
+/* Key registry (IBFT_FLAG_KEY_CACHE): hold at most max_tables comb tables (136 KiB each) from now on.  The call is opt-in and
+ * puts the engine in bounded mode for the rest of its life; the value may be changed again at any time (0 keeps every key
+ * learned but builds no table: every signature takes the recover path).  In bounded mode:
+ *   - ibft_set_validators never allocates comb-table memory and never fails for the registry; the tables live in a pool of
+ *     max_tables slots, allocated as slots are first used, so the pool never exceeds max_tables x 136 KiB;
+ *   - the known-key pass records which keys it looked up.  At each reclaim point -- ibft_set_validators,
+ *     ibft_set_key_table_budget and ibft_refresh_key_tables, which then wait for every lane and drain the device -- the
+ *     keys of the resident tables are ranked by the reclaim point at which they were last used (newest first), then those
+ *     that hold a table before those that do not, then by address, and the first max_tables keep or get a table.  A key
+ *     that loses its table stays known, and its signatures take the recover path (verdicts are identical);
+ *   - between reclaim points, the refresh on the way out of ibft_verify_batch / ibft_verify_wait builds tables only into
+ *     free slots, for keys learned since the last reclaim point, in ascending address order;
+ *   - lowering the budget moves the kept tables into the slots below it and returns the memory above it to the device;
+ *   - if the pool cannot be allocated, tables stop at what it holds: no error, the other keys stay known.
+ * IBFT_ERR_INVALID_ARG without IBFT_FLAG_KEY_CACHE, in a library built without a combined table (IBFT_WC == 0), or while a
+ * submitted call is pending. */
+int ibft_set_key_table_budget(ibft_engine* e, uint32_t max_tables);
+
 /* Number of kernel launches issued by this engine since creation (bench.py reports gpu_launches from it). */
 uint64_t ibft_engine_launch_count(ibft_engine* e);
 /* Dependent-free IMAD issue-rate probe on the engine's device (the integer-roofline denominator of bench.py):
@@ -371,13 +391,14 @@ int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* wide_mac_per
  * the combined table d1*G + d2*lambda*G). */
 int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count, uint8_t* out, int* wc, uint32_t* entries);
 /* Key registry entry of validator `validator` (validator-index order) of a table slot: *state_out = 0 unknown, 1 learned,
- * 2 comb table built; key_out (64 bytes) = the learned affine key, x then y as 8 little-endian words; out = `count` comb
+ * 2 comb table built (a key known in a bounded registry without a table reads 1); key_out (64 bytes) = the learned affine key, x then y as 8 little-endian words; out = `count` comb
  * entries starting at `first` in the format of ibft_debug_ctable, entry j * 128 + m - 1 = m * 2^(8j) * Q (j = 0..16,
  * m = 1..128).  Read through the table's reference into the engine's registry.  Any output may be NULL.  Waits for the device. */
 int ibft_debug_keytab(ibft_engine* e, uint32_t table_slot, uint32_t validator, uint32_t first, uint32_t count, uint8_t* out,
                       uint32_t* state_out, uint8_t* key_out);
 /* The key registry as a whole: *entries_in_use = distinct addresses of the resident tables, *entries_ready = those of them
- * whose comb table is built, *bytes_reserved = bytes of comb-table chunks allocated so far (whole chunks of 256 x 136 KiB).
+ * whose comb table is built, *bytes_reserved = bytes of comb-table chunks allocated so far (whole chunks of 256 x 136 KiB;
+ * in bounded mode, the bytes the pool holds now: 136 KiB per allocated table slot).
  * Any output may be NULL.  IBFT_ERR_INVALID_ARG without IBFT_FLAG_KEY_CACHE.  Waits for the device. */
 int ibft_debug_key_registry(ibft_engine* e, uint32_t* entries_in_use, uint32_t* entries_ready, uint64_t* bytes_reserved);
 /* Number of items the known-key pass (IBFT_FLAG_KEY_CACHE) of the most recent completed host-buffer call left to the recover
