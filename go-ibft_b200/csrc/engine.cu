@@ -3346,17 +3346,21 @@ extern "C" int ibft_debug_op(ibft_engine* e, int op, const uint8_t* a, const uin
   int rc = IBFT_OK;
   cudaError_t ce;
 #define CUK(call) if ((ce = (call)) != cudaSuccess) { set_err("%s failed: %s", #call, cudaGetErrorString(ce)); rc = IBFT_ERR_CUDA; goto done; }
+  // Operands, the cleared output and the kernel all go on the lane's stream.  That stream is non-blocking, so a copy or memset
+  // on the legacy default stream is not ordered before the kernel: a pageable cudaMemcpy may return before its DMA lands and
+  // cudaMemset returns before it runs, and the kernel could read the previous call's operands (cudaMalloc hands the same
+  // blocks back) or have a lane's result cleared after it was written.
   CUK(cudaMalloc(&d_a, (size_t)n * 32));
-  CUK(cudaMemcpy(d_a, a, (size_t)n * 32, cudaMemcpyHostToDevice));
-  if (b) { CUK(cudaMalloc(&d_b, (size_t)n * 32)); CUK(cudaMemcpy(d_b, b, (size_t)n * 32, cudaMemcpyHostToDevice)); }
-  if (c) { CUK(cudaMalloc(&d_c, (size_t)n * 64)); CUK(cudaMemcpy(d_c, c, (size_t)n * 64, cudaMemcpyHostToDevice)); }
+  CUK(cudaMemcpyAsync(d_a, a, (size_t)n * 32, cudaMemcpyHostToDevice, L->stream));
+  if (b) { CUK(cudaMalloc(&d_b, (size_t)n * 32)); CUK(cudaMemcpyAsync(d_b, b, (size_t)n * 32, cudaMemcpyHostToDevice, L->stream)); }
+  if (c) { CUK(cudaMalloc(&d_c, (size_t)n * 64)); CUK(cudaMemcpyAsync(d_c, c, (size_t)n * 64, cudaMemcpyHostToDevice, L->stream)); }
   CUK(cudaMalloc(&d_o, (size_t)n * out_stride));
-  CUK(cudaMemset(d_o, 0, (size_t)n * out_stride));
+  CUK(cudaMemsetAsync(d_o, 0, (size_t)n * out_stride, L->stream));
   k_debug_op<<<(n + 63) / 64, 64, 0, L->stream>>>(op, d_a, d_b, d_c, n, d_o, out_stride);
   e->launches++;
   CUK(cudaGetLastError());
+  CUK(cudaMemcpyAsync(out, d_o, (size_t)n * out_stride, cudaMemcpyDeviceToHost, L->stream));
   CUK(cudaStreamSynchronize(L->stream));
-  CUK(cudaMemcpy(out, d_o, (size_t)n * out_stride, cudaMemcpyDeviceToHost));
 done:
 #undef CUK
   cudaFree(d_a); cudaFree(d_b); cudaFree(d_c); cudaFree(d_o);

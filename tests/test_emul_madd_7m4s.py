@@ -40,7 +40,7 @@ def run(E, fn, item, arena=None):
 def test_crafted_vectors_with_7m4s_addition(emul_7m4s, fn):
     emul_7m4s.emul_branch_reset()
     for v in A.recover_vectors():
-        assert run(emul_7m4s, fn, A.recover_items([v])) == (int(v.key is not None), v.addr or bytes(20)), v.tag
+        assert run(emul_7m4s, fn, A.recover_items([v])) == (int(v.verdict), v.addr or bytes(20)), v.tag
     c = (ctypes.c_ulonglong * 12)()
     emul_7m4s.emul_branch_counts(c)
     assert c[0] >= 1 and c[1] >= 1 and c[2] >= 1, list(c)  # P + P, P - P, accumulator at infinity

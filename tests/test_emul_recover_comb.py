@@ -62,15 +62,18 @@ def non_abscissas(count, seed):
 
 def test_crafted_vectors_and_every_rare_branch(comb):
     """every crafted vector gives the oracle's verdict and address; A = B, A = -B (the "final-add" vectors), u1 = 0 (z = 0 and
-    z = n) and a non-residue r^3 + 7 (both recovery ids) each reach their branch of the final addition"""
+    z = n) and a non-residue r^3 + 7 (both recovery ids; among the crafted vectors only the x = r + n forgeries whose r is no
+    abscissa) each reach their branch of the final addition"""
     import workloads as wl
     comb.emul_branch_reset()
     vecs = A.recover_vectors()
     for v in vecs:
-        assert run(comb, "emul_verify_item_comb", A.recover_items([v])) == (int(v.key is not None), v.addr or bytes(20)), v.tag
+        assert run(comb, "emul_verify_item_comb", A.recover_items([v])) == (int(v.verdict), v.addr or bytes(20)), v.tag
     c = rec_counts(comb)
     assert c[REC["DBL"]] >= 1 and c[REC["NEG"]] >= 1 and c[REC["B_INF"]] >= 8, c
-    assert c[REC["NONRES"]] == 0, c
+    nonres = [v for v in vecs if A.in_range(v.sig) and ec.lift_x(int.from_bytes(v.sig[:32], "big"), 0) is None]
+    assert len(nonres) >= 6 and all(v.tag.startswith("r+n forgery") for v in nonres)
+    assert c[REC["NONRES"]] == len(nonres), c
     rnd = random.Random(11)
     for r in non_abscissas(6, 12):
         for v in (0, 1):
@@ -78,7 +81,7 @@ def test_crafted_vectors_and_every_rare_branch(comb):
             dig = rnd.randbytes(32)
             assert co.ecrecover_address(dig, sig) is None
             assert run(comb, "emul_verify_item_comb", wl.make_item(sig, bytes(20), 0, dig)) == (0, bytes(20))
-    assert rec_counts(comb)[REC["NONRES"]] == 12
+    assert rec_counts(comb)[REC["NONRES"]] == len(nonres) + 12
 
 
 def test_random_and_corrupted_signatures_both_parities(comb):

@@ -3,6 +3,7 @@ and the known-key pass made visible through the number of items it hands to the 
 
 A known-key pass that rejects everything still produces the recover path's bitmap (the recover pass decides what it leaves);
 only the handed-back count shows it.  Every count asserted here is derived from the oracle (see expected_handed_back)."""
+import functools
 import random
 
 import numpy as np
@@ -79,7 +80,7 @@ def crafted_batch(seed=5):
     rows, want, addrs = [], [], []
     for i, v in enumerate(A.recover_vectors()):
         rows.append(A.recover_items([v]))
-        want.append(v.key is not None)
+        want.append(v.verdict)
         addrs.append(v.addr or bytes(20))
         if i % 3 == 0:
             d = rnd.getrandbits(256) % (N - 1) + 1
@@ -131,45 +132,72 @@ def check_key_table(tab, Q, ms=(1, 2, 3, 4, 64, 127, 128)):
         base = ec.point_mul(256, base)
 
 
+@functools.lru_cache(maxsize=None)
+def key_table_reference(Q) -> tuple:
+    """the whole comb table of Q by the big-int oracle: entry j * 128 + m - 1 = m * 2^(8j) * Q, affine"""
+    out, base = [], Q
+    for _ in range(POSITIONS):
+        P = base
+        for _ in range(ENTRIES):
+            out.append(P)
+            P = ec.point_add(P, base)
+        base = ec.point_mul(256, base)
+    return tuple(out)
+
+
+def check_whole_key_table(tab, Q):
+    ref = key_table_reference(Q)
+    bad = [k for k in range(POSITIONS * ENTRIES) if point_of(tab[k]) != ref[k]]
+    assert not bad, (hex(Q[0]), hex(Q[1]), [divmod(k, ENTRIES) for k in bad[:4]], len(bad))
+
+
 def test_learned_keys_and_key_tables_on_every_recover_kernel():
     """Each recover kernel has its own learn_key call: one signature per validator through each forced kernel (recovered addresses
     requested, so the kernel itself runs), then the learned key must be Q exactly (canonical), entry m of position j of its comb
-    table m * 2^(8j) * Q, one full table of 2,176 entries must match, and the tables carried to the next height must be
-    byte-identical to the donor's."""
+    table m * 2^(8j) * Q, whole tables of 2,176 entries must match, and the tables carried to the next height must be
+    byte-identical to the donor's.  Besides four signing keys per kernel, each kernel learns its share of the coordinate-edge
+    keys of tests/adversarial.py (coordinates below 2^256 - p or near p: learned, stored and tabled only if normalised) from
+    signatures made without their private keys; every edge key's whole table is checked."""
     vs = wl.ValidatorSet(91, 4 * len(PATHS))
+    edge = [Q for _, Q in A.key_edge_points()]
+    keys = [ec.point_mul(d, ec.G) for d in vs.keys] + edge
+    addrs = vs.addrs + [ec.pubkey_to_address(Q) for Q in edge]
+    rnd = random.Random(92)
     eng = ib.Engine(**KC, key_cache=True)
     try:
-        eng.set_validators(0, 5, vs.addr_array(), None)
+        eng.set_validators(0, 5, np.frombuffer(b"".join(addrs), np.uint8).reshape(-1, 20).copy(), None)
         groups = groups_for(eng, 1)
         dig = co.keccak256(b"learn")
+
+        def item(i):
+            if i < vs.n:
+                return wl.make_item(wl.sign(vs.keys[i], dig, low_s=bool(i & 1)), vs.addrs[i], 0, dig)
+            v = A.signature_for("learn", keys[i], rnd)
+            return wl.make_item(v.sig, addrs[i], 0, v.digest)
+
         for k, path in enumerate(PATHS):
             eng.set_recover_path(path)
-            own = range(4 * k, 4 * k + 4)
-            items = np.concatenate([wl.make_item(wl.sign(vs.keys[i], dig, low_s=bool(i & 1)), vs.addrs[i], 0, dig) for i in own])
+            own = list(range(4 * k, 4 * k + 4)) + list(range(vs.n + k, len(keys), len(PATHS)))
+            items = np.concatenate([item(i) for i in own])
             bm, _, _ = eng.verify_batch(items, b"", groups, want_recovered=True)
-            assert bits(bm, 4).all(), path
+            assert bits(bm, len(own)).all(), path
             for i in own:
                 state, key, _ = eng.key_table(0, i)
                 assert state == 2, (path, i)                                 # learned, table built on the way out of the call
-                assert point_of(key) == ec.point_mul(vs.keys[i], ec.G), (path, i)
-        assert eng.refresh_key_tables() == vs.n
+                assert point_of(key) == keys[i], (path, i)
+        assert eng.refresh_key_tables() == len(keys)
         tables = []
-        for i in range(vs.n):
+        for i in range(len(keys)):
             _, _, tab = eng.key_table(0, i, 0, POSITIONS * ENTRIES)
-            check_key_table(tab, ec.point_mul(vs.keys[i], ec.G))
+            if i < vs.n:
+                check_key_table(tab, keys[i])
             tables.append(tab)
-        # one whole table, entry by entry
-        Q = ec.point_mul(vs.keys[5], ec.G)
-        base = Q
-        for j in range(POSITIONS):
-            P = base
-            for m in range(1, ENTRIES + 1):
-                assert point_of(tables[5][j * ENTRIES + m - 1]) == P, (j, m)
-                P = ec.point_add(P, base)
-            base = ec.point_mul(256, base)
+        # whole tables, entry by entry: one signing key's and every edge key's
+        for i in [5] + list(range(vs.n, len(keys))):
+            check_whole_key_table(tables[i], keys[i])
         # next height in the other slot: every table carried over, byte for byte
-        eng.set_validators(1, 6, vs.addr_array(), None)
-        for i in range(vs.n):
+        eng.set_validators(1, 6, np.frombuffer(b"".join(addrs), np.uint8).reshape(-1, 20).copy(), None)
+        for i in range(len(keys)):
             state, key, tab = eng.key_table(1, i, 0, POSITIONS * ENTRIES)
             _, key0, _ = eng.key_table(0, i)
             assert state == 2 and np.array_equal(key, key0) and tab.tobytes() == tables[i].tobytes(), i
@@ -179,32 +207,38 @@ def test_learned_keys_and_key_tables_on_every_recover_kernel():
 
 # ------------------------------------------------------------------------------------- crafted known-key vectors
 def known_batch(group=0):
-    """(items, oracle bits, number of items the known-key pass must hand back): the crafted valid set interleaved with its
-    misattributed, recovery-id-flipped and cancelling variants (all of them rejected by the verification, verdict 0)"""
+    """(items, number of items the known-key pass must hand back): the crafted valid set interleaved with its misattributed,
+    recovery-id-flipped, cancelling and x = r + n forgery variants (all of them rejected by the verification, verdict 0)"""
     rows, handed = [], 0
-    canc = A.known_cancelling()
+    extra = A.known_cancelling() + A.known_r_plus_n()
     for n, v in enumerate(A.known_vectors()):
         rows.append(wl.make_item(v.sig, A.known_addr(v.key_index), 0, v.digest, group))
         sig, j = A.misattributed(v)
         rows.append(wl.make_item(sig, A.known_addr(j), 0, v.digest, group))
         rows.append(wl.make_item(A.flipped(v), A.known_addr(v.key_index), 0, v.digest, group))
         handed += 2
-        if n < len(canc):
-            c = canc[n]
+        if n < len(extra):
+            c = extra[n]
             rows.append(wl.make_item(c.sig, A.known_addr(c.key_index), 0, c.digest, group))
             handed += 1
+    assert len(A.known_vectors()) >= len(extra)
     items = np.concatenate(rows)
     return items, handed
 
 
 def known_addrs():
-    return np.frombuffer(b"".join(A.known_addr(i) for i in range(len(A.KNOWN_KEYS))), np.uint8).reshape(-1, 20).copy()
+    return np.frombuffer(b"".join(A.known_addr(i) for i in range(len(A.known_points()))), np.uint8).reshape(-1, 20).copy()
+
+
+def valid_known_items(vectors=None):
+    return np.concatenate([wl.make_item(v.sig, A.known_addr(v.key_index), 0, v.digest) for v in vectors or A.known_vectors()])
 
 
 def test_crafted_known_key_vectors_on_every_known_key_kernel():
-    """Learn the six crafted keys, then run the crafted set through k_verify_known<32> (THREAD, small batch), k_verify_known<128>
-    (THREAD, replicated past SMs x 256), k_verify_split (SPLIT) and the AUTO four-piece path: bitmap = oracle, results = a plain
-    engine's; the all-valid set hands back nothing, each rejected variant exactly once."""
+    """Learn the crafted keys (the six multiples, the coordinate-edge keys and the x = r + n forgery keys), then run the crafted
+    set through k_verify_known<32> (THREAD, small batch), k_verify_known<128> (THREAD, replicated past SMs x 256), k_verify_split
+    (SPLIT) and the AUTO four-piece path: bitmap = oracle, results = a plain engine's; the all-valid set hands back nothing, each
+    rejected variant -- each x = r + n forgery, which plain ECDSA accepts for its key, among them -- exactly once."""
     addrs = known_addrs()
     sms = sm_count()
     eng = ib.Engine(**KC, key_cache=True)
@@ -213,10 +247,10 @@ def test_crafted_known_key_vectors_on_every_known_key_kernel():
         for e in (eng, plain):
             e.set_validators(0, 3, addrs, None)
         groups = groups_for(eng, 1)
-        valid = np.concatenate([wl.make_item(v.sig, A.known_addr(v.key_index), 0, v.digest) for v in A.known_vectors()])
+        valid = valid_known_items()
         bm, _, _ = eng.verify_batch(valid, b"", groups)                      # pass 1: keys learned, tables built on the way out
         assert bits(bm, len(valid)).all()
-        assert eng.refresh_key_tables() == len(A.KNOWN_KEYS)
+        assert eng.refresh_key_tables() == len(A.known_points())
         bm, _, _ = eng.verify_batch(valid, b"", groups)
         assert bits(bm, len(valid)).all() and eng.known_handed_back() == 0
         items, handed = known_batch()
@@ -224,6 +258,7 @@ def test_crafted_known_key_vectors_on_every_known_key_kernel():
         assert int(bits(want, len(items)).sum()) == len(A.known_vectors())
         cases = [(ib.Engine.PATH_THREAD, 1), (ib.Engine.PATH_THREAD, -(-(sms * 256 + 100) // len(items))), (ib.Engine.PATH_SPLIT, 1),
                  (ib.Engine.PATH_SPLIT, 7), (ib.Engine.PATH_AUTO, -(-(sms * 72) // len(items)))]
+        assert sms * 48 < cases[-1][1] * len(items) <= sms * 96                # AUTO's four-piece range
         for path, reps in cases:
             eng.set_recover_path(path)
             it = np.tile(items, reps)

@@ -7,9 +7,10 @@ import numpy as np
 import pytest
 import torch
 
+import adversarial as A
 import ibft_b200 as ib
 from oracle import coracle as co
-from test_gpu_adversarial import bits, expected_handed_back
+from test_gpu_adversarial import bits, check_whole_key_table, expected_handed_back, known_addrs, known_batch, valid_known_items
 from test_gpu_key_registry import make_engine, round_items, same_as_plain
 
 pytestmark = pytest.mark.gpu
@@ -191,6 +192,71 @@ def test_budget_changes_at_run_time():
         assert eng.key_registry() == (1000, 0, 0)
         assert check_round(eng, plain, round_items(privs, addrs, co.keccak256(b"rt-4")), addrs, 0, set()).all()
         assert eng.known_handed_back() == 1000
+    finally:
+        eng.close()
+        plain.close()
+
+
+def test_edge_keys_evicted_readmitted_and_moved_down():
+    """The crafted known-key set of tests/adversarial.py (its coordinate-edge keys: coordinates below 2^256 - p or near p; and the
+    keys of the x = r + n forgeries) at a budget 16 below its size.  The keys without a table sign and take tables from 16 others at
+    the reclaim point (EVICTED: state 1); those sign and are readmitted; then the budget is lowered, so that kept tables above it
+    move down.  After each step every verdict equals a plain engine's and the oracle's, the known-key pass hands back what the
+    tables predict -- every forgery among them -- and every edge key holding a table holds the big-int oracle's whole table."""
+    pts = A.known_points()
+    addrs = known_addrs()
+    edge = {bytes(A.known_addr(i)): Q for i, Q in enumerate(pts) if i >= len(A.KNOWN_KEYS)}
+    by_key: dict[int, list] = {}
+    for v in A.known_vectors():
+        by_key.setdefault(v.key_index, []).append(v)
+    mixed, _ = known_batch()
+
+    def signing(keys):
+        return valid_known_items([v for i in sorted(keys) for v in by_key[i]])
+
+    def check_tables(ready):
+        assert ready & set(edge)
+        for v in range(len(addrs)):
+            a = bytes(addrs[v])
+            if a in edge and a in ready:
+                check_whole_key_table(eng.key_table(0, v, 0, 17 * 128)[2], edge[a])
+
+    budget = len(pts) - 16
+    eng = make_engine(slots=2, max_validators=1024, key_cache=True, key_table_budget=budget)
+    plain = make_engine(slots=2, max_validators=1024)
+    try:
+        for e in (eng, plain):
+            e.set_validators(0, 1, addrs)
+        assert check_round(eng, plain, signing(range(len(pts))), addrs, 0, set()).all()  # every key learned
+        eng.refresh_key_tables()                                  # reclaim point: clears the used flags
+        first = ready_set(eng, 0, addrs)
+        assert len(first) == budget
+        check_tables(first)
+        cold = [i for i in range(len(pts)) if bytes(addrs[i]) not in first]
+        assert check_round(eng, plain, signing(cold), addrs, 0, first).all()
+        eng.refresh_key_tables()                                  # reclaim point: the cold keys take 16 tables
+        second = ready_set(eng, 0, addrs)
+        evicted = first - second
+        assert len(second) == budget and {bytes(addrs[i]) for i in cold} <= second and len(evicted) == 16
+        assert evicted & set(edge)
+        assert all(eng.key_table(0, v)[0] == 1 for v in range(len(addrs)) if bytes(addrs[v]) in evicted)
+        check_tables(second)
+        check_round(eng, plain, mixed, addrs, 0, second)
+        eng.refresh_key_tables()                                  # every key used alike: nothing moves
+        assert ready_set(eng, 0, addrs) == second
+        back = [i for i in range(len(pts)) if bytes(addrs[i]) in evicted]
+        assert check_round(eng, plain, signing(back), addrs, 0, second).all()
+        eng.refresh_key_tables()                                  # reclaim point: the evicted keys are readmitted
+        third = ready_set(eng, 0, addrs)
+        assert len(third) == budget and evicted <= third
+        check_tables(third)
+        check_round(eng, plain, mixed, addrs, 0, third)
+        eng.set_key_table_budget(budget - 16)                     # kept tables in the top 16 slots move down
+        fourth = ready_set(eng, 0, addrs)
+        assert len(fourth) == budget - 16 and fourth <= third and eng.key_registry()[1] == budget - 16
+        check_tables(fourth)
+        check_round(eng, plain, mixed, addrs, 0, fourth)
+        assert check_round(eng, plain, signing(range(len(pts))), addrs, 0, fourth).all()
     finally:
         eng.close()
         plain.close()
