@@ -191,13 +191,14 @@ __device__ __forceinline__ void learn_key(const slot_dev* __restrict__ slots, ui
 #endif
 // BLOCK = 128 for throughput (12 resident warps/SM at 166 registers); BLOCK = 32 for latency-critical small batches (a
 // 10k-validator COMMIT round is only 313 warps: one-warp CTAs spread them over all 132 SMs of an H100 instead of 79).
-template <int BLOCK>
+// WIDE: u1*G from the wide generator comb `wtable` (an engine that holds it launches these); else from the per-position comb.
+template <int BLOCK, bool WIDE>
 __global__ void __launch_bounds__(BLOCK, (IBFT_MIN_BLOCKS * IBFT_BLOCK) / BLOCK)
 k_recover(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __restrict__ arena, size_t arena_len,
           uint32_t shard_lo, uint32_t shard_hi, const ibft_group_desc* __restrict__ groups, uint32_t n_groups,
           const slot_dev* __restrict__ slots, uint32_t n_slots, uint32_t* __restrict__ bitmap,
           uint8_t* __restrict__ recovered, uint8_t* __restrict__ status, const uint32_t* __restrict__ ctable, vote_sink sink,
-          const uint32_t* __restrict__ list) {
+          const uint32_t* __restrict__ list, const uint32_t* __restrict__ wtable) {
   // list != nullptr: WORKLIST mode (second pass of the key-registry path): list[0] = count, list[1..] = item indices that the
   // verify pass could not decide; the items are gathered, verdict bits are OR-ed into the bitmap the first pass wrote.
 #if IBFT_GTAB_SMEM
@@ -261,6 +262,7 @@ k_recover(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __
     if (status != nullptr && list == nullptr) status[idx] = (uint8_t)st;
     gtab_view G{s_gtab};
     G.comb = ctable;
+    G.wide = WIDE ? wtable : nullptr;
     rtab_view T{s_rtab + tid, (uint32_t)BLOCK};
     // the signer is looked up FIRST: an item of an unknown group / a non-member can never get verdict 1 (its signature is
     // still recovered when the caller asked for the recovered addresses)
@@ -269,7 +271,12 @@ k_recover(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __
     const bool member = have && group_member(groups, n_groups, slots, n_slots, it.group, ri.signer, &v, &slot);
     if (have && (member || recovered != nullptr)) {
       aff K;
-      bool rec = ecrecover_address(ri.r, ri.s, ri.v, ri.z, G, T, addr, &K);
+#if IBFT_GEN_WIDE > 0
+      const bool rec = WIDE ? ecrecover_address_x(exec_serial_wide{}, ri.r, ri.s, ri.v, ri.z, G, T, addr, &K)
+                            : ecrecover_address(ri.r, ri.s, ri.v, ri.z, G, T, addr, &K);
+#else
+      const bool rec = ecrecover_address(ri.r, ri.s, ri.v, ri.z, G, T, addr, &K);
+#endif
       if (!rec) {
 #pragma unroll
         for (int i = 0; i < 20; i++) addr[i] = 0;
@@ -1405,6 +1412,100 @@ k_build_ctable(uint32_t* __restrict__ out) {  // blockIdx.y = comb position: ent
 }
 #endif
 
+#if IBFT_GEN_WIDE > 0
+// ------------------------------------------------------------------------------------------------------------
+// wide generator comb (secp_ec.cuh, IBFT_GEN_WIDE): built once per process and device.  A thread builds a run of IBFT_WIDE_RUN
+// consecutive entries of one position: the first by a scalar multiplication, the others by chained mixed additions of the
+// position's base 2^(w p) G, all normalised with one inversion (Montgomery's trick).  Every entry is checked on the curve; an
+// entry off the curve sets *bad.
+// ------------------------------------------------------------------------------------------------------------
+#define IBFT_WIDE_RUN 8  // 2 x 7 field elements of the run fit the thread's IBFT_RTAB_WORDS slice of shared memory
+// m * 2^(w pos) mod n
+__device__ sc wide_scalar(uint32_t pos, uint32_t m) {
+  sc a, t;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { a.v[i] = 0; t.v[i] = 0; }
+  a.v[0] = m;
+  t.v[(pos * IBFT_GEN_WIDE) / 32] = 1u << ((pos * IBFT_GEN_WIDE) % 32);  // 2^(w pos) <= 2^242 < n
+  return sc_mul(a, t);
+}
+// k * G (k in [1, n)) affine, by the kernel's own double-scalar multiplication with u2 = 0
+__device__ void wide_mult_affine(const sc& k, const rtab_view& T, fe& x, fe& y) {
+  gtab_view G{g_gtable};
+  aff g1;
+  G.load(0, g1.x, g1.y);
+  sc zero;
+#pragma unroll
+  for (int i = 0; i < 8; i++) zero.v[i] = 0;
+  const jac P = ecmult_double(k, zero, g1, G, T);
+  const fe zi = IBFT_FE_INV(P.z), zi2 = fe_sqr(zi);
+  x = fe_normalize(fe_mul(P.x, zi2));
+  y = fe_normalize(fe_mul(P.y, fe_mul(zi2, zi)));
+}
+__device__ void wide_store_checked(uint32_t* o, const fe& x, const fe& y, uint32_t* bad) {
+  if (!fe_equal(fe_sqr(y), fe_add(fe_mul(fe_sqr(x), x), fe_from_u32(7)))) atomicOr(bad, 1u);
+#pragma unroll
+  for (int i = 0; i < 8; i++) { o[i] = x.v[i]; o[8 + i] = y.v[i]; }
+}
+// bases[p] = 2^(w p) G, p = 0 .. IBFT_GW_POSITIONS - 1
+__global__ void __launch_bounds__(32) k_wide_bases(uint32_t* __restrict__ bases, uint32_t* __restrict__ bad) {
+  __shared__ uint32_t s_rtab[32 * IBFT_RTAB_WORDS];
+  const uint32_t p = threadIdx.x;
+  if (p >= IBFT_GW_POSITIONS) return;
+  fe x, y;
+  wide_mult_affine(wide_scalar(p, 1), rtab_view{s_rtab + p, 32u}, x, y);
+  wide_store_checked(bases + IBFT_GTAB_ENTRY_WORDS * p, x, y, bad);
+}
+// blockIdx.y = position; entry index e (m = e + 1) of a position at out + 16 * (pos * IBFT_GW_ENTRIES + e)
+__global__ void __launch_bounds__(64) k_build_wtable(uint32_t* __restrict__ out, const uint32_t* __restrict__ bases, uint32_t* __restrict__ bad) {
+  __shared__ uint32_t s_rtab[64 * IBFT_RTAB_WORDS];
+  const uint32_t pos = blockIdx.y;
+  const uint32_t count = pos + 1 < IBFT_GW_POSITIONS ? IBFT_GW_ENTRIES : IBFT_GW_TOP_ENTRIES;
+  const uint32_t first = (blockIdx.x * 64 + threadIdx.x) * IBFT_WIDE_RUN;
+  if (first >= count) return;
+  const int len = (int)min((uint32_t)IBFT_WIDE_RUN, count - first);
+  const rtab_view T{s_rtab + threadIdx.x, 64u};  // entry i of the run: (Z_i, Z_1 ... Z_i)
+  uint32_t* o = out + IBFT_GTAB_ENTRY_WORDS * ((size_t)pos * IBFT_GW_ENTRIES + first);
+  fe bx, by;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { bx.v[i] = bases[IBFT_GTAB_ENTRY_WORDS * pos + i]; by.v[i] = bases[IBFT_GTAB_ENTRY_WORDS * pos + 8 + i]; }
+  jac P;
+  wide_mult_affine(wide_scalar(pos, first + 1), T, P.x, P.y);
+  P.z = fe_from_u32(1);
+  P.inf = false;
+  wide_store_checked(o, P.x, P.y, bad);
+  // entries 1 .. len-1: P + base (m = 1 makes the first addition a doubling, which the adder handles); Jacobian X, Y parked
+  // in the output
+  fe pre = P.z;
+  IBFT_ROLLED
+  for (int i = 1; i < len; i++) {
+    P = jac_add_affine(P, bx, by);
+    pre = i == 1 ? P.z : fe_mul(pre, P.z);
+    T.store(i, P.z, pre);
+#pragma unroll
+    for (int k = 0; k < 8; k++) { o[16 * i + k] = P.x.v[k]; o[16 * i + 8 + k] = P.y.v[k]; }
+  }
+  if (len < 2) return;
+  fe acc = IBFT_FE_INV(pre);  // 1 / (Z_1 ... Z_{len-1})
+  IBFT_ROLLED
+  for (int i = len - 1; i >= 1; i--) {
+    fe zi = acc, z, t;
+    T.load(i, z, t);
+    if (i > 1) {
+      fe prev;
+      T.load(i - 1, t, prev);
+      zi = fe_mul(acc, prev);  // 1 / Z_i
+      acc = fe_mul(acc, z);
+    }
+    fe x, y;
+#pragma unroll
+    for (int k = 0; k < 8; k++) { x.v[k] = o[16 * i + k]; y.v[k] = o[16 * i + 8 + k]; }
+    const fe zi2 = fe_sqr(zi);
+    wide_store_checked(o + 16 * i, fe_normalize(fe_mul(x, zi2)), fe_normalize(fe_mul(y, fe_mul(zi2, zi))), bad);
+  }
+}
+#endif
+
 #if IBFT_WC > 0
 // key registry: comb tables for every registry entry whose key has been learned but whose table is missing.  One thread per
 // (entry, comb position): 8*pos doublings, 128 additions and 128 inversions each -- a whole 10k-validator set (170,000
@@ -1747,6 +1848,7 @@ struct ibft_engine {
   key_registry reg;
   int sm_count = 132;  // replaced by the device's count at engine creation
   uint32_t* d_ctable = nullptr;  // combined generator table (IBFT_WC > 0)
+  uint32_t* d_wtable = nullptr;  // wide generator comb of the device (IBFT_GEN_WIDE > 0), shared; nullptr when it did not fit
   cudaFuncAttributes recover_attr{};
   // hashing (ibft_keccak256_batch / ibft_proposal_hash_batch): own lock, own stream, own grow-only scratch -- a hash call
   // never waits for a verify call and never allocates on the per-call path
@@ -1756,6 +1858,11 @@ struct ibft_engine {
   size_t hs_arena_cap = 0;
   uint32_t hs_n_cap = 0;
 };
+// the one-thread recover kernel of an engine: u1*G from the wide comb when the engine holds it
+template <int BLOCK>
+static decltype(&k_recover<BLOCK, false>) recover_kernel(const ibft_engine* e) {
+  return e->d_wtable != nullptr ? k_recover<BLOCK, true> : k_recover<BLOCK, false>;
+}
 // every lane, in index order (validator-table replacement and other engine-wide operations)
 struct all_lanes_lock {
   ibft_engine* e;
@@ -1782,10 +1889,74 @@ static void lane_free(lane* L) {
   if (L->stream) cudaStreamDestroy(L->stream);
 }
 
+// The wide generator comb: 1.38 GiB at w = 22, so ONE per device, shared by every engine of the process and freed by the last
+// engine on the device to close.  Built on the first engine's lane-0 stream while the registry lock is held.
+struct wide_table_ref {
+  uint32_t* d = nullptr;
+  int refs = 0;
+};
+static std::mutex g_wide_mu;
+static std::unordered_map<int, wide_table_ref> g_wide;
+
+static int wide_acquire(ibft_engine* e, cudaStream_t st) {
+#if IBFT_GEN_WIDE > 0
+  std::lock_guard<std::mutex> lk(g_wide_mu);
+  wide_table_ref& w = g_wide[e->p.device];
+  if (w.refs == 0) {
+    // the table, then the positions' bases 2^(w p) G, then the on-curve flag (one entry's worth of words)
+    const size_t entries = IBFT_GW_TOTAL + IBFT_GW_POSITIONS + 1;
+    uint32_t* d = nullptr;
+    if (cudaMalloc(&d, entries * IBFT_GTAB_ENTRY_WORDS * 4) != cudaSuccess) {
+      (void)cudaGetLastError();  // does not fit: this engine adds u1*G by the per-position comb, with the same verdicts
+      g_wide.erase(e->p.device);
+      return IBFT_OK;
+    }
+    uint32_t* bases = d + IBFT_GW_TOTAL * IBFT_GTAB_ENTRY_WORDS;
+    uint32_t* bad = bases + IBFT_GW_POSITIONS * IBFT_GTAB_ENTRY_WORDS;
+    uint32_t h_bad = 0;
+    cudaError_t ce = cudaMemsetAsync(bad, 0, 4, st);
+    if (ce == cudaSuccess) {
+      k_wide_bases<<<1, 32, 0, st>>>(bases, bad);
+      k_build_wtable<<<dim3((IBFT_GW_ENTRIES + 64 * IBFT_WIDE_RUN - 1) / (64 * IBFT_WIDE_RUN), IBFT_GW_POSITIONS), 64, 0, st>>>(d, bases, bad);
+      e->launches += 2;
+      ce = cudaGetLastError();
+    }
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync(&h_bad, bad, 4, cudaMemcpyDeviceToHost, st);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+    if (ce != cudaSuccess || h_bad) {
+      cudaFree(d);
+      g_wide.erase(e->p.device);
+      if (ce != cudaSuccess) set_err("wide generator comb: %s", cudaGetErrorString(ce));
+      else set_err("wide generator comb: an entry built on the device is not on the curve");
+      return IBFT_ERR_CUDA;
+    }
+    w.d = d;
+  }
+  w.refs++;
+  e->d_wtable = w.d;
+#else
+  (void)e;
+  (void)st;
+#endif
+  return IBFT_OK;
+}
+
+static void wide_release(ibft_engine* e) {
+  if (!e->d_wtable) return;
+  std::lock_guard<std::mutex> lk(g_wide_mu);
+  auto it = g_wide.find(e->p.device);
+  if (--it->second.refs == 0) {
+    cudaFree(it->second.d);
+    g_wide.erase(it);
+  }
+  e->d_wtable = nullptr;
+}
+
 static void engine_free(ibft_engine* e) {
   if (!e) return;
   cudaSetDevice(e->p.device);
   cudaDeviceSynchronize();
+  wide_release(e);
   for (auto& s : e->slots) {
     if (s.d_keys) cudaFree(s.d_keys);
     if (s.d_powers) cudaFree(s.d_powers);
@@ -1869,13 +2040,16 @@ static int engine_alloc(ibft_engine* e) {
   e->slots.resize(p.max_table_slots);
   e->slots_shadow.assign(p.max_table_slots, slot_dev{});
   CU(cudaMemcpyToSymbol(g_gtable, IBFT_GTABLE, sizeof(uint32_t) * IBFT_GTAB_ENTRY_WORDS * IBFT_GTAB_ENTRIES));
-  CU(cudaFuncSetAttribute(k_recover<IBFT_BLOCK>, cudaFuncAttributeMaxDynamicSharedMemorySize, IBFT_BLOCK * IBFT_RTAB_WORDS * 4));
-  CU(cudaFuncSetAttribute(k_recover<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * IBFT_RTAB_WORDS * 4));
+  for (bool wide : {false, true}) {
+    CU(cudaFuncSetAttribute(wide ? k_recover<IBFT_BLOCK, true> : k_recover<IBFT_BLOCK, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            IBFT_BLOCK * IBFT_RTAB_WORDS * 4));
+    CU(cudaFuncSetAttribute(wide ? k_recover<32, true> : k_recover<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            32 * IBFT_RTAB_WORDS * 4));
+  }
 #if IBFT_WC > 0
   CU(cudaFuncSetAttribute(k_recover_split, cudaFuncAttributeMaxDynamicSharedMemorySize, IBFT_SPLIT_SMEM));
   CU(cudaFuncSetAttribute(k_verify_split, cudaFuncAttributeMaxDynamicSharedMemorySize, IBFT_VSPLIT_SMEM));
 #endif
-  CU(cudaFuncGetAttributes(&e->recover_attr, k_recover<IBFT_BLOCK>));
   {
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, p.device));
@@ -1892,6 +2066,9 @@ static int engine_alloc(ibft_engine* e) {
     CU(cudaGetLastError());
   }
 #endif
+  rc = wide_acquire(e, L->stream);
+  if (rc != IBFT_OK) return rc;
+  CU(cudaFuncGetAttributes(&e->recover_attr, recover_kernel<IBFT_BLOCK>(e)));
   CU(cudaDeviceSynchronize());
   return IBFT_OK;
 }
@@ -1911,6 +2088,26 @@ extern "C" int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count,
   return IBFT_OK;
 #else
   if (entries) *entries = 0;
+  (void)first; (void)out;
+  return count == 0 ? IBFT_OK : IBFT_ERR_INVALID_ARG;
+#endif
+}
+
+// test hook: copy `count` entries of the wide generator comb starting at entry `first` (entry p * entries + m - 1 = m * 2^(w p) G)
+extern "C" int ibft_debug_wtable(ibft_engine* e, uint32_t first, uint32_t count, uint8_t* out, int* w, uint32_t* entries, uint32_t* total) {
+  if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+  if (w) *w = e->d_wtable ? IBFT_GEN_WIDE : 0;
+#if IBFT_GEN_WIDE > 0
+  if (entries) *entries = IBFT_GW_ENTRIES;
+  if (total) *total = (uint32_t)IBFT_GW_TOTAL;
+  if (count == 0) return IBFT_OK;
+  if (!e->d_wtable || !out || (size_t)first + count > IBFT_GW_TOTAL) { set_err("range"); return IBFT_ERR_INVALID_ARG; }
+  CU(cudaSetDevice(e->p.device));
+  CU(cudaMemcpy(out, e->d_wtable + (size_t)first * IBFT_GTAB_ENTRY_WORDS, (size_t)count * 64, cudaMemcpyDeviceToHost));
+  return IBFT_OK;
+#else
+  if (entries) *entries = 0;
+  if (total) *total = 0;
   (void)first; (void)out;
   return count == 0 ? IBFT_OK : IBFT_ERR_INVALID_ARG;
 #endif
@@ -2640,21 +2837,22 @@ static int launch_recover(ibft_engine* e, lane* L, const ibft_sig_item* d_items,
                                                                                     e->d_slots, e->p.max_table_slots, d_bitmap, nullptr, nullptr,
                                                                                     e->d_ctable, sink, worklist);
     } else {
-      k_recover<IBFT_BLOCK><<<(cnt + IBFT_BLOCK - 1) / IBFT_BLOCK, IBFT_BLOCK, IBFT_BLOCK * IBFT_RTAB_WORDS * 4, st>>>(
+      recover_kernel<IBFT_BLOCK>(e)<<<(cnt + IBFT_BLOCK - 1) / IBFT_BLOCK, IBFT_BLOCK, IBFT_BLOCK * IBFT_RTAB_WORDS * 4, st>>>(
           d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots, e->p.max_table_slots, d_bitmap, nullptr, nullptr, e->d_ctable,
-          sink, worklist);
+          sink, worklist, e->d_wtable);
     }
     CU(cudaEventRecord(L->wl_ev[worklist_index & 3u], st));
   } else
 #endif
   if (small_batch) {  // one-warp CTAs
     uint32_t blocks = (cnt + 31) / 32;
-    k_recover<32><<<blocks, 32, 32 * IBFT_RTAB_WORDS * 4, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots,
-                                         e->p.max_table_slots, d_bitmap, d_recovered, d_status, e->d_ctable, sink, nullptr);
+    recover_kernel<32>(e)<<<blocks, 32, 32 * IBFT_RTAB_WORDS * 4, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots,
+                                         e->p.max_table_slots, d_bitmap, d_recovered, d_status, e->d_ctable, sink, nullptr, e->d_wtable);
   } else {
     uint32_t blocks = (cnt + IBFT_BLOCK - 1) / IBFT_BLOCK;
-    k_recover<IBFT_BLOCK><<<blocks, IBFT_BLOCK, IBFT_BLOCK * IBFT_RTAB_WORDS * 4, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots,
-                                                         e->p.max_table_slots, d_bitmap, d_recovered, d_status, e->d_ctable, sink, nullptr);
+    recover_kernel<IBFT_BLOCK>(e)<<<blocks, IBFT_BLOCK, IBFT_BLOCK * IBFT_RTAB_WORDS * 4, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots,
+                                                         e->p.max_table_slots, d_bitmap, d_recovered, d_status, e->d_ctable, sink, nullptr,
+                                                         e->d_wtable);
   }
   e->launches++;
   CU(cudaGetLastError());

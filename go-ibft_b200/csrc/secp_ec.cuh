@@ -9,6 +9,8 @@
 //     data-dependent digit positions would leave ~5/6 of the lanes idle in every addition);
 //   * the generator table ({1..2^(WG-1)} * G, affine, with beta*x alongside) is staged in shared memory once per
 //     CTA; the per-signature table {1..8} * R lives in thread-local memory;
+//   * the one-thread recovery takes u1*G from a WIDE comb in HBM (IBFT_GEN_WIDE = 22: m * 2^(22 j) * G, 12 positions,
+//     1.38 GiB per device, shared by every engine of the process): at most 12 mixed additions and no doubling;
 //   * exceptional cases (P + P, P - P, infinity) are handled exactly -- adversarial signatures can reach them
 //     and the verdict must be bit-exact with the oracle -- but by rarely-taken branches.
 #pragma once
@@ -519,11 +521,62 @@ static_assert(IBFT_WG % IBFT_WR == 0, "generator window must be a multiple of th
 #define IBFT_CTAB_ENTRIES (((1 << (IBFT_WC - 1)) + 1) * IBFT_CTAB_D2)
 #define IBFT_CTAB_POSITIONS ((IBFT_NWIN_R * IBFT_WR + IBFT_WC - 1) / IBFT_WC)  // comb positions covering the 132 window bits
 
+// WIDE generator comb of the one-thread recovery (IBFT_GEN_WIDE = its window w; 0 = off): a 1-D signed-window comb over u1
+// itself, without the GLV split.  Position j (0 .. IBFT_GW_POSITIONS - 1) holds m * 2^(w j) * G for m = 1 .. 2^(w-1), affine, 64
+// bytes per entry in the generator-table format; the top position only the m <= 2^(256 - w j) + 1 that a scalar below n can
+// reach.  w = 22: 12 positions, 11 x 128 MiB + 1 MiB = 1.38 GiB of HBM, one table per device shared by every engine of the
+// process (engine.cu); u1*G costs at most 12 mixed additions instead of the 17 of the per-position comb below.
+#ifndef IBFT_GEN_WIDE
+#define IBFT_GEN_WIDE 22
+#endif
+#if IBFT_WC == 0 || defined(IBFT_RECOVER_TABLE_INV)
+#undef IBFT_GEN_WIDE
+#define IBFT_GEN_WIDE 0  // only the inversion-free one-thread recovery reads it
+#endif
+#if IBFT_GEN_WIDE > 0
+#define IBFT_GW_POSITIONS ((256 + IBFT_GEN_WIDE - 1) / IBFT_GEN_WIDE)
+#define IBFT_GW_ENTRIES (1u << (IBFT_GEN_WIDE - 1))  // entries of every position but the top one
+#define IBFT_GW_TOP_BITS (256 - IBFT_GEN_WIDE * (IBFT_GW_POSITIONS - 1))
+#define IBFT_GW_TOP_ENTRIES ((1u << IBFT_GW_TOP_BITS) + 1u)
+#define IBFT_GW_TOTAL ((size_t)(IBFT_GW_POSITIONS - 1) * IBFT_GW_ENTRIES + IBFT_GW_TOP_ENTRIES)
+static_assert(IBFT_GW_TOP_BITS < IBFT_GEN_WIDE - 1, "the top digit of a scalar below n must stay below 2^(w-1): no sign, no carry out");
+#endif
+
 // Generator table accessor: entry i (0-based) = (i+1)*G as 16 words x[8] y[8] (shared memory on the device).
 #define IBFT_GTAB_ENTRY_WORDS 16
 struct gtab_view {
   const uint32_t* base;
   const uint32_t* comb = nullptr;  // combined table (global memory) or nullptr
+  const uint32_t* wide = nullptr;  // wide generator comb (global memory) or nullptr
+  // entry m of position pos of the wide comb: the device reads the table; the host emulation computes the entry through
+  // `host_wide` (a 1.38 GiB table is not built there)
+#if !defined(__CUDA_ARCH__)
+  void (*host_wide)(int pos, int m, uint32_t* xy16) = nullptr;
+#endif
+  IBFT_HD bool has_wide() const {
+#if defined(__CUDA_ARCH__)
+    return wide != nullptr;
+#else
+    return host_wide != nullptr;
+#endif
+  }
+#if IBFT_GEN_WIDE > 0
+  IBFT_HD const uint32_t* wide_entry(int pos, int m) const {
+    return wide + (size_t)IBFT_GTAB_ENTRY_WORDS * ((size_t)pos * IBFT_GW_ENTRIES + (size_t)(m - 1));
+  }
+  IBFT_HD void load_gen_wide(int pos, int m, fe& x, fe& y) const {
+#if defined(__CUDA_ARCH__)
+    const uint4* q = reinterpret_cast<const uint4*>(wide_entry(pos, m));
+    uint4 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 2), d = __ldg(q + 3);
+    x.v[0] = a.x; x.v[1] = a.y; x.v[2] = a.z; x.v[3] = a.w; x.v[4] = b.x; x.v[5] = b.y; x.v[6] = b.z; x.v[7] = b.w;
+    y.v[0] = c.x; y.v[1] = c.y; y.v[2] = c.z; y.v[3] = c.w; y.v[4] = d.x; y.v[5] = d.y; y.v[6] = d.z; y.v[7] = d.w;
+#else
+    uint32_t e[16];
+    host_wide(pos, m, e);
+    for (int i = 0; i < 8; i++) { x.v[i] = e[i]; y.v[i] = e[8 + i]; }
+#endif
+  }
+#endif
   IBFT_HD void load_comb(int d1, int d2, fe& x, fe& y) const {
     const uint32_t* e = comb + (size_t)IBFT_GTAB_ENTRY_WORDS * ((size_t)d1 * IBFT_CTAB_D2 + (size_t)(d2 + (1 << (IBFT_WC > 0 ? IBFT_WC - 1 : 0))));
 #if defined(__CUDA_ARCH__)
@@ -680,8 +733,13 @@ IBFT_HD fe ecmult_build_rtable_globalz(const aff& R, const rtab_view& T) {
 
 // digit streams of one double-scalar multiplication: 0 = u2 half 1 (R), 1 = u2 half 2 (lambda R), 2 = u1 half 1 (G),
 // 3 = u1 half 2 (lambda G); magnitudes < 2^129 in five limbs (+ one zero limb for the Booth window reads), signs apart
+// With the wide generator comb, streams 2 and 3 hold u1 itself instead of its split: words 12..23 of `flat` are its 8 limbs
+// and four zero words (ecmult_wide_into).
 struct ecmult_digits {
-  uint32_t ks[4][6];
+  union {
+    uint32_t ks[4][6];
+    uint32_t flat[24];
+  };
   bool kneg[4];
 };
 IBFT_HD void ecmult_split_into(const sc& k, ecmult_digits& d, int first) {
@@ -864,6 +922,50 @@ IBFT_HD void ecmult_gen_comb_prefetch(const ecmult_digits& dg, const gtab_view& 
     if (d1 < 0 || (d1 == 0 && d2 < 0)) { d1 = -d1; d2 = -d2; }
     const uint32_t* e = G.comb + (size_t)jg * IBFT_GTAB_ENTRY_WORDS * (size_t)IBFT_CTAB_ENTRIES +
                         (size_t)IBFT_GTAB_ENTRY_WORDS * ((size_t)d1 * IBFT_CTAB_D2 + (size_t)(d2 + (1 << (IBFT_WC - 1))));
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(e));
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(e + 8));
+  }
+#else
+  (void)dg;
+  (void)G;
+#endif
+}
+#endif
+
+#if IBFT_GEN_WIDE > 0
+// u1 itself into streams 2 and 3, for the wide comb (no GLV split)
+IBFT_HD void ecmult_wide_into(const sc& k, ecmult_digits& d) {
+#pragma unroll
+  for (int i = 0; i < 12; i++) d.flat[12 + i] = i < 8 ? k.v[i] : 0u;
+}
+
+// u1*G as the wide comb over u1's own Booth digits: one mixed addition per non-zero digit, at most IBFT_GW_POSITIONS, no doubling.
+// dg must hold u1 by ecmult_wide_into.
+IBFT_HD jac ecmult_gen_wide(const ecmult_digits& dg, const gtab_view& G) {
+  jac acc;
+  acc.x = fe_zero(); acc.y = fe_zero(); acc.z = fe_zero();
+  acc.inf = true;
+  IBFT_ROLLED
+  for (int j = IBFT_GW_POSITIONS - 1; j >= 0; j--) {
+    const int d = booth_digit<IBFT_GEN_WIDE, 12>(dg.flat + 12, j);
+    if (d == 0) continue;
+    fe x, y;
+    G.load_gen_wide(j, d < 0 ? -d : d, x, y);
+    if (d < 0) y = fe_neg(y);
+    IBFT_OPCOUNT(IBFT_OP_COMB_ADD);
+    acc = jac_add_affine(acc, x, y);
+  }
+  return acc;
+}
+
+// L2 prefetch of the wide comb entries ecmult_gen_wide is about to read (1.38 GiB: a random entry is never in L2 already)
+IBFT_HD void ecmult_gen_wide_prefetch(const ecmult_digits& dg, const gtab_view& G) {
+#if defined(__CUDA_ARCH__)
+  IBFT_ROLLED
+  for (int j = IBFT_GW_POSITIONS - 1; j >= 0; j--) {
+    const int d = booth_digit<IBFT_GEN_WIDE, 12>(dg.flat + 12, j);
+    if (d == 0) continue;
+    const uint32_t* e = G.wide_entry(j, d < 0 ? -d : d);
     asm volatile("prefetch.global.L2 [%0];" ::"l"(e));
     asm volatile("prefetch.global.L2 [%0];" ::"l"(e + 8));
   }

@@ -321,10 +321,10 @@ IBFT_HD void glv_split(const sc& k, glv_half& h1, glv_half& h2) {
   }
 }
 
-// Signed fixed-window (Booth) digit j of a non-negative scalar stored as 6 limbs (top limb zero-padded):
+// Signed fixed-window (Booth) digit j of a non-negative scalar stored as NL limbs (top limb zero-padded):
 //   d_j = k[wj .. wj+w-1] + k[wj-1] - 2^w * k[wj+w-1]   in [-2^(w-1), 2^(w-1)],   k = sum d_j 2^(wj)
 // Every window is independent of the others, so all lanes of a warp add at the same loop positions.
-template <int W>
+template <int W, int NL = 6>
 IBFT_HD int booth_digit(const uint32_t* k6, int j) {
   int pos = W * j - 1;  // lowest bit of the (W+1)-bit field; -1 for j = 0
   uint32_t field;
@@ -332,7 +332,7 @@ IBFT_HD int booth_digit(const uint32_t* k6, int j) {
     field = (k6[0] << 1) & ((2u << W) - 1u);
   } else {
     int limb = pos >> 5, sh = pos & 31;
-    uint64_t two = (uint64_t)k6[limb] | ((uint64_t)(limb + 1 < 6 ? k6[limb + 1] : 0u) << 32);
+    uint64_t two = (uint64_t)k6[limb] | ((uint64_t)(limb + 1 < NL ? k6[limb + 1] : 0u) << 32);
     field = (uint32_t)(two >> sh) & ((2u << W) - 1u);
   }
   int d = (int)((field + 1u) >> 1);       // window value (bits 1..W) + carry-in bit 0

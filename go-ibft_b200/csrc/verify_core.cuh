@@ -356,7 +356,8 @@ IBFT_HD bool recover_key(const EX& ex, const sc& r, const sc& s, uint8_t v, cons
 //      is made "effective affine" without an inversion (ecmult_build_rtable_globalz), and the window loop walks the R streams
 //      only.  Its result (X, Y, Z) on E' with the table's Z_8 is the Jacobian point A = (X, Y, W0 y) of E, W0 = Z Z_8: y stays
 //      unknown.
-//   2. u1 * G by the comb over the per-position tables (ecmult_gen_comb, no doubling) into B = (Xb, Yb, Zb).
+//   2. u1 * G by a comb, no doubling, into B = (Xb, Yb, Zb): the wide comb over u1's own digits when the engine holds it
+//      (ecmult_gen_wide, at most 12 additions), else the per-position comb over u1's GLV split (ecmult_gen_comb, 17).
 //   3. A + B (recover_final): Z_A^2 = W0^2 c needs no root, so H and V = W0 Zb H do not depend on y; ONE exponentiation of
 //      c V^4 gives y = sqrt(c) and 1 / (y V) = 1 / Z3 (fe_sqrt_inv), then S2 and the rest of the addition use y.
 // A = (X, Y, W0) is held with Z = W0 (the factor y kept apart); the rare cases are exact: A = +-B, u1 = 0, a non-residue c.
@@ -425,18 +426,26 @@ IBFT_HD bool recover_final(const jac& A, const fe& c, uint8_t v, const jac& B, f
   return recover_affine(x3, y3, w, qx, qy);
 }
 
-IBFT_HD bool recover_key(const exec_serial& ex, const sc& r, const sc& s, uint8_t v, const uint8_t* z_be, const gtab_view& G,
-                         const rtab_view& T, fe& qx, fe& qy) {
-#if !defined(__CUDA_ARCH__)
-  // the host emulation supplies the per-position comb entries through host_pos; without them it runs the composition above
-  if (G.host_pos == nullptr) return recover_key<exec_serial>(ex, r, s, v, z_be, G, T, qx, qy);
-#endif
+// WIDE: u1*G by the wide comb, else by the per-position comb.  Each kernel instantiation holds only one of the two loops (the
+// engine launches the wide one when it holds the table): with both behind a run-time branch the kernel ran 0.7 % slower on an H100.
+template <bool WIDE>
+IBFT_HD bool recover_key_serial(const sc& r, const sc& s, uint8_t v, const uint8_t* z_be, const gtab_view& G, const rtab_view& T,
+                                fe& qx, fe& qy) {
   // u1 = -z/r, u2 = s/r  (mod n)
   sc z = sc_reduce_once(sc_from_be(z_be));
   sc rinv = IBFT_SC_INV(r);
   ecmult_digits dg;
   ecmult_split_into(sc_mul(s, rinv), dg, 0);
-  ecmult_split_into(sc_neg(sc_mul(z, rinv)), dg, 2);
+  const sc u1 = sc_neg(sc_mul(z, rinv));
+#if IBFT_GEN_WIDE > 0
+  if (WIDE) {
+    ecmult_wide_into(u1, dg);
+    // the 12 gathers out of 1.38 GiB start here, a whole window loop before the comb reads them (they are prefetched again
+    // right before it, in case L2 let them go): +0.5 % on an H100 over prefetching only before the comb
+    ecmult_gen_wide_prefetch(dg, G);
+  } else
+#endif
+    ecmult_split_into(u1, dg, 2);
   IBFT_STAGE(3);
   // phi(R) on E' and its inversion-free table; c = x^3 + 7
   fe x;
@@ -455,13 +464,40 @@ IBFT_HD bool recover_key(const exec_serial& ex, const sc& r, const sc& s, uint8_
   const bool a_inf = A.inf;
   T.store(0, A.x, A.y);
   T.store(1, fe_mul(A.z, z8), c);
-  ecmult_gen_comb_prefetch(dg, G);
-  const jac B = ecmult_gen_comb(dg, G);
+  jac B;
+#if IBFT_GEN_WIDE > 0
+  if (WIDE) {
+    ecmult_gen_wide_prefetch(dg, G);
+    B = ecmult_gen_wide(dg, G);
+  } else
+#endif
+  {
+    ecmult_gen_comb_prefetch(dg, G);
+    B = ecmult_gen_comb(dg, G);
+  }
   T.load(0, A.x, A.y);
   T.load(1, A.z, c);
   A.inf = a_inf;
   return recover_final(A, c, v, B, qx, qy);
 }
+IBFT_HD bool recover_key(const exec_serial& ex, const sc& r, const sc& s, uint8_t v, const uint8_t* z_be, const gtab_view& G,
+                         const rtab_view& T, fe& qx, fe& qy) {
+#if !defined(__CUDA_ARCH__)
+  // the host emulation supplies the comb entries through host_pos or host_wide; without them it runs the composition above
+  if (G.has_wide()) return recover_key_serial<true>(r, s, v, z_be, G, T, qx, qy);
+  if (G.host_pos == nullptr) return recover_key<exec_serial>(ex, r, s, v, z_be, G, T, qx, qy);
+#endif
+  (void)ex;
+  return recover_key_serial<false>(r, s, v, z_be, G, T, qx, qy);
+}
+#if IBFT_GEN_WIDE > 0
+// the one-thread recovery with u1*G from the wide comb (G.wide must be set)
+struct exec_serial_wide : exec_serial {};
+IBFT_HD bool recover_key(const exec_serial_wide&, const sc& r, const sc& s, uint8_t v, const uint8_t* z_be, const gtab_view& G,
+                         const rtab_view& T, fe& qx, fe& qy) {
+  return recover_key_serial<true>(r, s, v, z_be, G, T, qx, qy);
+}
+#endif
 #endif
 
 // Recover the signer of (r, s, v) over digest z.  Returns false when the signature is invalid; addr20 then zero.

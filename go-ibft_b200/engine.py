@@ -39,7 +39,7 @@ EXPORTS = [
     "ibft_verify_wait", "ibft_bind_groups", "ibft_verify_batch_device", "ibft_quorum_reduce_device", "ibft_quorum_partial_words", "ibft_quorum_mark_device", "ibft_quorum_merge_device", "ibft_quorum_exchange_device",
     "ibft_exchange_alloc", "ibft_exchange_open", "ibft_exchange_close", "ibft_exchange_free", "ibft_exchange_clear",
     "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_set_key_table_budget", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
-    "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
+    "ibft_debug_wtable", "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
 ]
 
 
@@ -110,6 +110,7 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.ibft_sign_batch.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]
     lib.ibft_probe_int_peak.argtypes = [c_void_p, POINTER(c_double), POINTER(c_double)]
     lib.ibft_debug_ctable.argtypes = [c_void_p, c_uint32, c_uint32, c_void_p, POINTER(c_int), POINTER(c_uint32)]
+    lib.ibft_debug_wtable.argtypes = [c_void_p, c_uint32, c_uint32, c_void_p, POINTER(c_int), POINTER(c_uint32), POINTER(c_uint32)]
     lib.ibft_debug_keytab.argtypes = [c_void_p, c_uint32, c_uint32, c_uint32, c_uint32, c_void_p, POINTER(c_uint32), c_void_p]
     lib.ibft_debug_key_registry.argtypes = [c_void_p, POINTER(c_uint32), POINTER(c_uint32), POINTER(c_uint64)]
     lib.ibft_debug_known_handed_back.argtypes = [c_void_p, POINTER(c_uint32)]
@@ -400,6 +401,18 @@ class Engine:
         """entries of the generator comb tables: index p * entries + i = entry i of comb position p (position 0 = combined table)"""
         out = np.zeros((count, 16), dtype=np.uint32)
         self._check(self.lib.ibft_debug_ctable(self.handle, first, count, _ptr(out), None, None))
+        return out
+
+    def wide_table_info(self):
+        """(w, entries per position, entries in all) of the wide generator comb; w = 0 when the engine has none"""
+        w, n, total = c_int(), c_uint32(), c_uint32()
+        self._check(self.lib.ibft_debug_wtable(self.handle, 0, 0, None, ctypes.byref(w), ctypes.byref(n), ctypes.byref(total)))
+        return int(w.value), int(n.value), int(total.value)
+
+    def wide_table_entries(self, first: int, count: int) -> np.ndarray:
+        """entries of the wide generator comb: index p * entries + m - 1 = m * 2^(w p) * G"""
+        out = np.zeros((count, 16), dtype=np.uint32)
+        self._check(self.lib.ibft_debug_wtable(self.handle, first, count, _ptr(out), None, None, None))
         return out
 
     def key_table(self, slot: int, validator: int, first: int = 0, count: int = 0):

@@ -390,6 +390,11 @@ int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* wide_mac_per
  * other: entry p * entries + d1 * (2^wc + 1) + d2 + 2^(wc-1) holds (d1 + d2*lambda) * 2^(wc*p) * G, p = 0..16 (position 0 is
  * the combined table d1*G + d2*lambda*G). */
 int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count, uint8_t* out, int* wc, uint32_t* entries);
+/* Wide generator comb of the one-thread recovery: *w = window (0 when the engine has none: the library was built without it, or
+ * the device could not hold it), *entries = entries of one position (2^(w-1)), *total = entries of the whole table; copies
+ * `count` 64-byte entries (format of ibft_debug_ctable) starting at `first`: entry p * entries + m - 1 holds m * 2^(w p) * G,
+ * m = 1..entries (the top position only its first total - p * entries).  Any output may be NULL. */
+int ibft_debug_wtable(ibft_engine* e, uint32_t first, uint32_t count, uint8_t* out, int* w, uint32_t* entries, uint32_t* total);
 /* Key registry entry of validator `validator` (validator-index order) of a table slot: *state_out = 0 unknown, 1 learned,
  * 2 comb table built (a key known in a bounded registry without a table reads 1); key_out (64 bytes) = the learned affine key, x then y as 8 little-endian words; out = `count` comb
  * entries starting at `first` in the format of ibft_debug_ctable, entry j * 128 + m - 1 = m * 2^(8j) * Q (j = 0..16,

@@ -5,11 +5,12 @@ The recover kernel is bound by the FMA-heavy pipe (DESIGN.md §3.1): an IMAD.WID
 instruction, every other IMAD-class instruction (IMAD.MOV, IMAD.X, IMAD.HI, ...) for 2.  This tool puts a number on that
 pipe's work per recovery without a GPU:
 
-  static   the SASS of k_recover<128> (cuobjdump): every out-of-line routine it calls (fe_mul, fe_sqr, fe_sqrn, the doubling's
+  static   the SASS of k_recover<128, true> (cuobjdump; the instantiation an engine holding the wide comb runs): every out-of-line routine it calls (fe_mul, fe_sqr, fe_sqrn, the doubling's
            fused front end, the safegcd inversion, the root-and-inverse exponentiation fe_sqrt_inv), the window loop and the
-           u1*G comb loop after it, found by their back branches;
+           u1*G loop of the wide generator comb after it (ecmult_gen_wide), found by their back branches;
   dynamic  how often each of them runs per recovery, counted by the host emulation of the same sources (IBFT_OPCOUNT,
-           tests/emul/recover_comb.cpp: the product's one-thread composition) over the config-3 items (tests/golden/config3.npz).
+           tests/emul/recover_wide.cpp: the product's one-thread composition with the wide comb) over the config-3 items
+           (tests/golden/config3.npz).
 
 It prints per-routine instruction counts, then estimated FMA-pipe cycles, IMAD.WIDE and products per recovery and the
 hot-loop code size (window loop + every routine it calls outside the P + P block).  The estimate covers the field routines, the inversions and the
@@ -35,7 +36,7 @@ import tempfile
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KERNEL = "_Z9k_recoverILi128EEvPK13ibft_sig_itemjPKhmjjPK15ibft_group_descjPK8slot_devjPjPhSC_PKj9vote_sinkSE_"
+KERNEL = "_Z9k_recoverILi128ELb1EEvPK13ibft_sig_itemjPKhmjjPK15ibft_group_descjPK8slot_devjPjPhSC_PKj9vote_sinkSE_SE_"
 CUOBJDUMP = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "cuobjdump")
 
 # IBFT_OP_* of csrc/secp_fe.cuh
@@ -155,7 +156,8 @@ def cold_block(add_loop, bounds, names):
 
 
 def comb_loop(body, window_tail):
-    """the u1*G comb loop: the first loop after the window loop that makes calls (the prefetch loop before it makes none)"""
+    """the u1*G loop of the wide comb: the first loop after the window loop that makes calls (the prefetch loop before it makes
+    none)"""
     after = sorted((h, t) for h, t in loops(body) if h > window_tail and tally(span(body, h, t))["call"])
     if not after:
         raise SystemExit("comb loop not found in the SASS")
@@ -163,11 +165,11 @@ def comb_loop(body, window_tail):
 
 
 def counting_emulation(out_dir: str) -> ctypes.CDLL:
-    """the host emulation of the product's one-thread composition with its operation counters (tests/emul/recover_comb.cpp)"""
+    """the host emulation of the product's one-thread composition with its operation counters (tests/emul/recover_wide.cpp)"""
     emul = os.path.join(ROOT, "tests", "emul")
-    so = os.path.join(out_dir, "libibft_recover_comb.so")
+    so = os.path.join(out_dir, "libibft_recover_wide.so")
     subprocess.check_call([os.environ.get("CXX", "g++"), "-O2", "-fPIC", "-std=c++17", '-DEMUL_DIR="%s"' % emul, "-shared", "-o",
-                           so, os.path.join(emul, "recover_comb.cpp"), "-lpthread"])
+                           so, os.path.join(emul, "recover_wide.cpp"), "-lpthread"])
     return ctypes.CDLL(so)
 
 
@@ -181,10 +183,10 @@ def op_counts(items_limit: int):
         items = items[:items_limit]
     out = (ctypes.c_uint8 * 20)()
     ap = arena.ctypes.data_as(ctypes.c_void_p)
-    E.emul_verify_item_comb(items[0].ctypes.data_as(ctypes.c_void_p), ap, ctypes.c_size_t(len(arena)), out)  # builds the emulation's tables
+    E.emul_verify_item_wide(items[0].ctypes.data_as(ctypes.c_void_p), ap, ctypes.c_size_t(len(arena)), out)  # builds the emulation's tables
     E.emul_op_reset()
     for i in range(len(items)):
-        E.emul_verify_item_comb(items[i].ctypes.data_as(ctypes.c_void_p), ap, ctypes.c_size_t(len(arena)), out)
+        E.emul_verify_item_wide(items[i].ctypes.data_as(ctypes.c_void_p), ap, ctypes.c_size_t(len(arena)), out)
     buf = (ctypes.c_ulonglong * 32)()
     n = E.emul_op_counts_all(buf)
     assert n <= len(OPS), "IBFT_OP_* of secp_fe.cuh and OPS of this tool disagree"
