@@ -1,4 +1,5 @@
-// debug_arith.cuh -- the arithmetic parity hooks IBFT_DBG_FE_MUL_RAW .. IBFT_DBG_SC_DIGITS of include/ibft_verify.h (TEST ONLY).
+// debug_arith.cuh -- the arithmetic parity hooks IBFT_DBG_FE_MUL_RAW .. IBFT_DBG_SC_DIGITS and IBFT_DBG_RFC6979 of
+// include/ibft_verify.h (TEST ONLY).
 //
 // One body for the device (k_debug_op in engine.cu) and the host emulation (emul_debug_op in tests/emul/emul.cpp), so both run
 // the very routines the kernels run, on the same operands, and hand back their raw limbs: the tests chain non-canonical values
@@ -6,11 +7,13 @@
 #pragma once
 #include "../../include/ibft_verify.h"
 #include "secp_ec.cuh"
+#include "sha256.cuh"
 
 namespace ibft {
 
-// a, b: 32-byte big-endian operands; o: the op's output (see ibft_verify.h).  Returns false for an op it does not handle.
-IBFT_HD bool debug_arith_op(int op, const uint8_t* a, const uint8_t* b, uint8_t* o) {
+// a, b: 32-byte big-endian operands; o: the op's output (see ibft_verify.h); c: the 64-byte third operand of IBFT_DBG_RFC6979.
+// Returns false for an op it does not handle, and for IBFT_DBG_RFC6979 without c.
+IBFT_HD bool debug_arith_op(int op, const uint8_t* a, const uint8_t* b, uint8_t* o, const uint8_t* c = nullptr) {
   switch (op) {
     case IBFT_DBG_FE_MUL_RAW: fe_to_be(fe_mul(fe_from_be(a), fe_from_be(b)), o); return true;
     case IBFT_DBG_FE_SQR_RAW: fe_to_be(fe_sqr(fe_from_be(a)), o); return true;
@@ -44,6 +47,13 @@ IBFT_HD bool debug_arith_op(int op, const uint8_t* a, const uint8_t* b, uint8_t*
           q[73 + 2 * j] = (uint8_t)((d >> 8) & 0xFF);
         }
       }
+      return true;
+    }
+    case IBFT_DBG_RFC6979: {  // raw nonce candidate c[63] for the key a and the digest b
+      if (c == nullptr) return false;
+      uint8_t zm[32];
+      sc_to_be(sc_reduce_once(sc_from_be(b)), zm);
+      rfc6979_candidate(a, zm, c[63], o);
       return true;
     }
     default: return false;

@@ -1554,9 +1554,11 @@ k_adopt_entries(uint32_t* __restrict__ key_ref, uint32_t n, uint32_t* __restrict
 // ------------------------------------------------------------------------------------------------------------
 // batched signing (MessageConstructor side)
 // ------------------------------------------------------------------------------------------------------------
+// Three nonce modes: given (nonces != nullptr), Keccak-derived (nonces == nullptr), and libsecp256k1's RFC 6979 nonce (rfc6979,
+// ibft_sign_batch_rfc6979; nonces is then ignored).
 __global__ void __launch_bounds__(64)
-k_sign(const uint8_t* __restrict__ privkeys, const uint8_t* __restrict__ digests, const uint8_t* __restrict__ nonces, uint32_t n,
-       uint8_t* __restrict__ sigs) {
+k_sign(const uint8_t* __restrict__ privkeys, const uint8_t* __restrict__ digests, const uint8_t* __restrict__ nonces, bool rfc6979,
+       uint32_t n, uint8_t* __restrict__ sigs) {
   __shared__ uint32_t s_gtab[IBFT_GTAB_ENTRY_WORDS * IBFT_GTAB_ENTRIES];
   __shared__ uint32_t s_rtab[64 * IBFT_RTAB_WORDS];
   for (uint32_t i = threadIdx.x; i < IBFT_GTAB_ENTRY_WORDS * IBFT_GTAB_ENTRIES; i += 64) s_gtab[i] = g_gtable[i];
@@ -1569,7 +1571,9 @@ k_sign(const uint8_t* __restrict__ privkeys, const uint8_t* __restrict__ digests
   gtab_view G{s_gtab};
   rtab_view T{s_rtab + threadIdx.x, 64u};
   bool ok = false;
-  if (nonces != nullptr) {
+  if (rfc6979) {
+    ok = ecdsa_sign_rfc6979(d, z, G, T, sig);
+  } else if (nonces != nullptr) {
 #pragma unroll
     for (int j = 0; j < 32; j++) k[j] = nonces[32 * (size_t)i + j];
     ok = ecdsa_sign(d, z, k, G, T, sig);
@@ -1644,7 +1648,7 @@ __global__ void k_debug_op(int op, const uint8_t* a, const uint8_t* b, const uin
       }
       break;
     }
-    default: debug_arith_op(op, pa, pb, o); break;
+    default: debug_arith_op(op, pa, pb, o, c ? c + 64 * (size_t)i : nullptr); break;
   }
 }
 
@@ -3455,8 +3459,8 @@ extern "C" int ibft_proposal_hash_batch(ibft_engine* e, const uint8_t* arena, si
   return hash_batch_locked(e, arena, arena_len, offsets, lens, rounds, n, out32);
 }
 
-extern "C" int ibft_sign_batch(ibft_engine* e, const uint8_t* privkeys, const uint8_t* digests, const uint8_t* nonces, uint32_t n,
-                               uint8_t* sigs65_out) {
+static int sign_batch(ibft_engine* e, const uint8_t* privkeys, const uint8_t* digests, const uint8_t* nonces, bool rfc6979,
+                      uint32_t n, uint8_t* sigs65_out) {
   if (!e || (n && (!privkeys || !digests || !sigs65_out))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   if (n == 0) return IBFT_OK;
   lane* L = &e->lanes[0];
@@ -3475,7 +3479,7 @@ extern "C" int ibft_sign_batch(ibft_engine* e, const uint8_t* privkeys, const ui
     CUK(cudaMalloc(&d_k, (size_t)n * 32));
     CUK(cudaMemcpyAsync(d_k, nonces, (size_t)n * 32, cudaMemcpyHostToDevice, L->stream));
   }
-  k_sign<<<(n + 63) / 64, 64, 0, L->stream>>>(d_d, d_z, d_k, n, d_s);
+  k_sign<<<(n + 63) / 64, 64, 0, L->stream>>>(d_d, d_z, d_k, rfc6979, n, d_s);
   e->launches++;
   CUK(cudaGetLastError());
   CUK(cudaMemcpyAsync(sigs65_out, d_s, (size_t)n * 65, cudaMemcpyDeviceToHost, L->stream));
@@ -3488,6 +3492,16 @@ done:
 #undef CUK
   cudaFree(d_d); cudaFree(d_z); cudaFree(d_k); cudaFree(d_s);
   return rc;
+}
+
+extern "C" int ibft_sign_batch(ibft_engine* e, const uint8_t* privkeys, const uint8_t* digests, const uint8_t* nonces, uint32_t n,
+                               uint8_t* sigs65_out) {
+  return sign_batch(e, privkeys, digests, nonces, false, n, sigs65_out);
+}
+
+extern "C" int ibft_sign_batch_rfc6979(ibft_engine* e, const uint8_t* privkeys, const uint8_t* digests, uint32_t n,
+                                       uint8_t* sigs65_out) {
+  return sign_batch(e, privkeys, digests, nullptr, true, n, sigs65_out);
 }
 
 extern "C" int ibft_set_recover_path(ibft_engine* e, int path) {
@@ -3536,7 +3550,7 @@ extern "C" int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* w
 
 extern "C" int ibft_debug_op(ibft_engine* e, int op, const uint8_t* a, const uint8_t* b, const uint8_t* c, uint32_t n,
                              uint8_t* out, uint32_t out_stride) {
-  if (!e || !a || !out || n == 0) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  if (!e || !a || !out || n == 0 || (op == IBFT_DBG_RFC6979 && (!b || !c))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
   CU(cudaSetDevice(e->p.device));

@@ -9,6 +9,7 @@
 #include "keccak.cuh"
 #include "secp_ec.cuh"
 #include "secp_modinv.cuh"
+#include "sha256.cuh"
 
 namespace ibft {
 
@@ -775,6 +776,36 @@ IBFT_HD bool ecdsa_sign(const uint8_t* d_be, const uint8_t* z_be, const uint8_t*
   sc_to_be(s, sig65 + 32);
   sig65[64] = v;
   return true;
+}
+
+// ECDSA signing with libsecp256k1's default nonce: secp256k1_ecdsa_sign_recoverable with nonce_function_rfc6979, which is what
+// go-ethereum's crypto.Sign runs (the contract of ibft_sign_batch_rfc6979).  sig65 = R||S||V as ecdsa_sign makes it.  Returns
+// false (sig65 all zero) for a key outside [1, n), for R.x >= n, where libsecp256k1 would answer with recovery id 2 or 3, and
+// when four candidates gave no signature.
+IBFT_HD bool ecdsa_sign_rfc6979(const uint8_t* d_be, const uint8_t* z_be, const gtab_view& G, const rtab_view& T, uint8_t* sig65) {
+  const sc d = sc_from_be(d_be);
+  if (!sc_is_zero(d) && !sc_ge_n(d)) {
+    uint8_t zm[32], z1[32], k[32];
+    sc_to_be(sc_reduce_once(sc_from_be(z_be)), zm);
+    uint32_t carry = 1;  // z1 = (z mod n) + 1 < 2^256
+    for (int i = 31; i >= 0; i--) {
+      carry += zm[i];
+      z1[i] = (uint8_t)carry;
+      carry >>= 8;
+    }
+    for (uint32_t c = 0; c < 4; c++) {
+      rfc6979_candidate(d_be, zm, c, k);
+      const sc kc = sc_from_be(k);
+      if (sc_is_zero(kc) || sc_ge_n(kc)) continue;  // libsecp256k1 moves on to the next candidate
+      if (ecdsa_sign(d_be, zm, k, G, T, sig65)) return true;
+      // With d and k in [1, n) ecdsa_sign refuses only R.x >= n (r = 0 would need R.x = n: no point has x = 0) and s = 0.
+      // R does not depend on the digest, and s = k^-1 (z + r d) is k^-1 != 0 for the digest z + 1 where z gave 0.
+      if (!ecdsa_sign(d_be, z1, k, G, T, sig65)) break;  // R.x >= n: refused
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 65; i++) sig65[i] = 0;
+  return false;
 }
 
 }  // namespace ibft

@@ -22,7 +22,7 @@ QUORUM_DEFAULT, QUORUM_PREPREPARE, QUORUM_PREPARE = 0, 1, 2
 PROPOSER_NONE, PROPOSER_UNSET = 0xFFFFFFFF, 0xFFFFFFFE
 DBG = dict(FE_MUL=1, FE_SQR=2, FE_INV=3, FE_SQRT=4, SC_MUL=5, SC_INV=6, ECMULT=7, FE_ADD=8, FE_SUB=9, GLV=10,
            FE_MUL_RAW=11, FE_SQR_RAW=12, FE_ADD_RAW=13, FE_SUB_RAW=14, FE_NORMALIZE=15, FE_EQUAL=16, FE_SQRN=17, FE_SQRT_INV=18,
-           SC_ADD=19, SC_NEG=20, SC_REDUCE_ONCE=21, SC_DIGITS=22)
+           SC_ADD=19, SC_NEG=20, SC_REDUCE_ONCE=21, SC_DIGITS=22, RFC6979=23)
 
 # numpy mirrors of the ABI structs
 ITEM_DTYPE = np.dtype([
@@ -38,7 +38,7 @@ EXPORTS = [
     "ibft_set_validators", "ibft_get_quorum", "ibft_verify_batch", "ibft_verify_batch_ex", "ibft_last_item_status", "ibft_verify_submit", "ibft_verify_poll",
     "ibft_verify_wait", "ibft_bind_groups", "ibft_verify_batch_device", "ibft_quorum_reduce_device", "ibft_quorum_partial_words", "ibft_quorum_mark_device", "ibft_quorum_merge_device", "ibft_quorum_exchange_device",
     "ibft_exchange_alloc", "ibft_exchange_open", "ibft_exchange_close", "ibft_exchange_free", "ibft_exchange_clear",
-    "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_set_key_table_budget", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
+    "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_sign_batch_rfc6979", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_set_key_table_budget", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
     "ibft_debug_wtable", "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
 ]
 
@@ -108,6 +108,7 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.ibft_keccak256_batch.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_uint32, c_void_p]
     lib.ibft_proposal_hash_batch.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]
     lib.ibft_sign_batch.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]
+    lib.ibft_sign_batch_rfc6979.argtypes = [c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]
     lib.ibft_probe_int_peak.argtypes = [c_void_p, POINTER(c_double), POINTER(c_double)]
     lib.ibft_debug_ctable.argtypes = [c_void_p, c_uint32, c_uint32, c_void_p, POINTER(c_int), POINTER(c_uint32)]
     lib.ibft_debug_wtable.argtypes = [c_void_p, c_uint32, c_uint32, c_void_p, POINTER(c_int), POINTER(c_uint32), POINTER(c_uint32)]
@@ -390,6 +391,22 @@ class Engine:
         K = np.frombuffer(b"".join(x.to_bytes(32, "big") for x in nonces), dtype=np.uint8) if nonces is not None else None
         out = np.zeros((n, 65), dtype=np.uint8)
         self._check(self.lib.ibft_sign_batch(self.handle, _ptr(D), _ptr(Z), _ptr(K), n, _ptr(out)))
+        return [bytes(out[i]) for i in range(n)]
+
+    def sign_batch_rfc6979(self, privkeys: list[int], digests: list[bytes]) -> list[bytes]:
+        """65-byte R||S||V per row with libsecp256k1's RFC 6979 nonce: go-ethereum crypto.Sign's bytes (ibft_sign_batch_rfc6979).
+        Keys are 32-byte integers in [0, 2^256); a row whose key is 0 or >= n, or whose R.x >= n, comes back as 65 zero bytes."""
+        n = len(privkeys)
+        if n != len(digests):
+            raise ValueError("one digest per key")
+        if n == 0:
+            return []
+        if any(len(z) != 32 for z in digests):
+            raise ValueError("digests are 32 bytes")
+        D = np.frombuffer(b"".join(x.to_bytes(32, "big") for x in privkeys), dtype=np.uint8)
+        Z = np.frombuffer(b"".join(digests), dtype=np.uint8)
+        out = np.zeros((n, 65), dtype=np.uint8)
+        self._check(self.lib.ibft_sign_batch_rfc6979(self.handle, _ptr(D), _ptr(Z), n, _ptr(out)))
         return [bytes(out[i]) for i in range(n)]
 
     def combined_table_info(self):

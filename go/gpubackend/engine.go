@@ -329,3 +329,44 @@ func (e *Engine) Keccak256(data []byte) ([32]byte, error) {
 	}
 	return out, nil
 }
+
+// SignRFC6979 signs digests[i] with keys[i] on the device (ibft_sign_batch_rfc6979) and returns the 65-byte R||S||V of each:
+// the bytes go-ethereum's crypto.Sign returns for the same key and digest, so a validator's MessageConstructor can sign and
+// seal through the engine.  Keys and digests are 32 bytes each.  A row the engine refuses -- a key of 0 or >= n, or the
+// R.x >= n case where crypto.Sign would return a recovery id of 2 or 3 -- comes back as nil.
+// COMPILE-UNVERIFIED, like the rest of this package.
+func (e *Engine) SignRFC6979(keys, digests [][]byte) ([][]byte, error) {
+	n := len(keys)
+	if n != len(digests) {
+		return nil, errors.New("SignRFC6979: one digest per key")
+	}
+	if n == 0 {
+		return nil, nil
+	}
+	d := make([]byte, 32*n)
+	z := make([]byte, 32*n)
+	for i := range keys {
+		if len(keys[i]) != 32 || len(digests[i]) != 32 {
+			return nil, fmt.Errorf("SignRFC6979: row %d: keys and digests are 32 bytes", i)
+		}
+		copy(d[32*i:], keys[i])
+		copy(z[32*i:], digests[i])
+	}
+	sigs := make([]byte, 65*n)
+	rc := C.ibft_sign_batch_rfc6979(e.h, (*C.uint8_t)(unsafe.Pointer(&d[0])), (*C.uint8_t)(unsafe.Pointer(&z[0])), C.uint32_t(n),
+		(*C.uint8_t)(unsafe.Pointer(&sigs[0])))
+	for i := range d {
+		d[i] = 0 // the keys do not outlive the call on the Go heap either
+	}
+	if rc != C.IBFT_OK {
+		return nil, fmt.Errorf("ibft_sign_batch_rfc6979: %w", lastError())
+	}
+	out := make([][]byte, n)
+	var zero [65]byte
+	for i := range out {
+		if sig := sigs[65*i : 65*i+65]; string(sig) != string(zero[:]) {
+			out[i] = sig
+		}
+	}
+	return out, nil
+}

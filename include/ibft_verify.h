@@ -311,6 +311,24 @@ int ibft_proposal_hash_batch(ibft_engine* e, const uint8_t* arena, size_t arena_
 int ibft_sign_batch(ibft_engine* e, const uint8_t* privkeys, const uint8_t* digests, const uint8_t* nonces, uint32_t n,
                     uint8_t* sigs65_out);
 
+/* Batched signing with the nonce libsecp256k1 derives by default: the bytes go-ethereum's crypto.Sign returns for the same key
+ * and digest (secp256k1_ecdsa_sign_recoverable with nonce_function_rfc6979; without cgo, dcrd's RFC 6979 SignCompact, which
+ * agrees with it).  privkeys, digests: n x 32 bytes big-endian; sigs65_out: n x 65 bytes R||S||V.  Per row:
+ *   1. a key d = 0 or d >= n yields 65 zero bytes, as libsecp256k1 and go-ethereum refuse such a key.  This differs on purpose
+ *      from ibft_sign_batch, which signs with d mod n;
+ *   2. the HMAC-SHA256 DRBG of RFC 6979 §3.2 is seeded with the 64 bytes key || (z mod n): the raw key and the digest reduced
+ *      mod n, no extra data and no algorithm tag;
+ *   3. candidate c = 0, 1, 2, ... is the DRBG's (c+1)-th 32-byte output (from the second on, each output is preceded by
+ *      K = HMAC_K(V || 0x00), V = HMAC_K(V)).  A candidate outside [1, n), or one that gives s = 0, moves on to the next
+ *      (libsecp256k1's attempt counter); after 4 candidates the row is refused.  Real inputs reach neither case (< 2^-250);
+ *   4. r = (k G).x mod n, s = k^-1 (z + r d) mod n, s normalised to the low half; V = parity of R.y, flipped with s;
+ *   5. R.x >= n: libsecp256k1 would return recovery id 2 or 3, which no verify path of this engine accepts (v must be 0 or 1),
+ *      so the row is refused (65 zero bytes).  This is the one divergence from crypto.Sign; a random nonce reaches it with
+ *      probability about 2^-127 and an RFC 6979 nonce cannot be steered to it.
+ * Private keys are wiped from device memory before the call returns; the DRBG state never leaves the signing thread.  HOST
+ * buffers. */
+int ibft_sign_batch_rfc6979(ibft_engine* e, const uint8_t* privkeys, const uint8_t* digests, uint32_t n, uint8_t* sigs65_out);
+
 /* measurement / test hooks ------------------------------------------------------------------------- */
 /* Kernel selection of the recover step (the verdicts are identical on every path; only latency / throughput differ):
  *   AUTO    by batch size: up to SMs x 48 signatures (6,336 on an H100) QSPLIT, up to SMs x 192 (25,344) SPLIT, beyond
@@ -385,6 +403,8 @@ int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* wide_mac_per
 #define IBFT_DBG_SC_DIGITS 22      /* out(256): ecmult_split_into(a), a in [0, n), and the Booth digits of both halves: half h at
                                     * 128 h = magnitude (6 words, little-endian) || sign byte at 24 || 33 int8 4-bit digits at 32
                                     * || 17 int16 (little-endian) 8-bit digits at 72 */
+#define IBFT_DBG_RFC6979 23        /* out = raw nonce candidate c (before any range check) of ibft_sign_batch_rfc6979 for the key a
+                                    * and the digest b; c = the last byte of the 64-byte c operand */
 /* Generator comb tables (builds with IBFT_WC > 0): *wc = window (0 when absent), *entries = entries of one comb position;
  * copies `count` 64-byte entries (x, y as 8 little-endian words each) starting at `first`, positions laid out one after the
  * other: entry p * entries + d1 * (2^wc + 1) + d2 + 2^(wc-1) holds (d1 + d2*lambda) * 2^(wc*p) * G, p = 0..16 (position 0 is
