@@ -183,6 +183,32 @@ __device__ __forceinline__ void learn_key(const slot_dev* __restrict__ slots, ui
   if (atomicCAS(&s.key_state[r], IBFT_KEY_UNKNOWN, IBFT_KEY_LEARNED) == IBFT_KEY_UNKNOWN) atomicAdd(s.learn_count, 1u);
 }
 
+// stage the packed tuples [base, min(base + ROWS, hi)) into 33-word shared rows, THREADS threads with coalesced 16-byte loads
+template <int ROWS, int THREADS>
+__device__ __forceinline__ void stage_items(uint32_t* s_items, const ibft_sig_item* __restrict__ items, uint32_t base, uint32_t hi,
+                                            uint32_t tid) {
+  static_assert((ROWS * 8) % THREADS == 0, "every thread stages the same number of 16-byte pieces");
+  const uint4* src = reinterpret_cast<const uint4*>(items + base);
+  uint32_t avail = base < hi ? min((uint32_t)ROWS, hi - base) : 0u;
+#pragma unroll
+  for (int k = 0; k < (ROWS * 8) / THREADS; k++) {
+    uint32_t q = tid + k * THREADS;  // uint4 index within the staged block
+    uint32_t row = q >> 3, col = q & 7;
+    if (row < avail) {
+      uint4 v = __ldg(src + q);
+      uint32_t* d = s_items + row * IBFT_ITEM_ROW_WORDS + col * 4;
+      d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
+    }
+  }
+}
+// the tuple staged in shared row `row`
+__device__ __forceinline__ void load_item(ibft_sig_item& it, const uint32_t* s_items, uint32_t row) {
+  uint32_t* w = reinterpret_cast<uint32_t*>(&it);
+  const uint32_t* s = s_items + row * IBFT_ITEM_ROW_WORDS;
+#pragma unroll
+  for (int i = 0; i < 32; i++) w[i] = s[i];
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // K1 + K2: recover kernel.  One thread per signature; a warp's 32 verdicts become one bitmap word.
 // ------------------------------------------------------------------------------------------------------------
@@ -217,30 +243,14 @@ k_recover(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __
 #endif
   // stage this CTA's 128 packed tuples with coalesced 16-byte loads
   const uint32_t base = shard_lo + blockIdx.x * BLOCK;
-  if (list == nullptr) {
-    const uint4* src = reinterpret_cast<const uint4*>(items + base);
-    uint32_t avail = base < shard_hi ? min((uint32_t)BLOCK, shard_hi - base) : 0u;
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      uint32_t q = tid + k * BLOCK;  // uint4 index within the CTA's tuple block
-      uint32_t row = q >> 3, col = q & 7;
-      if (row < avail) {
-        uint4 v = __ldg(src + q);
-        uint32_t* d = s_items + row * IBFT_ITEM_ROW_WORDS + col * 4;
-        d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-      }
-    }
-  }
+  if (list == nullptr) stage_items<BLOCK, BLOCK>(s_items, items, base, shard_hi, tid);
   __syncthreads();
   uint32_t idx = base + tid;
   bool active = idx < shard_hi;
   bool ok = false;
   ibft_sig_item it;
   if (list == nullptr) {
-    uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-    const uint32_t* s = s_items + tid * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-    for (int i = 0; i < 32; i++) w[i] = s[i];
+    load_item(it, s_items, tid);
   } else {
     const uint32_t t = blockIdx.x * BLOCK + tid;
     active = t < list[0];
@@ -316,31 +326,13 @@ k_verify_known(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
   __shared__ uint32_t s_items[BLOCK * IBFT_ITEM_ROW_WORDS];
   const uint32_t tid = threadIdx.x;
   const uint32_t base = shard_lo + blockIdx.x * BLOCK;
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(items + base);
-    uint32_t avail = base < shard_hi ? min((uint32_t)BLOCK, shard_hi - base) : 0u;
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      uint32_t q = tid + k * BLOCK;
-      uint32_t row = q >> 3, col = q & 7;
-      if (row < avail) {
-        uint4 v = __ldg(src + q);
-        uint32_t* d = s_items + row * IBFT_ITEM_ROW_WORDS + col * 4;
-        d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-      }
-    }
-  }
+  stage_items<BLOCK, BLOCK>(s_items, items, base, shard_hi, tid);
   __syncthreads();
   const uint32_t idx = base + tid;
   bool ok = false;
   if (idx < shard_hi) {
     ibft_sig_item it;
-    {
-      uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-      const uint32_t* s = s_items + tid * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-      for (int i = 0; i < 32; i++) w[i] = s[i];
-    }
+    load_item(it, s_items, tid);
     resolved_item ri;
     bool have = false;
     int st = resolve_item(it, arena, arena_len, ri, &have);
@@ -389,32 +381,14 @@ k_recover_quad(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
   const uint32_t tid = threadIdx.x;
   const uint32_t q = tid >> 2;  // signature within the CTA
   const uint32_t base = shard_lo + blockIdx.x * IBFT_QUAD_SIGS;
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(items + base);
-    uint32_t avail = base < shard_hi ? min((uint32_t)IBFT_QUAD_SIGS, shard_hi - base) : 0u;
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-      uint32_t u = tid + k * 4 * IBFT_QUAD_SIGS;  // uint4 index within the CTA's tuple block (32 tuples x 8)
-      uint32_t row = u >> 3, col = u & 7;
-      if (row < avail) {
-        uint4 v = __ldg(src + u);
-        uint32_t* d = s_items + row * IBFT_ITEM_ROW_WORDS + col * 4;
-        d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-      }
-    }
-    if (tid == 0) s_word = 0;
-  }
+  stage_items<IBFT_QUAD_SIGS, 4 * IBFT_QUAD_SIGS>(s_items, items, base, shard_hi, tid);
+  if (tid == 0) s_word = 0;
   __syncthreads();
   const uint32_t idx = base + q;
   bool ok = false;
   if (idx < shard_hi) {  // uniform over the quad
     ibft_sig_item it;
-    {
-      uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-      const uint32_t* s = s_items + q * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-      for (int i = 0; i < 32; i++) w[i] = s[i];
-    }
+    load_item(it, s_items, q);
     exec_quad ex;
     ex.role = (int)(tid & 3u);
     ex.mask = 0xFu << (tid & 28u);
@@ -466,17 +440,77 @@ k_recover_quad(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
 // ------------------------------------------------------------------------------------------------------------
 #define IBFT_SPLIT_CHAINS 3
 #define IBFT_SPLIT_SIGS (32 * IBFT_SPLIT_CHAINS)
-#define IBFT_SLOT_WORDS 28  // [0..4] |k1|, [5..9] |k2| of u2, [10] phase-1 flags, [11..18] y then gx, [19..26] gy, [27] phase-2 flags
-                            // (the two phases have their own flag words: the helper may post phase 2 before a chain warp has
-                            // read phase 1 -- same bits either way, but two words keep the hand-off free of unordered accesses)
+// Hand-off slot of the split kernels (k_recover_split, k_verify_split, k_recover_qsplit): word w of signature i at
+// s_slot[w * S + i], S = signatures per CTA.  The two phases have their own flag words: the helper may post phase 2 before a
+// chain warp has read phase 1 -- same bits either way, but two words keep the hand-off free of unordered accesses.
+#define IBFT_SLOT_K1 0     // [0..4] |k1| of u2
+#define IBFT_SLOT_K2 5     // [5..9] |k2| of u2
+#define IBFT_SLOT_F1 10    // phase-1 flags
+#define IBFT_SLOT_A 11     // [11..18] the helper's parked operand (r or s, then its inverse), then u1*G's x
+#define IBFT_SLOT_B 19     // [19..26] the other parked operand (s or r), then u1*G's y
+#define IBFT_SLOT_F2 27    // phase-2 flags of the recovering kernels
+#define IBFT_SLOT_WORDS (IBFT_SLOT_F2 + 1)
+#define IBFT_VSLOT_SIGNER 27  // k_verify_split, in place of IBFT_SLOT_F2: validator index | table slot << 16 of the signer
+#define IBFT_VSLOT_F2 28      // k_verify_split: phase-2 flags
+#define IBFT_VSLOT_TAB 29     // k_verify_split: table slot of the signer's key
+#define IBFT_VSLOT_WORDS (IBFT_VSLOT_TAB + 1)
 #define IBFT_SPLIT_SMEM ((IBFT_SPLIT_SIGS * (IBFT_ITEM_ROW_WORDS + IBFT_RTAB_WORDS + IBFT_SLOT_WORDS + 8)) * 4)
-#define IBFT_SF_VALID 1u   // phase 1: (r, s, v) in range, digits posted
+#define IBFT_VSPLIT_SMEM ((IBFT_SPLIT_SIGS * (IBFT_ITEM_ROW_WORDS + IBFT_VSLOT_WORDS)) * 4)
+#define IBFT_SF_VALID 1u   // phase 1: digits of u2 posted, the chain runs
 #define IBFT_SF_NEG0 2u
 #define IBFT_SF_NEG1 4u
-#define IBFT_SF_ROOT 8u    // phase 2: r is an abscissa, y posted
+#define IBFT_SF_ROOT 8u    // recover phase 2: r is an abscissa, y posted
 #define IBFT_SF_GINF 16u   // phase 2: u1*G is the point at infinity
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+
+// the 8-word operands at IBFT_SLOT_A and (b != nullptr) IBFT_SLOT_B of signature i's slot
+__device__ __forceinline__ void slot_get8(const uint32_t* s_slot, uint32_t S, uint32_t i, uint32_t* a, uint32_t* b = nullptr) {
+#pragma unroll
+  for (int k = 0; k < 8; k++) {
+    a[k] = s_slot[(IBFT_SLOT_A + k) * S + i];
+    if (b != nullptr) b[k] = s_slot[(IBFT_SLOT_B + k) * S + i];
+  }
+}
+__device__ __forceinline__ void slot_put8(uint32_t* s_slot, uint32_t S, uint32_t i, const uint32_t* a, const uint32_t* b = nullptr) {
+#pragma unroll
+  for (int k = 0; k < 8; k++) {
+    s_slot[(IBFT_SLOT_A + k) * S + i] = a[k];
+    if (b != nullptr) s_slot[(IBFT_SLOT_B + k) * S + i] = b[k];
+  }
+}
+// helper: the phase-1 flags of the digits of u2, and their posting (two calls: each kernel keeps its own order of the two)
+__device__ __forceinline__ uint32_t u2_flags(const ecmult_digits& dg) {
+  return IBFT_SF_VALID | (dg.kneg[0] ? IBFT_SF_NEG0 : 0u) | (dg.kneg[1] ? IBFT_SF_NEG1 : 0u);
+}
+__device__ __forceinline__ void post_u2_digits(uint32_t* s_slot, uint32_t S, uint32_t i, const ecmult_digits& dg) {
+#pragma unroll
+  for (int k = 0; k < 5; k++) {
+    s_slot[(IBFT_SLOT_K1 + k) * S + i] = dg.ks[0][k];
+    s_slot[(IBFT_SLOT_K2 + k) * S + i] = dg.ks[1][k];
+  }
+}
+// chain: the posted digits of u2 (flags: phase-1 flags), the other two streams zero
+__device__ __forceinline__ void take_u2_digits(const uint32_t* s_slot, uint32_t S, uint32_t i, uint32_t flags, ecmult_digits& dg) {
+#pragma unroll
+  for (int k = 0; k < 5; k++) {
+    dg.ks[0][k] = s_slot[(IBFT_SLOT_K1 + k) * S + i];
+    dg.ks[1][k] = s_slot[(IBFT_SLOT_K2 + k) * S + i];
+    dg.ks[2][k] = dg.ks[3][k] = 0;
+  }
+  dg.ks[0][5] = dg.ks[1][5] = dg.ks[2][5] = dg.ks[3][5] = 0;
+  dg.kneg[0] = flags & IBFT_SF_NEG0; dg.kneg[1] = flags & IBFT_SF_NEG1;
+  dg.kneg[2] = dg.kneg[3] = false;
+}
+// chain: the root y and the affine u1*G the helper posted in phase 2 for signature i
+__device__ __forceinline__ void take_root_u1g(const uint32_t* s_slot, const uint32_t* s_y, uint32_t S, uint32_t i, fe& y, fe& gx, fe& gy) {
+#pragma unroll
+  for (int k = 0; k < 8; k++) {
+    y.v[k] = s_y[k * S + i];
+    gx.v[k] = s_slot[(IBFT_SLOT_A + k) * S + i];
+    gy.v[k] = s_slot[(IBFT_SLOT_B + k) * S + i];
+  }
+}
 
 __global__ void __launch_bounds__(32 * (IBFT_SPLIT_CHAINS + 1), 1)
 k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __restrict__ arena, size_t arena_len,
@@ -490,20 +524,7 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
   uint32_t* s_y = s_slot + IBFT_SPLIT_SIGS * IBFT_SLOT_WORDS;             // the root y, 8 words per signature, same interleave
   const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
   const uint32_t base = shard_lo + blockIdx.x * IBFT_SPLIT_SIGS;
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(items + base);
-    uint32_t avail = base < shard_hi ? min((uint32_t)IBFT_SPLIT_SIGS, shard_hi - base) : 0u;
-#pragma unroll
-    for (int k = 0; k < (IBFT_SPLIT_SIGS * 8) / (32 * (IBFT_SPLIT_CHAINS + 1)); k++) {
-      uint32_t u = tid + k * 32 * (IBFT_SPLIT_CHAINS + 1);
-      uint32_t row = u >> 3, col = u & 7;
-      if (row < avail) {
-        uint4 v = __ldg(src + u);
-        uint32_t* d = s_items + row * IBFT_ITEM_ROW_WORDS + col * 4;
-        d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-      }
-    }
-  }
+  stage_items<IBFT_SPLIT_SIGS, 32 * (IBFT_SPLIT_CHAINS + 1)>(s_items, items, base, shard_hi, tid);
   __syncthreads();
   gtab_view G{g_gtable};
   G.comb = ctable;
@@ -522,20 +543,13 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
       bool have = false;
       if (idx < shard_hi) {
         ibft_sig_item it;
-        uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-        const uint32_t* src = s_items + i * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-        for (int k = 0; k < 32; k++) w[k] = src[k];
+        load_item(it, s_items, i);
         resolved_item ri;
         resolve_item(it, arena, arena_len, ri, &have, false);
         have = have && split_sig_in_range(ri);
         if (have) {
           sc r = sc_from_be(ri.r), sv = sc_from_be(ri.s);
-#pragma unroll
-          for (int k = 0; k < 8; k++) {
-            s_slot[(11 + k) * IBFT_SPLIT_SIGS + i] = r.v[k];
-            s_slot[(19 + k) * IBFT_SPLIT_SIGS + i] = sv.v[k];
-          }
+          slot_put8(s_slot, IBFT_SPLIT_SIGS, i, r.v, sv.v);
         }
       }
       if (have) okmask |= 1u << p;
@@ -551,7 +565,7 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
         rr[p] = one;
         if ((okmask >> p) & 1u) {
 #pragma unroll
-          for (int k = 0; k < 8; k++) rr[p].v[k] = s_slot[(11 + k) * IBFT_SPLIT_SIGS + 32 * p + lane];
+          for (int k = 0; k < 8; k++) rr[p].v[k] = s_slot[(IBFT_SLOT_A + k) * IBFT_SPLIT_SIGS + 32 * p + lane];
         }
         pre[p] = p ? sc_mul(pre[p - 1], rr[p]) : rr[p];
       }
@@ -561,7 +575,7 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
         sc ri = p ? sc_mul(inv, pre[p - 1]) : inv;
         if (p) inv = sc_mul(inv, rr[p]);
 #pragma unroll
-        for (int k = 0; k < 8; k++) s_slot[(11 + k) * IBFT_SPLIT_SIGS + 32 * p + lane] = ri.v[k];  // r^-1 replaces r
+        for (int k = 0; k < 8; k++) s_slot[(IBFT_SLOT_A + k) * IBFT_SPLIT_SIGS + 32 * p + lane] = ri.v[k];  // r^-1 replaces r
       }
     }
     IBFT_ROLLED
@@ -570,21 +584,13 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
       uint32_t flags = 0;
       if ((okmask >> p) & 1u) {
         sc sv, rinv;
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-          rinv.v[k] = s_slot[(11 + k) * IBFT_SPLIT_SIGS + i];
-          sv.v[k] = s_slot[(19 + k) * IBFT_SPLIT_SIGS + i];
-        }
+        slot_get8(s_slot, IBFT_SPLIT_SIGS, i, rinv.v, sv.v);
         ecmult_digits dg;
         ecmult_split_into(sc_mul(sv, rinv), dg, 0);
-        flags = IBFT_SF_VALID | (dg.kneg[0] ? IBFT_SF_NEG0 : 0u) | (dg.kneg[1] ? IBFT_SF_NEG1 : 0u);
-#pragma unroll
-        for (int k = 0; k < 5; k++) {
-          s_slot[k * IBFT_SPLIT_SIGS + i] = dg.ks[0][k];
-          s_slot[(5 + k) * IBFT_SPLIT_SIGS + i] = dg.ks[1][k];
-        }
+        flags = u2_flags(dg);
+        post_u2_digits(s_slot, IBFT_SPLIT_SIGS, i, dg);
       }
-      s_slot[10 * IBFT_SPLIT_SIGS + i] = flags;
+      s_slot[IBFT_SLOT_F1 * IBFT_SPLIT_SIGS + i] = flags;
       __threadfence_block();
       named_bar_arrive(1 + p, 64);
     }
@@ -592,18 +598,15 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
     for (uint32_t p = 0; p < IBFT_SPLIT_CHAINS; p++) {
       const uint32_t i = 32 * p + lane;
       if ((okmask >> p) & 1u) {
-        uint32_t flags = s_slot[10 * IBFT_SPLIT_SIGS + i];
+        uint32_t flags = s_slot[IBFT_SLOT_F1 * IBFT_SPLIT_SIGS + i];
         ibft_sig_item it;
-        uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-        const uint32_t* src = s_items + i * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-        for (int k = 0; k < 32; k++) w[k] = src[k];
+        load_item(it, s_items, i);
         resolved_item ri;
         bool have = false;
         resolve_item(it, arena, arena_len, ri, &have, true);  // this time with the digest
         sc rinv;
 #pragma unroll
-        for (int k = 0; k < 8; k++) rinv.v[k] = s_slot[(11 + k) * IBFT_SPLIT_SIGS + i];
+        for (int k = 0; k < 8; k++) rinv.v[k] = s_slot[(IBFT_SLOT_A + k) * IBFT_SPLIT_SIGS + i];
         ecmult_digits dg;
 #pragma unroll
         for (int k = 0; k < 6; k++) dg.ks[0][k] = dg.ks[1][k] = 0;
@@ -617,12 +620,12 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
           for (int k = 0; k < 8; k++) {
             s_y[k * IBFT_SPLIT_SIGS + i] = y.v[k];
             if (!g_inf) {
-              s_slot[(11 + k) * IBFT_SPLIT_SIGS + i] = gx.v[k];
-              s_slot[(19 + k) * IBFT_SPLIT_SIGS + i] = gy.v[k];
+              s_slot[(IBFT_SLOT_A + k) * IBFT_SPLIT_SIGS + i] = gx.v[k];
+              s_slot[(IBFT_SLOT_B + k) * IBFT_SPLIT_SIGS + i] = gy.v[k];
             }
           }
         }
-        s_slot[27 * IBFT_SPLIT_SIGS + i] = flags;
+        s_slot[IBFT_SLOT_F2 * IBFT_SPLIT_SIGS + i] = flags;
       }
       __threadfence_block();
       named_bar_arrive(1 + IBFT_SPLIT_CHAINS + p, 64);
@@ -639,10 +642,7 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
   rtab_view T{s_rtab + i, (uint32_t)IBFT_SPLIT_SIGS};
   fe gz = fe_from_u32(1);  // global Z of the table (ecmult_build_rtable_globalz)
   if (active) {
-    uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-    const uint32_t* src = s_items + i * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-    for (int k = 0; k < 32; k++) w[k] = src[k];
+    load_item(it, s_items, i);
     st = resolve_item(it, arena, arena_len, ri, &have, false);  // fields only: the chain never needs the digest
     if (have) gz = ecmult_build_rtable_globalz(split_chain_point(ri.r), T);  // table on a second isomorphic curve: no inversion
   }
@@ -652,18 +652,10 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
   acc.inf = true;
   bool go = false;
   if (active && have) {
-    uint32_t flags = s_slot[10 * IBFT_SPLIT_SIGS + i];
+    uint32_t flags = s_slot[IBFT_SLOT_F1 * IBFT_SPLIT_SIGS + i];
     if (flags & IBFT_SF_VALID) {
       ecmult_digits dg;
-#pragma unroll
-      for (int k = 0; k < 5; k++) {
-        dg.ks[0][k] = s_slot[k * IBFT_SPLIT_SIGS + i];
-        dg.ks[1][k] = s_slot[(5 + k) * IBFT_SPLIT_SIGS + i];
-        dg.ks[2][k] = dg.ks[3][k] = 0;
-      }
-      dg.ks[0][5] = dg.ks[1][5] = dg.ks[2][5] = dg.ks[3][5] = 0;
-      dg.kneg[0] = flags & IBFT_SF_NEG0; dg.kneg[1] = flags & IBFT_SF_NEG1;
-      dg.kneg[2] = dg.kneg[3] = false;
+      take_u2_digits(s_slot, IBFT_SPLIT_SIGS, i, flags, dg);
       acc = ecmult_streams(dg, G, T, false);
       go = true;
     }
@@ -676,15 +668,10 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
   for (int k = 0; k < 20; k++) addr[k] = 0;
   bool ok = false;
   if (go) {
-    uint32_t flags = s_slot[27 * IBFT_SPLIT_SIGS + i];
+    uint32_t flags = s_slot[IBFT_SLOT_F2 * IBFT_SPLIT_SIGS + i];
     if (flags & IBFT_SF_ROOT) {
       fe y, gx, gy;
-#pragma unroll
-      for (int k = 0; k < 8; k++) {
-        y.v[k] = s_y[k * IBFT_SPLIT_SIGS + i];
-        gx.v[k] = s_slot[(11 + k) * IBFT_SPLIT_SIGS + i];
-        gy.v[k] = s_slot[(19 + k) * IBFT_SPLIT_SIGS + i];
-      }
+      take_root_u1g(s_slot, s_y, IBFT_SPLIT_SIGS, i, y, gx, gy);
       ok = split_chain_finish(acc, fe_mul(y, gz), (flags & IBFT_SF_GINF) != 0, gx, gy, addr, &K);  // Z' -> Z' * Z_8 * y
     }
   }
@@ -721,15 +708,8 @@ k_recover_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8
 // valid (malformed, out of range, unknown group, signer not in the set) are settled here.  A round in which every signature
 // verifies (the normal case of consensus) never runs a second chain.
 // ------------------------------------------------------------------------------------------------------------
-#define IBFT_VSLOT_WORDS 30   // [0..26] as IBFT_SLOT_WORDS, [27] validator index | slot << 16 of the signer, [28] phase-2 flags,
-                              // [29] table slot of the signer's key
-#define IBFT_VSPLIT_SMEM ((IBFT_SPLIT_SIGS * (IBFT_ITEM_ROW_WORDS + IBFT_VSLOT_WORDS)) * 4)
-#define IBFT_VF_VALID 1u      // digits of u2 posted: the chain runs
-#define IBFT_VF_NEG0 2u
-#define IBFT_VF_NEG1 4u
-#define IBFT_VF_GREADY 8u     // u1*G posted
-#define IBFT_VF_GINF 16u
-#define IBFT_VF_RECOVER 32u   // member, but the key is not known yet: worklist
+#define IBFT_VF_GREADY 8u     // phase 2: u1*G posted
+#define IBFT_VF_RECOVER 32u   // phase 1: member, but the key is not known yet: worklist
 __global__ void __launch_bounds__(32 * (IBFT_SPLIT_CHAINS + 1), 1)
 k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __restrict__ arena, size_t arena_len,
                uint32_t shard_lo, uint32_t shard_hi, const ibft_group_desc* __restrict__ groups, uint32_t n_groups,
@@ -741,20 +721,7 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
   const uint32_t S = IBFT_SPLIT_SIGS;
   const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
   const uint32_t base = shard_lo + blockIdx.x * IBFT_SPLIT_SIGS;
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(items + base);
-    uint32_t avail = base < shard_hi ? min((uint32_t)IBFT_SPLIT_SIGS, shard_hi - base) : 0u;
-#pragma unroll
-    for (int k = 0; k < (IBFT_SPLIT_SIGS * 8) / (32 * (IBFT_SPLIT_CHAINS + 1)); k++) {
-      uint32_t u = tid + k * 32 * (IBFT_SPLIT_CHAINS + 1);
-      uint32_t row = u >> 3, col = u & 7;
-      if (row < avail) {
-        uint4 v = __ldg(src + u);
-        uint32_t* d = s_items + row * IBFT_ITEM_ROW_WORDS + col * 4;
-        d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-      }
-    }
-  }
+  stage_items<IBFT_SPLIT_SIGS, 32 * (IBFT_SPLIT_CHAINS + 1)>(s_items, items, base, shard_hi, tid);
   __syncthreads();
   gtab_view G{g_gtable};
   G.comb = ctable;
@@ -767,10 +734,7 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
       uint32_t flags = 0;
       if (idx < shard_hi) {
         ibft_sig_item it;
-        uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-        const uint32_t* src = s_items + i * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-        for (int k = 0; k < 32; k++) w[k] = src[k];
+        load_item(it, s_items, i);
         resolved_item ri;
         bool have = false;
         int st = resolve_item(it, arena, arena_len, ri, &have, false);
@@ -784,20 +748,16 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
           if (v >= 0 && slots[slot].key_ref != nullptr) t = key_lookup(slots[slot], slots[slot].key_ref[v], &ready);
           if (ready) {
             sc r = sc_from_be(ri.r), sv = sc_from_be(ri.s);
-#pragma unroll
-            for (int k = 0; k < 8; k++) {
-              s_slot[(11 + k) * S + i] = sv.v[k];   // s (inverted below), then r
-              s_slot[(19 + k) * S + i] = r.v[k];
-            }
-            s_slot[27 * S + i] = (uint32_t)v | (slot << 16);
-            s_slot[29 * S + i] = t;
+            slot_put8(s_slot, S, i, sv.v, r.v);  // s (inverted below), then r
+            s_slot[IBFT_VSLOT_SIGNER * S + i] = (uint32_t)v | (slot << 16);
+            s_slot[IBFT_VSLOT_TAB * S + i] = t;
             okmask |= 1u << p;
           } else {
             flags = IBFT_VF_RECOVER;               // member whose key is not known (or no table: v < 0): the recover path decides
           }
         }
       }
-      s_slot[10 * S + i] = flags;
+      s_slot[IBFT_SLOT_F1 * S + i] = flags;
     }
     {
       // w = s^-1 for the lane's signatures with ONE inversion (Montgomery's trick; an absent one contributes 1)
@@ -810,7 +770,7 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
         ss[p] = one;
         if ((okmask >> p) & 1u) {
 #pragma unroll
-          for (int k = 0; k < 8; k++) ss[p].v[k] = s_slot[(11 + k) * S + 32 * p + lane];
+          for (int k = 0; k < 8; k++) ss[p].v[k] = s_slot[(IBFT_SLOT_A + k) * S + 32 * p + lane];
         }
         pre[p] = p ? sc_mul(pre[p - 1], ss[p]) : ss[p];
       }
@@ -820,7 +780,7 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
         sc wi = p ? sc_mul(inv, pre[p - 1]) : inv;
         if (p) inv = sc_mul(inv, ss[p]);
 #pragma unroll
-        for (int k = 0; k < 8; k++) s_slot[(11 + k) * S + 32 * p + lane] = wi.v[k];  // w replaces s
+        for (int k = 0; k < 8; k++) s_slot[(IBFT_SLOT_A + k) * S + 32 * p + lane] = wi.v[k];  // w replaces s
       }
     }
     IBFT_ROLLED
@@ -828,19 +788,11 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
       const uint32_t i = 32 * p + lane;
       if ((okmask >> p) & 1u) {
         sc w, r;
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-          w.v[k] = s_slot[(11 + k) * S + i];
-          r.v[k] = s_slot[(19 + k) * S + i];
-        }
+        slot_get8(s_slot, S, i, w.v, r.v);
         ecmult_digits dg;
         ecmult_split_into(sc_mul(r, w), dg, 0);
-#pragma unroll
-        for (int k = 0; k < 5; k++) {
-          s_slot[k * S + i] = dg.ks[0][k];
-          s_slot[(5 + k) * S + i] = dg.ks[1][k];
-        }
-        s_slot[10 * S + i] = IBFT_VF_VALID | (dg.kneg[0] ? IBFT_VF_NEG0 : 0u) | (dg.kneg[1] ? IBFT_VF_NEG1 : 0u);
+        post_u2_digits(s_slot, S, i, dg);
+        s_slot[IBFT_SLOT_F1 * S + i] = u2_flags(dg);
       }
       __threadfence_block();
       named_bar_arrive(1 + p, 64);
@@ -850,26 +802,17 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
       const uint32_t i = 32 * p + lane;
       if ((okmask >> p) & 1u) {
         ibft_sig_item it;
-        uint32_t* wd = reinterpret_cast<uint32_t*>(&it);
-        const uint32_t* src = s_items + i * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-        for (int k = 0; k < 32; k++) wd[k] = src[k];
+        load_item(it, s_items, i);
         resolved_item ri;
         bool have = false;
         resolve_item(it, arena, arena_len, ri, &have, true);  // this time with the digest
         sc w;
-#pragma unroll
-        for (int k = 0; k < 8; k++) w.v[k] = s_slot[(11 + k) * S + i];
+        slot_get8(s_slot, S, i, w.v);
         fe gx = fe_zero(), gy = fe_zero();
         bool g_inf = false;
         known_helper_u1g(ri, w, G, g_inf, gx, gy);
-        uint32_t flags = IBFT_VF_GREADY | (g_inf ? IBFT_VF_GINF : 0u);
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-          s_slot[(11 + k) * S + i] = gx.v[k];
-          s_slot[(19 + k) * S + i] = gy.v[k];
-        }
-        s_slot[28 * S + i] = flags;
+        slot_put8(s_slot, S, i, gx.v, gy.v);
+        s_slot[IBFT_VSLOT_F2 * S + i] = IBFT_VF_GREADY | (g_inf ? IBFT_SF_GINF : 0u);
       }
       __threadfence_block();
       named_bar_arrive(1 + IBFT_SPLIT_CHAINS + p, 64);
@@ -883,46 +826,31 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
   jac acc;
   acc.x = fe_zero(); acc.y = fe_zero(); acc.z = fe_zero();
   acc.inf = true;
-  uint32_t flags = active ? s_slot[10 * S + i] : 0u;
+  uint32_t flags = active ? s_slot[IBFT_SLOT_F1 * S + i] : 0u;
   uint32_t vslot = 0;
-  if (flags & IBFT_VF_VALID) {
+  if (flags & IBFT_SF_VALID) {
     ecmult_digits dg;
-#pragma unroll
-    for (int k = 0; k < 5; k++) {
-      dg.ks[0][k] = s_slot[k * S + i];
-      dg.ks[1][k] = s_slot[(5 + k) * S + i];
-      dg.ks[2][k] = dg.ks[3][k] = 0;
-    }
-    dg.ks[0][5] = dg.ks[1][5] = dg.ks[2][5] = dg.ks[3][5] = 0;
-    dg.kneg[0] = flags & IBFT_VF_NEG0; dg.kneg[1] = flags & IBFT_VF_NEG1;
-    dg.kneg[2] = dg.kneg[3] = false;
-    vslot = s_slot[27 * S + i];
-    gtab_view Qt{key_table_of(slots[vslot >> 16].key_chunks, s_slot[29 * S + i])};
+    take_u2_digits(s_slot, S, i, flags, dg);
+    vslot = s_slot[IBFT_VSLOT_SIGNER * S + i];
+    gtab_view Qt{key_table_of(slots[vslot >> 16].key_chunks, s_slot[IBFT_VSLOT_TAB * S + i])};
     acc = ecmult_streams_known(dg, G, Qt, false);
   }
   named_bar_sync(1 + IBFT_SPLIT_CHAINS + warp, 64);  // u1*G is posted
   bool ok = false;
-  if (flags & IBFT_VF_VALID) {
-    const uint32_t f2 = s_slot[28 * S + i];
+  if (flags & IBFT_SF_VALID) {
+    const uint32_t f2 = s_slot[IBFT_VSLOT_F2 * S + i];
     fe gx, gy;
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      gx.v[k] = s_slot[(11 + k) * S + i];
-      gy.v[k] = s_slot[(19 + k) * S + i];
-    }
+    slot_get8(s_slot, S, i, gx.v, gy.v);
     ibft_sig_item it;
-    uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-    const uint32_t* src = s_items + i * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-    for (int k = 0; k < 32; k++) w[k] = src[k];
+    load_item(it, s_items, i);
     resolved_item ri;
     bool have = false;
     resolve_item(it, arena, arena_len, ri, &have, false);
-    ok = known_chain_finish(acc, (f2 & IBFT_VF_GINF) != 0, gx, gy, ri);
+    ok = known_chain_finish(acc, (f2 & IBFT_SF_GINF) != 0, gx, gy, ri);
     if (ok) record_vote(sink, groups, it.group, (int)(vslot & 0xFFFFu));
   }
   // whatever was not accepted but could still be valid goes to the recover pass
-  if (active && !ok && (flags & (IBFT_VF_VALID | IBFT_VF_RECOVER))) worklist[1 + atomicAdd(&worklist[0], 1u)] = idx;
+  if (active && !ok && (flags & (IBFT_SF_VALID | IBFT_VF_RECOVER))) worklist[1 + atomicAdd(&worklist[0], 1u)] = idx;
   uint32_t word = __ballot_sync(0xFFFFFFFFu, ok);
   if (lane == 0 && active) bitmap[idx >> 5] = word;
 }
@@ -986,25 +914,18 @@ k_recover_qsplit(const ibft_sig_item* __restrict__ items, uint32_t n, const uint
     sc rinv;
     uint32_t flags = 0;
     if (mine) {
-      uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-      const uint32_t* src = s_items + i * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-      for (int k = 0; k < 32; k++) w[k] = src[k];
+      load_item(it, s_items, i);
       bool have = false;
       resolve_item(it, arena, arena_len, ri, &have, false);
       if (have && split_sig_in_range(ri)) {
         rinv = IBFT_SC_INV(sc_from_be(ri.r));
         ecmult_digits dg;
         split_helper_u2(ri, rinv, dg);
-        flags = IBFT_SF_VALID | (dg.kneg[0] ? IBFT_SF_NEG0 : 0u) | (dg.kneg[1] ? IBFT_SF_NEG1 : 0u);
-#pragma unroll
-        for (int k = 0; k < 5; k++) {
-          s_slot[k * S + i] = dg.ks[0][k];
-          s_slot[(5 + k) * S + i] = dg.ks[1][k];
-        }
+        flags = u2_flags(dg);
+        post_u2_digits(s_slot, S, i, dg);
       }
     }
-    if (lane < S) s_slot[10 * S + i] = flags;
+    if (lane < S) s_slot[IBFT_SLOT_F1 * S + i] = flags;
     __threadfence_block();
     named_bar_arrive(1, 64); named_bar_arrive(2, 64); named_bar_arrive(3, 64);
     if (flags & IBFT_SF_VALID) {
@@ -1023,12 +944,12 @@ k_recover_qsplit(const ibft_sig_item* __restrict__ items, uint32_t n, const uint
         for (int k = 0; k < 8; k++) {
           s_y[k * S + i] = y.v[k];
           if (!g_inf) {
-            s_slot[(11 + k) * S + i] = gx.v[k];
-            s_slot[(19 + k) * S + i] = gy.v[k];
+            s_slot[(IBFT_SLOT_A + k) * S + i] = gx.v[k];
+            s_slot[(IBFT_SLOT_B + k) * S + i] = gy.v[k];
           }
         }
       }
-      s_slot[27 * S + i] = flags;
+      s_slot[IBFT_SLOT_F2 * S + i] = flags;
     }
     __threadfence_block();
     named_bar_arrive(4, 64); named_bar_arrive(5, 64); named_bar_arrive(6, 64);
@@ -1049,10 +970,7 @@ k_recover_qsplit(const ibft_sig_item* __restrict__ items, uint32_t n, const uint
   fe c = fe_zero();
   qtab_view T{s_qtab + q, S};
   if (active) {
-    uint32_t* w = reinterpret_cast<uint32_t*>(&it);
-    const uint32_t* src = s_items + q * IBFT_ITEM_ROW_WORDS;
-#pragma unroll
-    for (int k = 0; k < 32; k++) w[k] = src[k];
+    load_item(it, s_items, q);
     st = resolve_item(it, arena, arena_len, ri, &have, false);
     if (have) ecmult_build_qtable(ex, split_chain_point(ri.r, &c), T);
   }
@@ -1062,18 +980,10 @@ k_recover_qsplit(const ibft_sig_item* __restrict__ items, uint32_t n, const uint
   acc.inf = true;
   bool go = false;
   if (active && have) {
-    uint32_t flags = s_slot[10 * S + q];
+    uint32_t flags = s_slot[IBFT_SLOT_F1 * S + q];
     if (flags & IBFT_SF_VALID) {
       ecmult_digits dg;
-#pragma unroll
-      for (int k = 0; k < 5; k++) {
-        dg.ks[0][k] = s_slot[k * S + q];
-        dg.ks[1][k] = s_slot[(5 + k) * S + q];
-        dg.ks[2][k] = dg.ks[3][k] = 0;
-      }
-      dg.ks[0][5] = dg.ks[1][5] = dg.ks[2][5] = dg.ks[3][5] = 0;
-      dg.kneg[0] = flags & IBFT_SF_NEG0; dg.kneg[1] = flags & IBFT_SF_NEG1;
-      dg.kneg[2] = dg.kneg[3] = false;
+      take_u2_digits(s_slot, S, q, flags, dg);
       acc = ecmult_streams_x(ex, dg, G, T, false);
       go = true;
     }
@@ -1086,15 +996,10 @@ k_recover_qsplit(const ibft_sig_item* __restrict__ items, uint32_t n, const uint
   for (int k = 0; k < 20; k++) addr[k] = 0;
   bool ok = false;
   if (go) {
-    uint32_t flags = s_slot[27 * S + q];
+    uint32_t flags = s_slot[IBFT_SLOT_F2 * S + q];
     if (flags & IBFT_SF_ROOT) {
       fe y, gx, gy;
-#pragma unroll
-      for (int k = 0; k < 8; k++) {
-        y.v[k] = s_y[k * S + q];
-        gx.v[k] = s_slot[(11 + k) * S + q];
-        gy.v[k] = s_slot[(19 + k) * S + q];
-      }
+      take_root_u1g(s_slot, s_y, S, q, y, gx, gy);
       ok = split_chain_finish_x(ex, acc, c, y, (flags & IBFT_SF_GINF) != 0, gx, gy, addr, &K);
     }
   }
