@@ -15,7 +15,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
 
 
 def sources():
-    out = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith((".cu", ".cuh", ".inc"))]
+    out = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith((".cu", ".cuh", ".inc", ".hpp"))]
     out.append(os.path.join(HERE, "..", "include", "ibft_verify.h"))
     return out
 

@@ -17,7 +17,10 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <mutex>
+#include <shared_mutex>
+#include <string>
 #include <thread>
 #include <unordered_map>
 #include <vector>
@@ -26,6 +29,7 @@
 #include "verify_core.cuh"
 #include "debug_arith.cuh"
 #include "key_budget.hpp"
+#include "shard_plan.hpp"
 
 #include "secp_gtable.inc"
 
@@ -1766,7 +1770,40 @@ struct ibft_engine {
   uint8_t *hs_arena = nullptr, *hs_h_arena = nullptr, *hs_meta = nullptr, *hs_h_meta = nullptr;
   size_t hs_arena_cap = 0;
   uint32_t hs_n_cap = 0;
+  // multi-device engines (ibft_engine_create_multi): a coordinator holds one ordinary engine per device and allocates nothing
+  // above; a view is the borrowed diagnostics handle of one of them (ibft_engine_sub)
+  struct multi_engine* multi = nullptr;
+  ibft_engine* view_of = nullptr;
 };
+// Entry points of a coordinator or a view (defined with ibft_engine_create_multi at the end of this file)
+static int multi_refused(ibft_engine* e, const char* fn);
+static ibft_engine* diag_engine(ibft_engine* e);
+static void multi_destroy(ibft_engine* e);
+static int multi_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t height, const uint8_t* addrs, const uint8_t* powers_be,
+                                uint32_t n);
+static int multi_verify(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                        const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
+                        uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words);
+static int multi_submit(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                        const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
+                        uint8_t* recovered_out);
+static int multi_poll(ibft_engine* e, int* done);
+static int multi_wait(ibft_engine* e);
+static int multi_last_item_status(ibft_engine* e, uint8_t* status_out, uint32_t n);
+static int multi_known_handed_back(ibft_engine* e, uint32_t* n_out);
+static int multi_hash(ibft_engine* e, const uint8_t* arena, size_t arena_len, const uint32_t* offsets, const uint32_t* lens,
+                      const uint64_t* rounds, uint32_t n, uint8_t* out32);
+static int multi_sign(ibft_engine* e, const uint8_t* privkeys, const uint8_t* digests, const uint8_t* nonces, bool rfc6979, uint32_t n,
+                      uint8_t* sigs65_out);
+static int multi_refresh_key_tables(ibft_engine* e, uint32_t* n_keys_out);
+static int multi_set_key_table_budget(ibft_engine* e, uint32_t max_tables);
+static int multi_set_recover_path(ibft_engine* e, int path);
+static uint64_t multi_launch_count(ibft_engine* e);
+// a coordinator or a view: device-pointer calls name memory of one device, and a view only answers diagnostics
+#define IBFT_REFUSE_MULTI(e) \
+  if ((e) && ((e)->multi || (e)->view_of)) return multi_refused((e), __func__)
+#define IBFT_REFUSE_VIEW(e) \
+  if ((e) && (e)->view_of) return multi_refused((e), __func__)
 // the one-thread recover kernel of an engine: u1*G from the wide comb when the engine holds it
 template <int BLOCK>
 static decltype(&k_recover<BLOCK, false>) recover_kernel(const ibft_engine* e) {
@@ -1986,6 +2023,7 @@ static int engine_alloc(ibft_engine* e) {
 // little-endian words); entry p * entries + i is entry i of comb position p (position 0 = the combined table).  Returns
 // IBFT_ERR_INVALID_ARG when the library was built without a combined table
 extern "C" int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count, uint8_t* out, int* wc, uint32_t* entries) {
+  e = diag_engine(e);
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
   if (wc) *wc = IBFT_WC;
 #if IBFT_WC > 0
@@ -2004,6 +2042,7 @@ extern "C" int ibft_debug_ctable(ibft_engine* e, uint32_t first, uint32_t count,
 
 // test hook: copy `count` entries of the wide generator comb starting at entry `first` (entry p * entries + m - 1 = m * 2^(w p) G)
 extern "C" int ibft_debug_wtable(ibft_engine* e, uint32_t first, uint32_t count, uint8_t* out, int* w, uint32_t* entries, uint32_t* total) {
+  e = diag_engine(e);
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
   if (w) *w = e->d_wtable ? IBFT_GEN_WIDE : 0;
 #if IBFT_GEN_WIDE > 0
@@ -2028,6 +2067,7 @@ extern "C" int ibft_debug_wtable(ibft_engine* e, uint32_t first, uint32_t count,
 // engine's registry.  Waits for the device.
 extern "C" int ibft_debug_keytab(ibft_engine* e, uint32_t table_slot, uint32_t validator, uint32_t first, uint32_t count, uint8_t* out,
                                  uint32_t* state_out, uint8_t* key_out) {
+  e = diag_engine(e);
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
 #if IBFT_WC > 0
   all_lanes_lock lk(e);
@@ -2063,6 +2103,7 @@ extern "C" int ibft_debug_keytab(ibft_engine* e, uint32_t table_slot, uint32_t v
 // test hook: the key registry as a whole -- entries in use (distinct addresses of the resident tables), how many of those have a
 // finished comb table, and the bytes of comb-table chunks allocated so far.  Any output may be NULL.  Waits for the device.
 extern "C" int ibft_debug_key_registry(ibft_engine* e, uint32_t* entries_in_use, uint32_t* entries_ready, uint64_t* bytes_reserved) {
+  e = diag_engine(e);
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
   all_lanes_lock lk(e);
   const key_registry& R = e->reg;
@@ -2085,6 +2126,8 @@ extern "C" int ibft_debug_key_registry(ibft_engine* e, uint32_t* entries_in_use,
 // (the sum of the heads of the worklists that call filled; 0 when it took no known-key pass)
 extern "C" int ibft_debug_known_handed_back(ibft_engine* e, uint32_t* n_out) {
   if (!e || !n_out) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  if (e->multi) return multi_known_handed_back(e, n_out);
+  e = diag_engine(e);
   lane* L = &e->lanes[e->last_lane.load()];
   std::lock_guard<std::mutex> lk(L->mu);
   if (L->pending.active) { set_err("a submitted call is still pending"); return IBFT_ERR_INVALID_ARG; }
@@ -2124,9 +2167,14 @@ extern "C" int ibft_engine_create(const ibft_engine_params* params, ibft_engine*
   return IBFT_OK;
 }
 
-extern "C" void ibft_engine_destroy(ibft_engine* e) { engine_free(e); }
+extern "C" void ibft_engine_destroy(ibft_engine* e) {
+  if (e && e->view_of) return;  // borrowed: it goes with its coordinator
+  if (e && e->multi) return multi_destroy(e);
+  engine_free(e);
+}
 
 extern "C" int ibft_engine_device_info(ibft_engine* e, ibft_device_info* out) {
+  e = diag_engine(e);
   if (!e || !out) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   cudaDeviceProp prop;
   CU(cudaGetDeviceProperties(&prop, e->p.device));
@@ -2352,6 +2400,8 @@ static int budget_enable(ibft_engine* e) {
 
 extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t height, const uint8_t* addrs,
                                    const uint8_t* powers_be, uint32_t n) {
+  IBFT_REFUSE_VIEW(e);
+  if (e && e->multi) return multi_set_validators(e, table_slot, height, addrs, powers_be, n);
   if (!e || (!addrs && n)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   if (table_slot >= e->p.max_table_slots) { set_err("table slot %u out of range", table_slot); return IBFT_ERR_INVALID_ARG; }
   if (n > e->p.max_validators) { set_err("validator table of %u exceeds capacity %u", n, e->p.max_validators); return IBFT_ERR_CAPACITY; }
@@ -2557,6 +2607,8 @@ static int refresh_key_tables_locked(ibft_engine* e, lane* L, uint32_t* n_ready_
 }
 extern "C" int ibft_refresh_key_tables(ibft_engine* e, uint32_t* n_keys_out) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (e->multi) return multi_refresh_key_tables(e, n_keys_out);
   lane* L = &e->lanes[0];
   std::unique_lock<std::mutex> lk(L->mu), lk1;
   if (L->pending.active) { set_err("a submitted call is still pending"); return IBFT_ERR_INVALID_ARG; }
@@ -2574,6 +2626,8 @@ extern "C" int ibft_refresh_key_tables(ibft_engine* e, uint32_t* n_keys_out) {
 
 extern "C" int ibft_set_key_table_budget(ibft_engine* e, uint32_t max_tables) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (e->multi) return multi_set_key_table_budget(e, max_tables);
 #if IBFT_WC > 0
   if (!(e->p.flags & IBFT_FLAG_KEY_CACHE) || !e->reg.d_state) { set_err("engine has no key registry"); return IBFT_ERR_INVALID_ARG; }
   all_lanes_lock lk(e);
@@ -2596,6 +2650,7 @@ extern "C" int ibft_set_key_table_budget(ibft_engine* e, uint32_t max_tables) {
 
 extern "C" int ibft_get_quorum(ibft_engine* e, uint32_t table_slot, uint64_t quorum_out[5], uint64_t* height_out,
                                uint32_t* n_out) {
+  e = diag_engine(e);
   if (!e || table_slot >= e->p.max_table_slots) { set_err("bad slot"); return IBFT_ERR_INVALID_ARG; }
   std::lock_guard<std::mutex> lk(e->lanes[0].mu);
   const slot_host& s = e->slots[table_slot];
@@ -2809,7 +2864,8 @@ static void stage_copy(void* dst, const void* src, size_t bytes) {
 
 static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
                          const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
-                         ibft_group_result* results_out, uint8_t* recovered_out) {
+                         ibft_group_result* results_out, uint8_t* recovered_out, bool votes_only = false) {
+  // votes_only: a shard of a multi-device call -- record the votes, leave the reduce to the coordinator's merge
   if (L->pending.active) { set_err("a submitted call is still pending; wait for it first"); return IBFT_ERR_INVALID_ARG; }
   if ((n && !items) || (n && !bitmap_out) || (arena_len && !arena) || (n_groups && !groups)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   if (n > L->cap_items || arena_len > L->cap_arena || n_groups > e->p.max_groups) {
@@ -2833,7 +2889,7 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
   }
   cudaStream_t st = L->stream;
   if (arena_len) {
-    memcpy(L->h_arena, arena, arena_len);
+    if (arena != L->h_arena) memcpy(L->h_arena, arena, arena_len);  // a shard is planned straight into the staging
     CU(cudaMemcpyAsync(L->d_arena, L->h_arena, arena_len, cudaMemcpyHostToDevice, st));
   }
   if (n_groups) {
@@ -2842,7 +2898,7 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
   }
   // quorum requested: the recover kernels record the votes themselves (no k_quorum_mark pass over the tuples afterwards)
   vote_sink sink{nullptr, nullptr, nullptr};
-  if (n_groups && results_out) {
+  if (n_groups && (results_out || votes_only)) {
     CU(cudaMemsetAsync(L->d_voted, 0, std::max<size_t>(voted_words, 1) * 4, st));
     CU(cudaMemsetAsync(L->d_nvalid, 0, (size_t)n_groups * 4, st));
     sink = vote_sink{L->d_voted, L->d_nvalid, L->d_gdev};
@@ -3002,14 +3058,8 @@ static lane* acquire_lane(ibft_engine* e, uint32_t n, size_t arena_len) {
   return big;
 }
 
-static int verify_batch_on_lane(ibft_engine* e, lane* L, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
-                                const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
-                                uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words) {
-  int rc = submit_locked(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out);
-  if (rc != IBFT_OK) return rc;
-  rc = wait_locked(e, L);
-  if (rc != IBFT_OK) return rc;
-  if (status_out && n) memcpy(status_out, L->h_status, n);
+// the voted sets of the lane's last call into voted_out (n_groups rows of voted_stride_words words)
+static int copy_voted(ibft_engine* e, lane* L, uint32_t n_groups, bool recorded, uint32_t* voted_out, uint32_t voted_stride_words) {
   if (voted_out && n_groups) {
     CU(cudaSetDevice(e->p.device));
     for (uint32_t g = 0; g < n_groups; g++) {
@@ -3017,7 +3067,7 @@ static int verify_batch_on_lane(ibft_engine* e, lane* L, const ibft_sig_item* it
       uint32_t* dst = voted_out + (size_t)g * voted_stride_words;
       uint32_t w = std::min<uint32_t>(gd.n_words, voted_stride_words);
       // without results_out the recover kernels recorded no votes: the sets are all-zero by definition
-      if (w && results_out) CU(cudaMemcpyAsync(dst, L->d_voted + gd.voted_off, (size_t)w * 4, cudaMemcpyDeviceToHost, L->stream));
+      if (w && recorded) CU(cudaMemcpyAsync(dst, L->d_voted + gd.voted_off, (size_t)w * 4, cudaMemcpyDeviceToHost, L->stream));
       else w = 0;
       for (uint32_t i = w; i < voted_stride_words; i++) dst[i] = 0;
     }
@@ -3026,10 +3076,24 @@ static int verify_batch_on_lane(ibft_engine* e, lane* L, const ibft_sig_item* it
   return IBFT_OK;
 }
 
+static int verify_batch_on_lane(ibft_engine* e, lane* L, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                                const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
+                                uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words) {
+  int rc = submit_locked(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out);
+  if (rc != IBFT_OK) return rc;
+  rc = wait_locked(e, L);
+  if (rc != IBFT_OK) return rc;
+  if (status_out && n) memcpy(status_out, L->h_status, n);
+  return copy_voted(e, L, n_groups, results_out != nullptr, voted_out, voted_stride_words);
+}
+
 extern "C" int ibft_verify_batch(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
                                  const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
                                  ibft_group_result* results_out, uint8_t* recovered_out) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (e->multi)
+    return multi_verify(e, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, nullptr, nullptr, 0);
   lane* L = acquire_lane(e, n, arena_len);
   std::lock_guard<std::mutex> lk(L->mu, std::adopt_lock);
   return verify_batch_on_lane(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, nullptr, nullptr, 0);
@@ -3041,6 +3105,10 @@ extern "C" int ibft_verify_batch_ex(ibft_engine* e, const ibft_sig_item* items, 
                                     uint32_t voted_stride_words) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
   if (voted_out && !results_out) { set_err("voted_out needs results_out (votes are recorded only when quorum results are requested)"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (e->multi)
+    return multi_verify(e, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, status_out, voted_out,
+                        voted_stride_words);
   lane* L = acquire_lane(e, n, arena_len);
   std::lock_guard<std::mutex> lk(L->mu, std::adopt_lock);
   return verify_batch_on_lane(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, status_out, voted_out,
@@ -3049,6 +3117,8 @@ extern "C" int ibft_verify_batch_ex(ibft_engine* e, const ibft_sig_item* items, 
 
 extern "C" int ibft_last_item_status(ibft_engine* e, uint8_t* status_out, uint32_t n) {
   if (!e || (n && !status_out)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  if (e->multi) return multi_last_item_status(e, status_out, n);
+  e = diag_engine(e);
   lane* L = &e->lanes[e->last_lane.load()];
   std::lock_guard<std::mutex> lk(L->mu);
   if (L->pending.active) { set_err("a submitted call is still pending"); return IBFT_ERR_INVALID_ARG; }
@@ -3063,6 +3133,8 @@ extern "C" int ibft_verify_submit(ibft_engine* e, const ibft_sig_item* items, ui
                                   const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
                                   ibft_group_result* results_out, uint8_t* recovered_out) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (e->multi) return multi_submit(e, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out);
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
   return submit_locked(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out);
@@ -3070,6 +3142,8 @@ extern "C" int ibft_verify_submit(ibft_engine* e, const ibft_sig_item* items, ui
 
 extern "C" int ibft_verify_poll(ibft_engine* e, int* done) {
   if (!e || !done) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (e->multi) return multi_poll(e, done);
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
   if (!L->pending.active) { *done = 1; return IBFT_OK; }
@@ -3083,6 +3157,8 @@ extern "C" int ibft_verify_poll(ibft_engine* e, int* done) {
 
 extern "C" int ibft_verify_wait(ibft_engine* e) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (e->multi) return multi_wait(e);
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
   return wait_locked(e, L);
@@ -3090,6 +3166,7 @@ extern "C" int ibft_verify_wait(ibft_engine* e) {
 
 extern "C" int ibft_verify_batch_device(ibft_engine* e, const void* d_items, uint32_t n, const void* d_arena, size_t arena_len,
                                         uint32_t shard_lo, uint32_t shard_hi, void* d_bitmap, void* d_recovered, void* stream) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || (n && (!d_items || !d_bitmap))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   if (shard_hi > n || shard_lo > shard_hi || (shard_lo & 31) || ((shard_hi & 31) && shard_hi != n)) {
     set_err("shard [%u,%u) of %u must be 32-aligned", shard_lo, shard_hi, n);
@@ -3109,6 +3186,7 @@ extern "C" int ibft_verify_batch_device(ibft_engine* e, const void* d_items, uin
 
 // binds the groups used by the device-resident entry points (copied to the engine's device buffers)
 extern "C" int ibft_bind_groups(ibft_engine* e, const ibft_group_desc* groups, uint32_t n_groups) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || (n_groups && !groups)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   if (n_groups > e->p.max_groups) { set_err("too many groups"); return IBFT_ERR_CAPACITY; }
   lane* L = &e->lanes[0];
@@ -3132,6 +3210,7 @@ extern "C" int ibft_bind_groups(ibft_engine* e, const ibft_group_desc* groups, u
 
 extern "C" int ibft_quorum_reduce_device(ibft_engine* e, const void* d_items, uint32_t n, const void* d_bitmap,
                                          const void* d_groups, uint32_t n_groups, void* d_results, void* stream) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !d_results || (n && (!d_items || !d_bitmap))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
@@ -3146,6 +3225,7 @@ extern "C" int ibft_quorum_reduce_device(ibft_engine* e, const void* d_items, ui
 }
 
 extern "C" int ibft_quorum_partial_words(ibft_engine* e, uint32_t* words_out) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !words_out) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
@@ -3157,6 +3237,7 @@ extern "C" int ibft_quorum_partial_words(ibft_engine* e, uint32_t* words_out) {
 
 extern "C" int ibft_quorum_mark_device(ibft_engine* e, const void* d_items, uint32_t n, uint32_t shard_lo, uint32_t shard_hi,
                                        const void* d_bitmap, void* d_partial, void* stream) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !d_partial || (n && (!d_items || !d_bitmap))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   if (shard_hi > n || shard_lo > shard_hi) { set_err("bad shard"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
@@ -3181,6 +3262,7 @@ extern "C" int ibft_quorum_mark_device(ibft_engine* e, const void* d_items, uint
 
 extern "C" int ibft_quorum_merge_device(ibft_engine* e, const void* d_partials, uint32_t n_parts, uint32_t part_stride_words,
                                         void* d_results, void* stream) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !d_partials || !d_results || n_parts == 0) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
@@ -3208,6 +3290,7 @@ extern "C" int ibft_quorum_merge_device(ibft_engine* e, const void* d_partials, 
 // which is what makes the mapping dereferenceable from the peer's kernels over NVLink.
 static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle is 64 bytes");
 extern "C" int ibft_exchange_alloc(ibft_engine* e, uint32_t words, void** d_buf_out, uint8_t handle_out[64]) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !d_buf_out || !handle_out || words == 0) { set_err("bad argument"); return IBFT_ERR_INVALID_ARG; }
   CU(cudaSetDevice(e->p.device));
   void* p = nullptr;
@@ -3221,6 +3304,7 @@ extern "C" int ibft_exchange_alloc(ibft_engine* e, uint32_t words, void** d_buf_
   return IBFT_OK;
 }
 extern "C" int ibft_exchange_open(ibft_engine* e, const uint8_t handle[64], void** d_peer_out) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !handle || !d_peer_out) { set_err("bad argument"); return IBFT_ERR_INVALID_ARG; }
   CU(cudaSetDevice(e->p.device));
   cudaIpcMemHandle_t h;
@@ -3231,12 +3315,14 @@ extern "C" int ibft_exchange_open(ibft_engine* e, const uint8_t handle[64], void
   return IBFT_OK;
 }
 extern "C" int ibft_exchange_close(ibft_engine* e, void* d_peer) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !d_peer) { set_err("bad argument"); return IBFT_ERR_INVALID_ARG; }
   CU(cudaSetDevice(e->p.device));
   CU(cudaIpcCloseMemHandle(d_peer));
   return IBFT_OK;
 }
 extern "C" int ibft_exchange_free(ibft_engine* e, void* d_buf) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !d_buf) { set_err("bad argument"); return IBFT_ERR_INVALID_ARG; }
   CU(cudaSetDevice(e->p.device));
   CU(cudaDeviceSynchronize());
@@ -3244,6 +3330,7 @@ extern "C" int ibft_exchange_free(ibft_engine* e, void* d_buf) {
   return IBFT_OK;
 }
 extern "C" int ibft_exchange_clear(ibft_engine* e, void* d_buf, uint32_t word_off, uint32_t words, void* stream) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !d_buf) { set_err("bad argument"); return IBFT_ERR_INVALID_ARG; }
   CU(cudaSetDevice(e->p.device));
   CU(cudaMemsetAsync((uint32_t*)d_buf + word_off, 0, (size_t)words * 4, stream ? (cudaStream_t)stream : e->lanes[0].stream));
@@ -3253,6 +3340,7 @@ extern "C" int ibft_exchange_clear(ibft_engine* e, void* d_buf, uint32_t word_of
 extern "C" int ibft_quorum_exchange_device(ibft_engine* e, const uint64_t* peer_bufs_in, uint32_t world, uint32_t rank,
                                            uint32_t words_per_rank, uint32_t bitmap_words_per_rank, uint32_t epoch, void* d_bitmap_full,
                                            void* d_results, void* d_timeout_flag, void* stream) {
+  IBFT_REFUSE_MULTI(e);
   if (!e || !peer_bufs_in || !d_bitmap_full || !d_results || !d_timeout_flag || world == 0 || world > 8 || rank >= world || epoch == 0) {
     set_err("bad argument");
     return IBFT_ERR_INVALID_ARG;
@@ -3285,6 +3373,7 @@ extern "C" int ibft_quorum_exchange_device(ibft_engine* e, const uint64_t* peer_
 }
 
 extern "C" int ibft_get_voted_bitmap(ibft_engine* e, uint32_t group, uint32_t* words_out, uint32_t n_words) {
+  e = diag_engine(e);  // a coordinator's merged voted sets are on its lead device
   if (!e || !words_out) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[e->last_lane.load()];
   std::lock_guard<std::mutex> lk(L->mu);
@@ -3351,7 +3440,9 @@ static int hash_batch_locked(ibft_engine* e, const uint8_t* arena, size_t arena_
 extern "C" int ibft_keccak256_batch(ibft_engine* e, const uint8_t* arena, size_t arena_len, const uint32_t* offsets,
                                     const uint32_t* lens, uint32_t n, uint8_t* out32) {
   if (!e || (n && (!offsets || !lens || !out32)) || (arena_len && !arena)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
   if (n == 0) return IBFT_OK;
+  if (e->multi) return multi_hash(e, arena, arena_len, offsets, lens, nullptr, n, out32);
   std::lock_guard<std::mutex> lk(e->hash_mu);
   return hash_batch_locked(e, arena, arena_len, offsets, lens, nullptr, n, out32);
 }
@@ -3359,7 +3450,9 @@ extern "C" int ibft_keccak256_batch(ibft_engine* e, const uint8_t* arena, size_t
 extern "C" int ibft_proposal_hash_batch(ibft_engine* e, const uint8_t* arena, size_t arena_len, const uint32_t* offsets,
                                         const uint32_t* lens, const uint64_t* rounds, uint32_t n, uint8_t* out32) {
   if (!e || (n && (!offsets || !lens || !rounds || !out32)) || (arena_len && !arena)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
   if (n == 0) return IBFT_OK;
+  if (e->multi) return multi_hash(e, arena, arena_len, offsets, lens, rounds, n, out32);
   std::lock_guard<std::mutex> lk(e->hash_mu);
   return hash_batch_locked(e, arena, arena_len, offsets, lens, rounds, n, out32);
 }
@@ -3367,7 +3460,9 @@ extern "C" int ibft_proposal_hash_batch(ibft_engine* e, const uint8_t* arena, si
 static int sign_batch(ibft_engine* e, const uint8_t* privkeys, const uint8_t* digests, const uint8_t* nonces, bool rfc6979,
                       uint32_t n, uint8_t* sigs65_out) {
   if (!e || (n && (!privkeys || !digests || !sigs65_out))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
   if (n == 0) return IBFT_OK;
+  if (e->multi) return multi_sign(e, privkeys, digests, nonces, rfc6979, n, sigs65_out);
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
   CU(cudaSetDevice(e->p.device));
@@ -3411,13 +3506,20 @@ extern "C" int ibft_sign_batch_rfc6979(ibft_engine* e, const uint8_t* privkeys, 
 
 extern "C" int ibft_set_recover_path(ibft_engine* e, int path) {
   if (e == nullptr || path < IBFT_PATH_AUTO || path > IBFT_PATH_QSPLIT) { set_err("bad recover path"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (e->multi) return multi_set_recover_path(e, path);
   e->recover_path.store(path);
   return IBFT_OK;
 }
 
-extern "C" uint64_t ibft_engine_launch_count(ibft_engine* e) { return e ? e->launches.load() : 0; }
+extern "C" uint64_t ibft_engine_launch_count(ibft_engine* e) {
+  if (e && e->multi) return multi_launch_count(e);
+  e = diag_engine(e);
+  return e ? e->launches.load() : 0;
+}
 
 extern "C" int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* wide_mac_per_s) {
+  e = diag_engine(e);
   if (!e || !imad_per_s || !wide_mac_per_s) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
@@ -3455,6 +3557,7 @@ extern "C" int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* w
 
 extern "C" int ibft_debug_op(ibft_engine* e, int op, const uint8_t* a, const uint8_t* b, const uint8_t* c, uint32_t n,
                              uint8_t* out, uint32_t out_stride) {
+  e = diag_engine(e);
   if (!e || !a || !out || n == 0 || (op == IBFT_DBG_RFC6979 && (!b || !c))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
@@ -3482,4 +3585,553 @@ done:
 #undef CUK
   cudaFree(d_a); cudaFree(d_b); cudaFree(d_c); cudaFree(d_o);
   return rc;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// multi-device engines (ibft_engine_create_multi)
+// ------------------------------------------------------------------------------------------------------------
+// A coordinator holds one ordinary engine per listed device (its sub-engines; the first is the lead).  A host-buffer verify call
+// is cut into contiguous 32-aligned shards (shard_plan.hpp); each shard is planned straight into its device's pinned staging with
+// an arena of its own, and each device verifies it through the usual staging, chunking and key-registry paths, recording its votes
+// without a reduce.  The lead then gathers every device's voted sets and valid counts with peer copies (ordered by the devices'
+// completion events; they work with or without peer access and on a repeated ordinal) and runs the merge and the weighted reduce
+// of the device-resident multi-GPU path.  Caller buffers are written only once every device has succeeded.
+
+// one host-buffer call in flight on a lane kind
+struct multi_call {
+  bool active = false;
+  uint32_t n = 0, n_groups = 0, used = 0;  // used: devices [0, used) hold its shards
+  bool merge = false;                      // quorum results of a call on more than one device: merged on the lead
+  uint32_t* bitmap_out = nullptr;
+  ibft_group_result* results_out = nullptr;
+  uint8_t* recovered_out = nullptr;
+  std::vector<std::vector<uint32_t>> bitmap;   // each shard's verdict words and recovered addresses, until every device is done
+  std::vector<std::vector<uint8_t>> recovered;
+};
+
+// a slot's table as the devices hold it, for the roll-back of a replication that failed part way
+struct multi_table {
+  bool valid = false;
+  uint64_t height = 0;
+  uint32_t n = 0;
+  std::vector<uint8_t> addrs, powers;  // powers empty: unit power
+};
+
+struct multi_engine {
+  std::vector<ibft_engine*> subs;   // one per listed device, in list order
+  std::vector<ibft_engine*> views;  // their ibft_engine_sub handles
+  // verify, hash and sign calls share it; the calls that replace tables or change the key registries hold it alone, so that no
+  // call ever sees the devices disagree
+  std::shared_mutex state_mu;
+  uint32_t* d_parts[IBFT_LANES] = {nullptr, nullptr};  // on the lead, per lane kind: one partial (voted words | valid counts) per device
+  cudaEvent_t merged[IBFT_LANES] = {nullptr, nullptr};
+  multi_call pending;  // the asynchronous API (lane 0); guarded by the lead's lane-0 mutex
+  std::mutex last_mu;  // the most recent completed host-buffer call
+  std::vector<uint8_t> last_status;
+  uint32_t last_used = 0;
+  std::vector<multi_table> tables;
+};
+
+static int multi_refused(ibft_engine* e, const char* fn) {
+  if (e->view_of) set_err("%s: a sub-engine handle (ibft_engine_sub) answers diagnostics only", fn);
+  else set_err("%s takes device pointers of one device: a multi-device engine has no such call; use one engine per device "
+               "(go-ibft_b200/sharding.py)", fn);
+  return IBFT_ERR_INVALID_ARG;
+}
+
+static ibft_engine* diag_engine(ibft_engine* e) {
+  if (e && e->multi) return e->multi->subs[0];
+  if (e && e->view_of) return e->view_of;
+  return e;
+}
+
+// lane `kind` of devices [0, used), in device-list order: two calls never wait for each other in a cycle
+struct multi_lanes_lock {
+  multi_engine* M;
+  int kind;
+  uint32_t used;
+  multi_lanes_lock(multi_engine* M_, int kind_, uint32_t used_) : M(M_), kind(kind_), used(used_) {
+    for (uint32_t k = 0; k < used; k++) M->subs[k]->lanes[kind].mu.lock();
+  }
+  ~multi_lanes_lock() {
+    for (uint32_t k = used; k-- > 0;) M->subs[k]->lanes[kind].mu.unlock();
+  }
+};
+
+// fn(k) for every device k < used, each on a thread of its own (k = 0 on the caller's) when `parallel`; returns the first failure,
+// with its error text on the calling thread
+static int for_devices(uint32_t used, bool parallel, const std::function<int(uint32_t)>& fn) {
+  std::vector<int> rc(used, IBFT_OK);
+  std::vector<std::string> err(used);
+  auto one = [&](uint32_t k) {
+    rc[k] = fn(k);
+    if (rc[k] != IBFT_OK) err[k] = tl_err;
+  };
+  std::vector<std::thread> th;
+  for (uint32_t k = parallel ? 1 : used; k < used; k++) th.emplace_back(one, k);
+  if (parallel) one(0);
+  else
+    for (uint32_t k = 0; k < used; k++) one(k);
+  for (auto& t : th) t.join();
+  for (uint32_t k = 0; k < used; k++)
+    if (rc[k] != IBFT_OK) {
+      set_err("device %u: %s", k, err[k].c_str());
+      return rc[k];
+    }
+  return IBFT_OK;
+}
+
+// the lead gathers every shard's voted sets and valid counts and reduces them; enqueued on the lead's lane stream
+static int multi_merge_enqueue(multi_engine* M, int kind, uint32_t used, uint32_t n_groups) {
+  ibft_engine* lead = M->subs[0];
+  lane* L0 = &lead->lanes[kind];
+  size_t vw = 0;
+  for (auto& g : L0->last_gdev) vw += g.n_words;
+  const size_t stride = vw + n_groups;
+  CU(cudaSetDevice(lead->p.device));
+  cudaStream_t st = L0->stream;
+  uint32_t parts = 0;
+  for (uint32_t k = 0; k < used; k++) {
+    ibft_engine* s = M->subs[k];
+    lane* L = &s->lanes[kind];
+    if (!L->pending.active) continue;  // an empty trailing shard
+    if (k) CU(cudaStreamWaitEvent(st, L->done_ev, 0));
+    uint32_t* dst = M->d_parts[kind] + parts * stride;
+    if (vw) CU(cudaMemcpyPeerAsync(dst, lead->p.device, L->d_voted, s->p.device, vw * 4, st));
+    CU(cudaMemcpyPeerAsync(dst + vw, lead->p.device, L->d_nvalid, s->p.device, (size_t)n_groups * 4, st));
+    parts++;
+  }
+  k_quorum_merge<<<(uint32_t)((stride + 255) / 256), 256, 0, st>>>(M->d_parts[kind], parts, (uint32_t)stride, (uint32_t)vw, n_groups,
+                                                                   L0->d_voted, L0->d_nvalid);
+  lead->launches++;
+  CU(cudaGetLastError());
+  k_quorum_reduce<<<n_groups, IBFT_REDUCE_THREADS, 0, st>>>(L0->d_groups, L0->d_gdev, n_groups, lead->d_slots, lead->p.max_table_slots,
+                                                            L0->d_voted, L0->d_nvalid, L0->d_results);
+  lead->launches++;
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(L0->h_results, L0->d_results, (size_t)n_groups * sizeof(ibft_group_result), cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(M->merged[kind], st));
+  return IBFT_OK;
+}
+
+// Stages and enqueues a call on lane `kind` of devices [0, used), whose mutexes the caller holds.  Nothing is written to the
+// caller's buffers here.
+static int multi_submit_locked(ibft_engine* E, int kind, uint32_t used, const ibft_sig_item* items, uint32_t n, const uint8_t* arena,
+                               size_t arena_len, const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
+                               ibft_group_result* results_out, uint8_t* recovered_out, multi_call& mc) {
+  multi_engine* M = E->multi;
+  ibft_engine* lead = M->subs[0];
+  lane* L0 = &lead->lanes[kind];
+  for (uint32_t k = 0; k < used; k++)
+    if (M->subs[k]->lanes[kind].pending.active) { set_err("a submitted call is still pending; wait for it first"); return IBFT_ERR_INVALID_ARG; }
+  mc = multi_call{};
+  mc.n = n;
+  mc.n_groups = n_groups;
+  mc.used = used;
+  mc.bitmap_out = bitmap_out;
+  mc.results_out = results_out;
+  mc.recovered_out = recovered_out;
+  if (used == 1) {  // the lead's own call, as on a single-device engine
+    int rc = submit_locked(lead, L0, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out);
+    mc.active = rc == IBFT_OK;
+    return rc;
+  }
+  // the checks of a single-device call, on the host before any device is touched
+  if ((n && !items) || (n && !bitmap_out) || (arena_len && !arena) || (n_groups && !groups)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  if (n > L0->cap_items || arena_len > L0->cap_arena || n_groups > E->p.max_groups) {
+    set_err("batch (%u items, %zu payload bytes, %u groups) exceeds engine capacity (%u, %zu, %u)", n, arena_len, n_groups,
+            L0->cap_items, L0->cap_arena, E->p.max_groups);
+    return IBFT_ERR_CAPACITY;
+  }
+  if (n_groups) {
+    std::vector<group_dev> gdev(n_groups);
+    size_t voted_words = 0;
+    int rc = plan_groups(lead, L0, groups, n_groups, gdev.data(), &voted_words);
+    if (rc != IBFT_OK) return rc;
+  }
+  mc.merge = n_groups && results_out;
+  mc.bitmap.resize(used);
+  mc.recovered.resize(used);
+  // each device plans its shard into its own pinned staging: large pageable batches are staged on all devices at once
+  const bool parallel = (uint64_t)n * sizeof(ibft_sig_item) + arena_len >= (4u << 20);
+  int rc = for_devices(used, parallel, [&](uint32_t k) {
+    ibft_engine* s = M->subs[k];
+    lane* L = &s->lanes[kind];
+    uint32_t lo, hi;
+    shard_bounds(n, used, k, &lo, &hi);
+    if (hi == lo) return IBFT_OK;
+    std::vector<arena_run> runs;
+    const size_t len = plan_shard(items, lo, hi, arena_len, L->h_items, runs);
+    copy_runs(arena, runs, L->h_arena);
+    mc.bitmap[k].assign((hi - lo + 31) / 32, 0);
+    if (recovered_out) mc.recovered[k].assign((size_t)(hi - lo) * 20, 0);
+    return submit_locked(s, L, L->h_items, hi - lo, L->h_arena, len, groups, n_groups, mc.bitmap[k].data(), nullptr,
+                         recovered_out ? mc.recovered[k].data() : nullptr, /*votes_only=*/mc.merge);
+  });
+  if (rc == IBFT_OK && mc.merge) rc = multi_merge_enqueue(M, kind, used, n_groups);
+  if (rc != IBFT_OK) {  // drain what was enqueued; its outputs go to this call's own buffers
+    const std::string err = tl_err;
+    for (uint32_t k = 0; k < used; k++)
+      if (M->subs[k]->lanes[kind].pending.active) (void)wait_locked(M->subs[k], &M->subs[k]->lanes[kind]);
+    if (mc.merge) {
+      cudaSetDevice(lead->p.device);
+      (void)cudaStreamSynchronize(L0->stream);
+    }
+    set_err("%s", err.c_str());
+    return rc;
+  }
+  mc.active = true;
+  return IBFT_OK;
+}
+
+// Waits for a call of multi_submit_locked (same lanes held) and, once every device has succeeded, writes the caller's buffers.
+static int multi_wait_locked(ibft_engine* E, int kind, multi_call& mc, uint8_t* status_out, uint32_t* voted_out,
+                             uint32_t voted_stride_words) {
+  multi_engine* M = E->multi;
+  if (!mc.active) { set_err("no submitted call to wait for"); return IBFT_ERR_INVALID_ARG; }
+  mc.active = false;
+  ibft_engine* lead = M->subs[0];
+  lane* L0 = &lead->lanes[kind];
+  if (mc.used == 1) {
+    int rc = wait_locked(lead, L0);
+    if (rc != IBFT_OK) return rc;
+  } else {
+    int rc = IBFT_OK;
+    std::string err;
+    for (uint32_t k = 0; k < mc.used; k++) {
+      lane* L = &M->subs[k]->lanes[kind];
+      if (!L->pending.active) continue;
+      int r = wait_locked(M->subs[k], L);
+      if (r != IBFT_OK && rc == IBFT_OK) { rc = r; err = tl_err; }
+    }
+    if (mc.merge) {
+      cudaError_t ce = cudaSetDevice(lead->p.device);
+      if (ce == cudaSuccess) ce = cudaEventSynchronize(M->merged[kind]);
+      if (ce != cudaSuccess && rc == IBFT_OK) {
+        rc = IBFT_ERR_CUDA;
+        err = std::string("quorum merge on the lead device failed: ") + cudaGetErrorString(ce);
+      }
+    }
+    if (rc != IBFT_OK) { set_err("%s", err.c_str()); return rc; }
+    for (uint32_t k = 0; k < mc.used; k++) {
+      uint32_t lo, hi;
+      shard_bounds(mc.n, mc.used, k, &lo, &hi);
+      if (hi == lo) continue;
+      memcpy(mc.bitmap_out + lo / 32, mc.bitmap[k].data(), mc.bitmap[k].size() * 4);
+      if (mc.recovered_out) memcpy(mc.recovered_out + (size_t)lo * 20, mc.recovered[k].data(), mc.recovered[k].size());
+    }
+    if (mc.merge) memcpy(mc.results_out, L0->h_results, (size_t)mc.n_groups * sizeof(ibft_group_result));
+  }
+  {
+    std::lock_guard<std::mutex> lk(M->last_mu);
+    M->last_status.resize(mc.n);
+    for (uint32_t k = 0; k < mc.used; k++) {
+      uint32_t lo, hi;
+      shard_bounds(mc.n, mc.used, k, &lo, &hi);
+      if (hi > lo) memcpy(M->last_status.data() + lo, M->subs[k]->lanes[kind].h_status, hi - lo);
+    }
+    M->last_used = mc.used;
+    if (status_out && mc.n) memcpy(status_out, M->last_status.data(), mc.n);
+  }
+  return copy_voted(lead, L0, mc.n_groups, mc.results_out != nullptr, voted_out, voted_stride_words);
+}
+
+static int multi_verify(ibft_engine* E, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                        const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
+                        uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words) {
+  multi_engine* M = E->multi;
+  std::shared_lock<std::shared_mutex> st(M->state_mu);
+  const lane& small = M->subs[0]->lanes[1];
+  const int kind = n <= small.cap_items && arena_len <= small.cap_arena ? 1 : 0;  // chosen once, for every device
+  const uint32_t used = shard_devices(n, (uint32_t)M->subs.size());
+  multi_lanes_lock lk(M, kind, used);
+  multi_call mc;
+  int rc = multi_submit_locked(E, kind, used, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, mc);
+  if (rc != IBFT_OK) return rc;
+  return multi_wait_locked(E, kind, mc, status_out, voted_out, voted_stride_words);
+}
+
+static int multi_submit(ibft_engine* E, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                        const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
+                        uint8_t* recovered_out) {
+  multi_engine* M = E->multi;
+  std::shared_lock<std::shared_mutex> st(M->state_mu);
+  multi_lanes_lock lk(M, 0, (uint32_t)M->subs.size());
+  return multi_submit_locked(E, 0, shard_devices(n, (uint32_t)M->subs.size()), items, n, arena, arena_len, groups, n_groups, bitmap_out,
+                             results_out, recovered_out, M->pending);
+}
+
+static int multi_poll(ibft_engine* E, int* done) {
+  multi_engine* M = E->multi;
+  multi_lanes_lock lk(M, 0, (uint32_t)M->subs.size());
+  *done = 1;
+  if (!M->pending.active) return IBFT_OK;
+  auto query = [&](ibft_engine* s, cudaEvent_t ev) {
+    CU(cudaSetDevice(s->p.device));
+    cudaError_t ce = cudaEventQuery(ev);
+    if (ce == cudaErrorNotReady) *done = 0;
+    else if (ce != cudaSuccess) { set_err("device execution failed: %s", cudaGetErrorString(ce)); return IBFT_ERR_CUDA; }
+    return IBFT_OK;
+  };
+  for (uint32_t k = 0; k < M->pending.used && *done; k++) {
+    ibft_engine* s = M->subs[k];
+    if (!s->lanes[0].pending.active) continue;
+    int rc = query(s, s->lanes[0].done_ev);
+    if (rc != IBFT_OK) return rc;
+  }
+  if (M->pending.merge && *done) return query(M->subs[0], M->merged[0]);
+  return IBFT_OK;
+}
+
+static int multi_wait(ibft_engine* E) {
+  multi_engine* M = E->multi;
+  multi_lanes_lock lk(M, 0, (uint32_t)M->subs.size());
+  return multi_wait_locked(E, 0, M->pending, nullptr, nullptr, 0);
+}
+
+static int multi_last_item_status(ibft_engine* E, uint8_t* status_out, uint32_t n) {
+  multi_engine* M = E->multi;
+  {
+    std::lock_guard<std::mutex> lk(M->subs[0]->lanes[0].mu);
+    if (M->pending.active) { set_err("a submitted call is still pending"); return IBFT_ERR_INVALID_ARG; }
+  }
+  std::lock_guard<std::mutex> lk(M->last_mu);
+  if (n > M->last_status.size()) { set_err("last call had %zu items", M->last_status.size()); return IBFT_ERR_INVALID_ARG; }
+  memcpy(status_out, M->last_status.data(), n);
+  return IBFT_OK;
+}
+
+static int multi_known_handed_back(ibft_engine* E, uint32_t* n_out) {
+  multi_engine* M = E->multi;
+  uint32_t used;
+  {
+    std::lock_guard<std::mutex> lk(M->last_mu);
+    used = M->last_used;
+  }
+  uint32_t total = 0;
+  for (uint32_t k = 0; k < used; k++) {
+    uint32_t c = 0;
+    int rc = ibft_debug_known_handed_back(M->subs[k], &c);
+    if (rc != IBFT_OK) return rc;
+    total += c;
+  }
+  *n_out = total;
+  return IBFT_OK;
+}
+
+static int multi_hash(ibft_engine* E, const uint8_t* arena, size_t arena_len, const uint32_t* offsets, const uint32_t* lens,
+                      const uint64_t* rounds, uint32_t n, uint8_t* out32) {
+  multi_engine* M = E->multi;
+  std::shared_lock<std::shared_mutex> st(M->state_mu);
+  const uint32_t used = shard_devices(n, (uint32_t)M->subs.size());
+  std::vector<uint8_t> out((size_t)n * 32);
+  int rc = for_devices(used, true, [&](uint32_t k) {
+    uint32_t lo, hi;
+    shard_bounds(n, used, k, &lo, &hi);
+    if (hi == lo) return IBFT_OK;
+    ibft_engine* s = M->subs[k];
+    std::lock_guard<std::mutex> lk(s->hash_mu);
+    return hash_batch_locked(s, arena, arena_len, offsets + lo, lens + lo, rounds ? rounds + lo : nullptr, hi - lo, out.data() + (size_t)lo * 32);
+  });
+  if (rc == IBFT_OK) memcpy(out32, out.data(), out.size());
+  return rc;
+}
+
+static int multi_sign(ibft_engine* E, const uint8_t* privkeys, const uint8_t* digests, const uint8_t* nonces, bool rfc6979, uint32_t n,
+                      uint8_t* sigs65_out) {
+  multi_engine* M = E->multi;
+  std::shared_lock<std::shared_mutex> st(M->state_mu);
+  const uint32_t used = shard_devices(n, (uint32_t)M->subs.size());
+  std::vector<uint8_t> out((size_t)n * 65);
+  int rc = for_devices(used, true, [&](uint32_t k) {
+    uint32_t lo, hi;
+    shard_bounds(n, used, k, &lo, &hi);
+    if (hi == lo) return IBFT_OK;
+    return sign_batch(M->subs[k], privkeys + (size_t)lo * 32, digests + (size_t)lo * 32, nonces ? nonces + (size_t)lo * 32 : nullptr, rfc6979,
+                      hi - lo, out.data() + (size_t)lo * 65);
+  });
+  if (rc == IBFT_OK) memcpy(sigs65_out, out.data(), out.size());
+  return rc;
+}
+
+// Unsets a slot: the roll-back, on the devices that already took it, of a table another device refused
+static void slot_clear(ibft_engine* e, uint32_t slot) {
+  all_lanes_lock lk(e);
+  cudaSetDevice(e->p.device);
+  cudaDeviceSynchronize();
+  slot_host old = std::move(e->slots[slot]);
+  e->slots[slot] = slot_host{};
+  registry_release(e, old.key_ref);
+  cudaFree(old.d_keys); cudaFree(old.d_powers); cudaFree(old.d_key_ref);
+  e->slots_shadow[slot] = slot_dev{};
+  cudaMemcpy(e->d_slots + slot, &e->slots_shadow[slot], sizeof(slot_dev), cudaMemcpyHostToDevice);
+#if IBFT_WC > 0
+  if (e->reg.bounded) (void)budget_reclaim(e, e->reg.budget.max_tables);
+#endif
+}
+
+static int multi_set_validators(ibft_engine* E, uint32_t table_slot, uint64_t height, const uint8_t* addrs, const uint8_t* powers_be,
+                                uint32_t n) {
+  multi_engine* M = E->multi;
+  std::unique_lock<std::shared_mutex> st(M->state_mu);
+  // the lead checks every argument on the host before it touches its device: a refused table leaves every device as it was
+  int rc = ibft_set_validators(M->subs[0], table_slot, height, addrs, powers_be, n);
+  if (rc != IBFT_OK) return rc;
+  for (size_t k = 1; k < M->subs.size(); k++) {
+    rc = ibft_set_validators(M->subs[k], table_slot, height, addrs, powers_be, n);
+    if (rc == IBFT_OK) continue;
+    const std::string err = tl_err;
+    const multi_table& old = M->tables[table_slot];
+    for (size_t j = 0; j < k; j++) {  // the devices that took the new table get the slot's previous content back
+      if (old.valid) (void)ibft_set_validators(M->subs[j], table_slot, old.height, old.addrs.data(), old.powers.empty() ? nullptr : old.powers.data(), old.n);
+      else slot_clear(M->subs[j], table_slot);
+    }
+    set_err("device %zu: %s", k, err.c_str());
+    return rc;
+  }
+  multi_table& t = M->tables[table_slot];
+  t.valid = true;
+  t.height = height;
+  t.n = n;
+  t.addrs.assign(addrs, addrs + (size_t)n * 20);
+  if (powers_be) t.powers.assign(powers_be, powers_be + (size_t)n * 32);
+  else t.powers.clear();
+  return IBFT_OK;
+}
+
+// per (slot, validator): whether device e knows the validator's key
+static int known_members(ibft_engine* e, std::vector<std::vector<uint8_t>>& known) {
+  known.resize(e->slots.size());
+#if IBFT_WC > 0
+  if (!(e->p.flags & IBFT_FLAG_KEY_CACHE) || !e->reg.d_state) return IBFT_OK;
+  all_lanes_lock lk(e);
+  const key_registry& R = e->reg;
+  CU(cudaSetDevice(e->p.device));
+  CU(cudaDeviceSynchronize());
+  std::vector<uint32_t> state(R.used);
+  if (R.used) CU(cudaMemcpy(state.data(), R.d_state, (size_t)R.used * 4, cudaMemcpyDeviceToHost));
+  for (size_t s = 0; s < e->slots.size(); s++) {
+    const slot_host& sh = e->slots[s];
+    if (!sh.valid) continue;
+    known[s].resize(sh.key_ref.size());
+    for (size_t v = 0; v < sh.key_ref.size(); v++) known[s][v] |= state[sh.key_ref[v]] != IBFT_KEY_UNKNOWN;
+  }
+#endif
+  return IBFT_OK;
+}
+
+static int multi_refresh_key_tables(ibft_engine* E, uint32_t* n_keys_out) {
+  multi_engine* M = E->multi;
+  std::unique_lock<std::shared_mutex> st(M->state_mu);
+  for (ibft_engine* s : M->subs) {
+    int rc = ibft_refresh_key_tables(s, nullptr);
+    if (rc != IBFT_OK) return rc;
+  }
+  if (!n_keys_out) return IBFT_OK;
+  // the tables are the same on every device: a member counts once when any device knows its key
+  std::vector<std::vector<uint8_t>> known;
+  for (ibft_engine* s : M->subs) {
+    int rc = known_members(s, known);
+    if (rc != IBFT_OK) return rc;
+  }
+  uint32_t total = 0;
+  for (const auto& row : known)
+    for (uint8_t b : row) total += b;
+  *n_keys_out = total;
+  return IBFT_OK;
+}
+
+static int multi_set_key_table_budget(ibft_engine* E, uint32_t max_tables) {
+  multi_engine* M = E->multi;
+  std::unique_lock<std::shared_mutex> st(M->state_mu);
+  for (ibft_engine* s : M->subs) {
+    int rc = ibft_set_key_table_budget(s, max_tables);
+    if (rc != IBFT_OK) return rc;
+  }
+  return IBFT_OK;
+}
+
+static int multi_set_recover_path(ibft_engine* E, int path) {
+  for (ibft_engine* s : E->multi->subs) s->recover_path.store(path);
+  return IBFT_OK;
+}
+
+static uint64_t multi_launch_count(ibft_engine* E) {
+  uint64_t total = 0;
+  for (ibft_engine* s : E->multi->subs) total += s->launches.load();
+  return total;
+}
+
+static void multi_destroy(ibft_engine* E) {
+  multi_engine* M = E->multi;
+  if (!M->subs.empty()) {
+    cudaSetDevice(M->subs[0]->p.device);
+    cudaDeviceSynchronize();
+    for (int k = 0; k < IBFT_LANES; k++) {
+      cudaFree(M->d_parts[k]);
+      if (M->merged[k]) cudaEventDestroy(M->merged[k]);
+    }
+  }
+  for (ibft_engine* s : M->subs) engine_free(s);
+  for (ibft_engine* v : M->views) delete v;
+  delete M;
+  delete E;
+}
+
+extern "C" int ibft_engine_create_multi(const ibft_engine_params* params, const int32_t* devices, uint32_t n_devices, ibft_engine** out) {
+  if (!params || !out || (n_devices && !devices)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  *out = nullptr;
+  if (n_devices == 0 || n_devices > 8) { set_err("a multi-device engine takes 1 to 8 devices, not %u", n_devices); return IBFT_ERR_INVALID_ARG; }
+  ibft_engine_params p = *params;
+  p.device = devices[0];
+  if (n_devices == 1) return ibft_engine_create(&p, out);
+  ibft_engine* E = new ibft_engine();
+  E->multi = new multi_engine();
+  multi_engine* M = E->multi;
+  for (uint32_t k = 0; k < n_devices; k++) {
+    p.device = devices[k];
+    ibft_engine* s = nullptr;
+    int rc = ibft_engine_create(&p, &s);
+    if (rc != IBFT_OK) {
+      const std::string err = tl_err;
+      multi_destroy(E);
+      set_err("device %u (ordinal %d): %s", k, (int)devices[k], err.c_str());
+      return rc;
+    }
+    M->subs.push_back(s);
+    ibft_engine* v = new ibft_engine();
+    v->view_of = s;
+    v->p = s->p;
+    M->views.push_back(v);
+  }
+  ibft_engine* lead = M->subs[0];
+  E->p = lead->p;
+  M->tables.resize(E->p.max_table_slots);
+  cudaError_t ce = cudaSetDevice(lead->p.device);
+  const size_t part_words = lead->lanes[0].voted_words_cap + E->p.max_groups;
+  for (int k = 0; k < IBFT_LANES && ce == cudaSuccess; k++) {
+    ce = cudaMalloc(&M->d_parts[k], (size_t)n_devices * part_words * 4);
+    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&M->merged[k], cudaEventDisableTiming);
+  }
+  if (ce != cudaSuccess) {
+    set_err("merge buffers on the lead device: %s", cudaGetErrorString(ce));
+    multi_destroy(E);
+    return IBFT_ERR_CUDA;
+  }
+  *out = E;
+  return IBFT_OK;
+}
+
+extern "C" int ibft_engine_device_count(ibft_engine* e, uint32_t* n_out) {
+  if (!e || !n_out) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  *n_out = e->multi ? (uint32_t)e->multi->subs.size() : 1u;
+  return IBFT_OK;
+}
+
+extern "C" int ibft_engine_sub(ibft_engine* e, uint32_t k, ibft_engine** sub_out) {
+  if (!e || !sub_out) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  const uint32_t n = e->multi ? (uint32_t)e->multi->subs.size() : 1u;
+  if (k >= n) { set_err("device %u of an engine over %u", k, n); return IBFT_ERR_INVALID_ARG; }
+  *sub_out = e->multi ? e->multi->views[k] : e;  // a single-device engine is its own only device engine
+  return IBFT_OK;
 }

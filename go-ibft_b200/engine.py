@@ -40,6 +40,7 @@ EXPORTS = [
     "ibft_exchange_alloc", "ibft_exchange_open", "ibft_exchange_close", "ibft_exchange_free", "ibft_exchange_clear",
     "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_sign_batch_rfc6979", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_set_key_table_budget", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
     "ibft_debug_wtable", "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
+    "ibft_engine_create_multi", "ibft_engine_device_count", "ibft_engine_sub",
 ]
 
 
@@ -80,6 +81,9 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.ibft_engine_launch_count.restype = c_uint64
     lib.ibft_engine_launch_count.argtypes = [c_void_p]
     lib.ibft_engine_create.argtypes = [POINTER(EngineParams), POINTER(c_void_p)]
+    lib.ibft_engine_create_multi.argtypes = [POINTER(EngineParams), c_void_p, c_uint32, POINTER(c_void_p)]
+    lib.ibft_engine_device_count.argtypes = [c_void_p, POINTER(c_uint32)]
+    lib.ibft_engine_sub.argtypes = [c_void_p, c_uint32, POINTER(c_void_p)]
     lib.ibft_engine_destroy.argtypes = [c_void_p]
     lib.ibft_engine_destroy.restype = None
     lib.ibft_engine_device_info.argtypes = [c_void_p, POINTER(DeviceInfo)]
@@ -144,18 +148,25 @@ def group_descs(n_groups: int, slot=0, rule=QUORUM_DEFAULT, proposer=0, slot_hei
 
 
 class Engine:
-    """One engine per process per GPU (one process per GPU is the deployment model)."""
+    """One engine on one GPU, or with `devices` one engine over several (ibft_engine_create_multi): host-buffer calls are then
+    sharded over the devices and their quorum merged on the first.  Across processes or nodes use sharding.ShardedVerifier."""
 
     def __init__(self, device: int = 0, max_items: int = 1 << 16, max_payload_bytes: int = 1 << 24, max_groups: int = 64,
                  max_table_slots: int = 16, max_validators: int = 16384, key_cache: bool = False,
-                 key_table_budget: int | None = None):
+                 key_table_budget: int | None = None, devices: list[int] | None = None):
         """key_cache: IBFT_FLAG_KEY_CACHE -- verify (instead of recover) signatures of validators whose key is already known.
-        key_table_budget: with key_cache, hold at most this many comb tables (136 KiB each; set_key_table_budget)."""
+        key_table_budget: with key_cache, hold at most this many comb tables (136 KiB each; set_key_table_budget).
+        devices: CUDA ordinals of a multi-device engine (1..8, may repeat); `device` is then ignored."""
         self.lib = load_library()
         self.params = EngineParams(device, max_items, max_payload_bytes, max_groups, max_table_slots, max_validators, 1 if key_cache else 0)
         self.handle = c_void_p()
         self.slot_height: dict[int, int] = {}  # slot -> height of the resident validator table (mirrors the engine's own record)
-        rc = self.lib.ibft_engine_create(ctypes.byref(self.params), ctypes.byref(self.handle))
+        self._owned = True
+        if devices is not None:
+            devs = (c_int32 * max(1, len(devices)))(*[int(d) for d in devices])
+            rc = self.lib.ibft_engine_create_multi(ctypes.byref(self.params), devs, len(devices), ctypes.byref(self.handle))
+        else:
+            rc = self.lib.ibft_engine_create(ctypes.byref(self.params), ctypes.byref(self.handle))
         if rc != IBFT_OK:
             self.handle = None
             raise EngineError(rc, self.lib.ibft_last_error().decode())
@@ -168,8 +179,24 @@ class Engine:
 
     def close(self):
         if getattr(self, "handle", None):
-            self.lib.ibft_engine_destroy(self.handle)
+            if getattr(self, "_owned", True):
+                self.lib.ibft_engine_destroy(self.handle)
             self.handle = None
+
+    def device_count(self) -> int:
+        n = c_uint32()
+        self._check(self.lib.ibft_engine_device_count(self.handle, ctypes.byref(n)))
+        return int(n.value)
+
+    def sub(self, k: int) -> "Engine":
+        """Borrowed diagnostics handle of the k-th device's engine (ibft_engine_sub): device info, get_quorum, debug reads and the
+        launch count; every call that changes state or verifies raises.  Valid while this engine is open."""
+        h = c_void_p()
+        self._check(self.lib.ibft_engine_sub(self.handle, int(k), ctypes.byref(h)))
+        s = Engine.__new__(Engine)
+        s.lib, s.params, s.handle, s._owned, s._parent = self.lib, self.params, h, False, self
+        s.slot_height = dict(self.slot_height)
+        return s
 
     def __del__(self):
         try:

@@ -44,6 +44,8 @@ def load_host() -> ctypes.CDLL:
         lib = ctypes.CDLL(build_host())
         lib.ibfthost_create.restype = c_void_p
         lib.ibfthost_create.argtypes = [c_int, POINTER(Callbacks), c_char_p, c_size_t, POINTER(EngineParams)]
+        lib.ibfthost_create_multi.restype = c_void_p
+        lib.ibfthost_create_multi.argtypes = [POINTER(Callbacks), c_char_p, c_size_t, POINTER(EngineParams), c_void_p, c_uint32]
         lib.ibfthost_destroy.argtypes = [c_void_p]
         lib.ibfthost_destroy.restype = None
         lib.ibfthost_set_validators.argtypes = [c_void_p, c_uint64, c_char_p, POINTER(c_uint32), c_char_p, c_uint32]
@@ -121,9 +123,11 @@ class HostContext:
     """kind="callback": fns = dict of Python closures taking decoded arguments:
          is_valid_proposal(raw) / is_valid_validator(wire) / is_proposer(id, h, r) / is_valid_proposal_hash(proposal_wire|None, hash|None)
          / is_valid_committed_seal(hash|None, (signer, sig)|None)
-       kind="gpu": is_proposer / is_valid_proposal closures only; signature work goes to the device."""
+       kind="gpu": is_proposer / is_valid_proposal closures only; signature work goes to the device -- to the devices listed in
+       `devices` (one engine over all of them, ibft_engine_create_multi) when given."""
 
-    def __init__(self, kind: str = "callback", fns: dict | None = None, node_id: bytes = b"", gpu_params: EngineParams | None = None):
+    def __init__(self, kind: str = "callback", fns: dict | None = None, node_id: bytes = b"", gpu_params: EngineParams | None = None,
+                 devices: list[int] | None = None):
         self.lib = load_host()
         fns = fns or {}
         self._keep = []
@@ -145,8 +149,14 @@ class HostContext:
         if "is_valid_committed_seal" in fns:
             cbs.is_valid_committed_seal = wrap(CB_SEAL, lambda h, hn, hh, s, sn, g, gn, hs: int(bool(
                 fns["is_valid_committed_seal"](_bytes(h, hn) if hh else None, (_bytes(s, sn), _bytes(g, gn)) if hs else None))))
-        self.ctx = self.lib.ibfthost_create(0 if kind == "callback" else 1, ctypes.byref(cbs), node_id, len(node_id),
-                                            ctypes.byref(gpu_params) if gpu_params is not None else None)
+        if devices:
+            if kind != "gpu" or gpu_params is None:
+                raise ValueError("devices needs kind='gpu' and gpu_params")
+            devs = (ctypes.c_int32 * len(devices))(*[int(d) for d in devices])
+            self.ctx = self.lib.ibfthost_create_multi(ctypes.byref(cbs), node_id, len(node_id), ctypes.byref(gpu_params), devs, len(devices))
+        else:
+            self.ctx = self.lib.ibfthost_create(0 if kind == "callback" else 1, ctypes.byref(cbs), node_id, len(node_id),
+                                                ctypes.byref(gpu_params) if gpu_params is not None else None)
         if not self.ctx:
             raise RuntimeError("ibfthost_create failed (a GPU verifier needs a CUDA device: there is no CPU fallback)")
 

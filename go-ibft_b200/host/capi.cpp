@@ -42,8 +42,8 @@ struct ibfthost_ctx {
 
 static Bytes B(const uint8_t* p, size_t n) { return p ? Bytes((const char*)p, n) : Bytes(); }
 
-ibfthost_ctx* ibfthost_create(int kind, const ibfthost_callbacks* cbs, const uint8_t* id, size_t id_len,
-                              const ibft_engine_params* gpu_params) {
+static ibfthost_ctx* create_ctx(int kind, const ibfthost_callbacks* cbs, const uint8_t* id, size_t id_len,
+                                const ibft_engine_params* gpu_params, const std::vector<int32_t>& devices) {
   auto* c = new ibfthost_ctx();
   if (kind == 0) {
     auto v = std::make_unique<CallbackVerifier>();
@@ -73,7 +73,7 @@ ibfthost_ctx* ibfthost_create(int kind, const ibfthost_callbacks* cbs, const uin
     c->verifier = std::move(v);
   } else {
     if (!gpu_params) { delete c; return nullptr; }
-    auto v = std::make_unique<GpuVerifier>(*gpu_params);
+    auto v = std::make_unique<GpuVerifier>(*gpu_params, devices);
     if (!v->ok()) { delete c; return nullptr; }  // no CPU fallback: no engine, no context
     v->id = B(id, id_len);
     if (cbs && cbs->is_proposer) {
@@ -94,6 +94,16 @@ ibfthost_ctx* ibfthost_create(int kind, const ibfthost_callbacks* cbs, const uin
     c->signals.push_back(r);
   };
   return c;
+}
+ibfthost_ctx* ibfthost_create(int kind, const ibfthost_callbacks* cbs, const uint8_t* id, size_t id_len,
+                              const ibft_engine_params* gpu_params) {
+  return create_ctx(kind, cbs, id, id_len, gpu_params, {});
+}
+// a GPU verifier over several devices (ibft_engine_create_multi)
+ibfthost_ctx* ibfthost_create_multi(const ibfthost_callbacks* cbs, const uint8_t* id, size_t id_len, const ibft_engine_params* gpu_params,
+                                    const int32_t* devices, uint32_t n_devices) {
+  if (!devices || n_devices == 0) return nullptr;
+  return create_ctx(1, cbs, id, id_len, gpu_params, std::vector<int32_t>(devices, devices + n_devices));
 }
 void ibfthost_destroy(ibfthost_ctx* c) { delete c; }
 

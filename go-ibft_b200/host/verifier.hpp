@@ -85,9 +85,13 @@ class GpuVerifier : public Verifier {
   uint32_t ingress_second_min = 32;  // queue length from which a SECOND flush goes up while one is still on the device
 
   // key_table_budget >= 0 (with IBFT_FLAG_KEY_CACHE): hold at most that many comb tables (ibft_set_key_table_budget)
-  explicit GpuVerifier(const ibft_engine_params& params, int64_t key_table_budget = -1) {
+  explicit GpuVerifier(const ibft_engine_params& params, int64_t key_table_budget = -1) : GpuVerifier(params, {}, key_table_budget) {}
+  // devices non-empty: one engine over those CUDA devices (ibft_engine_create_multi; params.device is ignored) -- every
+  // host-buffer call is sharded over them and its quorum merged on the first
+  GpuVerifier(const ibft_engine_params& params, const std::vector<int32_t>& devices, int64_t key_table_budget = -1) {
     params_ = params;
-    int rc = ibft_engine_create(&params_, &engine_);
+    int rc = devices.empty() ? ibft_engine_create(&params_, &engine_)
+                             : ibft_engine_create_multi(&params_, devices.data(), (uint32_t)devices.size(), &engine_);
     if (rc == IBFT_OK && key_table_budget >= 0) {
       rc = ibft_set_key_table_budget(engine_, (uint32_t)std::min<int64_t>(key_table_budget, UINT32_MAX));
       if (rc != IBFT_OK) {

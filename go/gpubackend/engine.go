@@ -46,6 +46,10 @@ type Params struct {
 	// KeyTableBudget, when non-nil (with KeyCache), bounds the comb tables to that many (ibft_set_key_table_budget): the keys
 	// used most recently keep theirs, the others are verified by recovery, and SetValidators never fails for table memory.
 	KeyTableBudget *uint32
+	// Devices, when it has more than one entry, makes one engine over those CUDA ordinals (ibft_engine_create_multi; Device is
+	// then ignored, and an ordinal may repeat): every host-buffer call is sharded over them and its quorum merged on the first,
+	// with the same results as one device.  NCCL is only needed across processes or nodes.
+	Devices []int
 }
 
 func lastError() error { return errors.New(C.GoString(C.ibft_last_error())) }
@@ -59,8 +63,21 @@ func NewEngine(p Params) (*Engine, error) {
 	if p.KeyCache {
 		e.params.flags = C.IBFT_FLAG_KEY_CACHE
 	}
-	if rc := C.ibft_engine_create(&e.params, &e.h); rc != C.IBFT_OK {
-		return nil, fmt.Errorf("ibft_engine_create: %w", lastError())
+	if len(p.Devices) > 1 {
+		devs := make([]C.int32_t, len(p.Devices))
+		for i, d := range p.Devices {
+			devs[i] = C.int32_t(d)
+		}
+		if rc := C.ibft_engine_create_multi(&e.params, &devs[0], C.uint32_t(len(devs)), &e.h); rc != C.IBFT_OK {
+			return nil, fmt.Errorf("ibft_engine_create_multi: %w", lastError())
+		}
+	} else {
+		if len(p.Devices) == 1 {
+			e.params.device = C.int32_t(p.Devices[0])
+		}
+		if rc := C.ibft_engine_create(&e.params, &e.h); rc != C.IBFT_OK {
+			return nil, fmt.Errorf("ibft_engine_create: %w", lastError())
+		}
 	}
 	if p.KeyTableBudget != nil {
 		if rc := C.ibft_set_key_table_budget(e.h, C.uint32_t(*p.KeyTableBudget)); rc != C.IBFT_OK {

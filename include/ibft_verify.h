@@ -179,6 +179,50 @@ int ibft_engine_create(const ibft_engine_params* params, ibft_engine** out);
 void ibft_engine_destroy(ibft_engine* e);
 int ibft_engine_device_info(ibft_engine* e, ibft_device_info* out);
 
+/* multi-device engines ---------------------------------------------------------------------------- */
+/* One engine over n_devices CUDA devices (1..8; an ordinal may repeat).  params->device is ignored; every device gets the other
+ * parameters.  All or nothing: if any device cannot be used, nothing stays allocated and the call returns that device's status
+ * (IBFT_ERR_NO_DEVICE, IBFT_ERR_CUDA, or IBFT_ERR_INVALID_ARG for an ordinal that does not exist).  n_devices == 1 is
+ * ibft_engine_create on that device.  The engine holds one ordinary engine per listed device (its sub-engines; the first is the
+ * lead); the wide generator comb is shared per process and device, so a repeated ordinal does not hold a second copy.
+ *
+ *   ibft_set_validators            replicated on every device.  The arguments are checked on the host before any device is
+ *                                  touched (IBFT_ERR_VOTING_POWER included).  If a device fails after others took the new table,
+ *                                  those get the slot's previous table back (or the slot unset), so the slot answers as before.
+ *   ibft_get_quorum                the lead answers.
+ *   ibft_verify_batch, _ex,        split into contiguous shards whose boundaries are multiples of 32 over
+ *   _submit / _poll / _wait        min(n_devices, ceil(n / 1,024)) devices.  Each shard gets its own payload arena: the union of
+ *                                  the byte ranges its items reference, each byte once, never longer than the call's arena.  Every
+ *                                  device verifies its shard (its kernel chosen for the shard's size) and records its votes; the
+ *                                  lead gathers the voted sets and valid counts with peer copies, merges them and decides each
+ *                                  group's quorum rule.  The caller's buffers are written only after every device has succeeded;
+ *                                  any failure returns its status with every output untouched.  A call takes the small lane of
+ *                                  every device when the whole call fits it, else the bulk lane, locked in device-list order.
+ *                                  The results are byte for byte those of a single-device engine.
+ *   ibft_last_item_status,         the most recent completed call: statuses assembled from the shards, the merged voted sets,
+ *   ibft_get_voted_bitmap,         handed-back summed over the devices that call used.
+ *   ibft_debug_known_handed_back
+ *   ibft_keccak256_batch,          rows split the same way; the output bytes are a single-device call's.
+ *   ibft_proposal_hash_batch,
+ *   ibft_sign_batch, _rfc6979
+ *   ibft_refresh_key_tables,       applied to every device (a budget bounds each device's pool).  Key registries stay per device:
+ *   ibft_set_key_table_budget,     each learns from the signatures of its shards, with identical verdicts either way.
+ *   ibft_set_recover_path          *n_keys_out counts (table, member) pairs whose key is known on at least one device.
+ *   ibft_engine_launch_count       the sum over the devices.
+ *   ibft_engine_device_info,       the lead answers; ibft_engine_sub reaches the others.
+ *   ibft_probe_int_peak, ibft_debug_*
+ *   ibft_bind_groups, ibft_verify_batch_device, ibft_quorum_*_device, ibft_exchange_*
+ *                                  IBFT_ERR_INVALID_ARG: they take device pointers of one device.  Across processes or nodes, or
+ *                                  with device-resident buffers, use one engine per device (go-ibft_b200/sharding.py). */
+int ibft_engine_create_multi(const ibft_engine_params* params, const int32_t* devices, uint32_t n_devices, ibft_engine** out);
+/* Number of devices of an engine (1 for ibft_engine_create). */
+int ibft_engine_device_count(ibft_engine* e, uint32_t* n_out);
+/* Borrowed handle of the k-th device's engine, for diagnostics only: ibft_engine_device_info, ibft_get_quorum, ibft_debug_*,
+ * ibft_probe_int_peak, ibft_engine_launch_count, ibft_last_item_status and ibft_get_voted_bitmap of that device's last shard.
+ * Every call that changes state, verifies, hashes or signs returns IBFT_ERR_INVALID_ARG on it, and ibft_engine_destroy ignores
+ * it.  It stays valid until the parent is destroyed.  On a single-device engine, k = 0 gives the engine itself. */
+int ibft_engine_sub(ibft_engine* e, uint32_t k, ibft_engine** sub_out);
+
 /* validator tables --------------------------------------------------------------------------------- */
 /* Replaces ValidatorManager.Init -> Backend.GetVotingPowers(height) (core/validator_manager.go:50-74,
  * core/backend.go via ValidatorBackend :17-20).  addrs: n x 20 bytes in validator-index order;
