@@ -1239,6 +1239,47 @@ k_quorum_reduce(const ibft_group_desc* __restrict__ groups, const group_dev* __r
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// Reject reasons (ibft_explain_batch): the rejected items only, compacted on the host, one thread each in one-warp CTAs, each
+// decided again step by step by explain_item (verify_core.cuh) with the one-thread recovery of k_recover and its membership test.
+// A cold path kept apart from the verify kernels, whose register budget and hot loop it leaves alone.  WIDE: u1*G from the wide
+// comb, as in k_recover.  Dynamic shared memory: the per-signature R tables, 32 x IBFT_RTAB_WORDS words.
+// ------------------------------------------------------------------------------------------------------------
+template <bool WIDE>
+__global__ void __launch_bounds__(32)
+k_explain(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __restrict__ arena, size_t arena_len,
+          const ibft_group_desc* __restrict__ groups, uint32_t n_groups, const slot_dev* __restrict__ slots, uint32_t n_slots,
+          const uint32_t* __restrict__ ctable, const uint32_t* __restrict__ wtable, uint8_t* __restrict__ reasons,
+          uint8_t* __restrict__ recovered) {
+  extern __shared__ uint32_t s_rtab[];
+  const uint32_t i = blockIdx.x * 32 + threadIdx.x;
+  if (i >= n) return;
+  ibft_sig_item it;
+  const uint4* src = reinterpret_cast<const uint4*>(items + i);
+  uint4* w = reinterpret_cast<uint4*>(&it);
+#pragma unroll
+  for (int k = 0; k < 8; k++) w[k] = __ldg(src + k);
+  gtab_view G{g_gtable};
+  G.comb = ctable;
+  G.wide = WIDE ? wtable : nullptr;
+  rtab_view T{s_rtab + threadIdx.x, 32u};
+  auto member = [&](uint32_t group, const uint8_t* signer) {
+    int v;
+    uint32_t slot;
+    return group_member(groups, n_groups, slots, n_slots, group, signer, &v, &slot);
+  };
+  uint8_t addr[20];
+  uint8_t why;
+#if IBFT_GEN_WIDE > 0
+  if (WIDE) why = explain_item(exec_serial_wide{}, it, arena, arena_len, groups != nullptr, n_groups, G, T, member, addr);
+  else
+#endif
+    why = explain_item(exec_serial{}, it, arena, arena_len, groups != nullptr, n_groups, G, T, member, addr);
+  reasons[i] = why;
+#pragma unroll
+  for (int k = 0; k < 20; k++) recovered[(size_t)i * 20 + k] = addr[k];
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // hash-only batch (IsValidProposalHash)
 // ------------------------------------------------------------------------------------------------------------
 __global__ void k_keccak_batch(const uint8_t* __restrict__ arena, size_t arena_len, const uint32_t* __restrict__ offs,
@@ -1790,6 +1831,9 @@ static int multi_submit(ibft_engine* e, const ibft_sig_item* items, uint32_t n, 
 static int multi_poll(ibft_engine* e, int* done);
 static int multi_wait(ibft_engine* e);
 static int multi_last_item_status(ibft_engine* e, uint8_t* status_out, uint32_t n);
+static int multi_explain(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                         const ibft_group_desc* groups, uint32_t n_groups, const uint32_t* bitmap, uint8_t* reasons_out,
+                         uint8_t* recovered_out);
 static int multi_known_handed_back(ibft_engine* e, uint32_t* n_out);
 static int multi_hash(ibft_engine* e, const uint8_t* arena, size_t arena_len, const uint32_t* offsets, const uint32_t* lens,
                       const uint64_t* rounds, uint32_t n, uint8_t* out32);
@@ -3127,6 +3171,82 @@ extern "C" int ibft_last_item_status(ibft_engine* e, uint8_t* status_out, uint32
   return IBFT_OK;
 }
 
+// ibft_explain_batch on one device's engine
+static int explain_batch(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                         const ibft_group_desc* groups, uint32_t n_groups, const uint32_t* bitmap, uint8_t* reasons_out,
+                         uint8_t* recovered_out) {
+  if (n > e->p.max_items || arena_len > e->p.max_payload_bytes || n_groups > e->p.max_groups) {
+    set_err("batch (%u items, %zu payload bytes, %u groups) exceeds engine capacity (%u, %u, %u)", n, arena_len, n_groups, e->p.max_items,
+            e->p.max_payload_bytes, e->p.max_groups);
+    return IBFT_ERR_CAPACITY;
+  }
+  std::vector<uint32_t> idx;  // the items to explain: those whose verdict bit is 0
+  for (uint32_t i = 0; i < n; i++)
+    if (bitmap == nullptr || !((bitmap[i >> 5] >> (i & 31u)) & 1u)) idx.push_back(i);
+  const uint32_t m = (uint32_t)idx.size();
+  lane* L = acquire_lane(e, m, arena_len);
+  std::lock_guard<std::mutex> lk(L->mu, std::adopt_lock);
+  if (L->pending.active) { set_err("a submitted call is still pending; wait for it first"); return IBFT_ERR_INVALID_ARG; }
+  if (n_groups) {  // the verify calls' checks of slots, heights and quorum rules
+    std::vector<group_dev> gdev(n_groups);
+    size_t voted_words = 0;
+    int rc = plan_groups(e, L, groups, n_groups, gdev.data(), &voted_words);
+    if (rc != IBFT_OK) return rc;
+  }
+  std::vector<uint8_t> why(m);
+  std::vector<uint8_t> rec(recovered_out ? (size_t)m * 20 : 0);
+  if (m) {
+    CU(cudaSetDevice(e->p.device));
+    cudaStream_t st = L->stream;
+    for (uint32_t k = 0; k < m; k++) L->h_items[k] = items[idx[k]];
+    if (arena_len) {
+      memcpy(L->h_arena, arena, arena_len);
+      CU(cudaMemcpyAsync(L->d_arena, L->h_arena, arena_len, cudaMemcpyHostToDevice, st));
+    }
+    // The groups go through the lane's quorum-result buffer (56 bytes per group, no longer needed once a call has returned):
+    // d_groups of lane 0 holds the groups bound for the device-resident calls, which this call must not replace.
+    ibft_group_desc* d_groups = reinterpret_cast<ibft_group_desc*>(L->d_results);
+    if (n_groups) {
+      memcpy(L->h_groups, groups, (size_t)n_groups * sizeof(ibft_group_desc));
+      CU(cudaMemcpyAsync(d_groups, L->h_groups, (size_t)n_groups * sizeof(ibft_group_desc), cudaMemcpyHostToDevice, st));
+    }
+    CU(cudaMemcpyAsync(L->d_items, L->h_items, (size_t)m * sizeof(ibft_sig_item), cudaMemcpyHostToDevice, st));
+    auto kernel = e->d_wtable != nullptr ? k_explain<true> : k_explain<false>;
+    kernel<<<(m + 31) / 32, 32, 32 * IBFT_RTAB_WORDS * 4, st>>>(L->d_items, m, L->d_arena, arena_len, n_groups ? d_groups : nullptr, n_groups,
+                                                                e->d_slots, e->p.max_table_slots, e->d_ctable, e->d_wtable, L->d_status,
+                                                                L->d_recovered);
+    e->launches++;
+    CU(cudaGetLastError());
+    // the answers land in the pinned tuple staging, which the upload above (same stream) has finished with
+    uint8_t* h_out = reinterpret_cast<uint8_t*>(L->h_items);
+    CU(cudaMemcpyAsync(h_out, L->d_status, m, cudaMemcpyDeviceToHost, st));
+    if (recovered_out) CU(cudaMemcpyAsync(h_out + m, L->d_recovered, (size_t)m * 20, cudaMemcpyDeviceToHost, st));
+    cudaError_t ce = cudaStreamSynchronize(st);
+    if (ce != cudaSuccess) {
+      set_err("device execution failed: %s", cudaGetErrorString(ce));
+      return IBFT_ERR_CUDA;
+    }
+    memcpy(why.data(), h_out, m);
+    if (recovered_out) memcpy(rec.data(), h_out + m, (size_t)m * 20);
+  }
+  if (n) memset(reasons_out, IBFT_REASON_OK, n);
+  if (recovered_out && n) memset(recovered_out, 0, (size_t)n * 20);
+  for (uint32_t k = 0; k < m; k++) {
+    reasons_out[idx[k]] = bitmap != nullptr && why[k] == IBFT_REASON_OK ? (uint8_t)IBFT_REASON_INCONSISTENT : why[k];
+    if (recovered_out) memcpy(recovered_out + (size_t)idx[k] * 20, rec.data() + (size_t)k * 20, 20);
+  }
+  return IBFT_OK;
+}
+
+extern "C" int ibft_explain_batch(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                                  const ibft_group_desc* groups, uint32_t n_groups, const uint32_t* bitmap, uint8_t* reasons_out,
+                                  uint8_t* recovered_out) {
+  if (!e || (n && (!items || !reasons_out)) || (arena_len && !arena) || (n_groups && !groups)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (e->multi) return multi_explain(e, items, n, arena, arena_len, groups, n_groups, bitmap, reasons_out, recovered_out);
+  return explain_batch(e, items, n, arena, arena_len, groups, n_groups, bitmap, reasons_out, recovered_out);
+}
+
 // The asynchronous API lives on lane 0 (one call pending at a time, as before); synchronous calls that fit the small lane keep
 // working while it is pending.
 extern "C" int ibft_verify_submit(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
@@ -3849,6 +3969,15 @@ static int multi_verify(ibft_engine* E, const ibft_sig_item* items, uint32_t n, 
   int rc = multi_submit_locked(E, kind, used, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, mc);
   if (rc != IBFT_OK) return rc;
   return multi_wait_locked(E, kind, mc, status_out, voted_out, voted_stride_words);
+}
+
+// the lead explains: every device holds the same tables, and the items to explain are few
+static int multi_explain(ibft_engine* E, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                         const ibft_group_desc* groups, uint32_t n_groups, const uint32_t* bitmap, uint8_t* reasons_out,
+                         uint8_t* recovered_out) {
+  multi_engine* M = E->multi;
+  std::shared_lock<std::shared_mutex> st(M->state_mu);
+  return explain_batch(M->subs[0], items, n, arena, arena_len, groups, n_groups, bitmap, reasons_out, recovered_out);
 }
 
 static int multi_submit(ibft_engine* E, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,

@@ -524,6 +524,39 @@ IBFT_HD bool ecrecover_address(const uint8_t* r_be, const uint8_t* s_be, uint8_t
   return ecrecover_address_x(exec_serial{}, r_be, s_be, v, z_be, G, T, addr20, key_out);
 }
 
+// Why one item is rejected (ibft_explain_batch): the recover path's decision, step by step, as an IBFT_REASON_* code.  The steps
+// run in the order the verify kernels decide, so the first failing one is the reason.  member(group, signer) is the validator-set
+// test of the kernels (true for a group without a table).  grouped: the call has groups (without, no item is ever of an unknown
+// group, as in the verify calls).  addr20 = the recovered address when recovery succeeded, else zero.
+template <class EX, class MEMBER>
+IBFT_HD uint8_t explain_item(const EX& ex, const ibft_sig_item& it, const uint8_t* arena, size_t arena_len, bool grouped,
+                             uint32_t n_groups, const gtab_view& G, const rtab_view& T, const MEMBER& member, uint8_t* addr20) {
+#pragma unroll
+  for (int i = 0; i < 20; i++) addr20[i] = 0;
+  if (grouped && it.group >= n_groups) return IBFT_REASON_NO_GROUP;
+  resolved_item ri;
+  bool have = false;
+  if (resolve_item(it, arena, arena_len, ri, &have) == IBFT_ITEM_NEEDS_HOST) return IBFT_REASON_NEEDS_HOST;
+  if (!have) return IBFT_REASON_MALFORMED;
+  if (ri.v > 1) return IBFT_REASON_BAD_V;
+  const sc r = sc_from_be(ri.r), s = sc_from_be(ri.s);
+  if (sc_is_zero(r) || sc_ge_n(r)) return IBFT_REASON_R_RANGE;
+  if (sc_is_zero(s) || sc_ge_n(s)) return IBFT_REASON_S_RANGE;
+  // recover_key answers false both for a non-residue and for the point at infinity: tell them apart first
+  fe x;
+#pragma unroll
+  for (int i = 0; i < 8; i++) x.v[i] = r.v[i];
+  const fe c = fe_add(fe_mul(fe_sqr(x), x), fe_from_u32(7));
+  if (!fe_equal(fe_sqr(fe_sqrt_candidate(c)), c)) return IBFT_REASON_R_NOT_X;
+  if (!ecrecover_address_x(ex, ri.r, ri.s, ri.v, ri.z, G, T, addr20)) return IBFT_REASON_NO_KEY;
+  bool same = true;
+#pragma unroll
+  for (int i = 0; i < 20; i++) same = same && addr20[i] == ri.signer[i];
+  if (!same) return IBFT_REASON_SIGNER_MISMATCH;
+  if (!member(it.group, ri.signer)) return IBFT_REASON_NOT_VALIDATOR;
+  return IBFT_REASON_OK;
+}
+
 #if IBFT_WC > 0
 // ------------------------------------------------------------------------------------------------------------
 // Split pipeline of the mid-size latency kernel (k_recover_split): one signature's serial chain is cut between a CHAIN warp

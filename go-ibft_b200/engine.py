@@ -16,6 +16,10 @@ from . import build as _build
 IBFT_OK, ERR_INVALID_ARG, ERR_NO_DEVICE, ERR_CUDA, ERR_CAPACITY, ERR_VOTING_POWER, ERR_NO_TABLE = range(7)
 KIND_DIGEST, KIND_PAYLOAD, KIND_SEAL, KIND_WIRE, KIND_WIRE_SEAL, KIND_PAYLOAD2, KIND_INVALID = 0, 1, 2, 3, 4, 5, 255
 ITEM_OK, ITEM_NEEDS_HOST = 0, 1
+# why an item was rejected (ibft_explain_batch, IBFT_REASON_*): when several apply, the first in this order
+(REASON_OK, REASON_NO_GROUP, REASON_MALFORMED, REASON_NEEDS_HOST, REASON_BAD_V, REASON_R_RANGE, REASON_S_RANGE, REASON_R_NOT_X,
+ REASON_NO_KEY, REASON_SIGNER_MISMATCH, REASON_NOT_VALIDATOR) = range(11)
+REASON_INCONSISTENT = 255
 NO_TABLE = 0xFFFF
 # quorum rule of a group (ibft_group_desc.flags bits 0-1) and the proposer markers of the PREPARE rule (ibft_group_desc.reserved)
 QUORUM_DEFAULT, QUORUM_PREPREPARE, QUORUM_PREPARE = 0, 1, 2
@@ -40,7 +44,7 @@ EXPORTS = [
     "ibft_exchange_alloc", "ibft_exchange_open", "ibft_exchange_close", "ibft_exchange_free", "ibft_exchange_clear",
     "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_sign_batch_rfc6979", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_set_key_table_budget", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
     "ibft_debug_wtable", "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
-    "ibft_engine_create_multi", "ibft_engine_device_count", "ibft_engine_sub",
+    "ibft_engine_create_multi", "ibft_engine_device_count", "ibft_engine_sub", "ibft_explain_batch",
 ]
 
 
@@ -94,6 +98,7 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.ibft_verify_batch_ex.argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_size_t, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_uint32]
     lib.ibft_last_item_status.argtypes = [c_void_p, c_void_p, c_uint32]
+    lib.ibft_explain_batch.argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_size_t, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p]
     lib.ibft_verify_poll.argtypes = [c_void_p, POINTER(c_int)]
     lib.ibft_verify_wait.argtypes = [c_void_p]
     lib.ibft_bind_groups.argtypes = [c_void_p, c_void_p, c_uint32]
@@ -305,6 +310,30 @@ class Engine:
         out = np.zeros(n, dtype=np.uint8)
         self._check(self.lib.ibft_last_item_status(self.handle, _ptr(out) if n else None, n))
         return out
+
+    def explain_batch(self, items: np.ndarray, arena: bytes | np.ndarray = b"", groups: np.ndarray | None = None,
+                      bitmap: np.ndarray | None = None):
+        """ibft_explain_batch: (reasons uint8[n], recovered uint8[n, 20]) -- why each item whose bit of `bitmap` (the verdict bitmap of
+        a verify call over the same inputs) is 0 was rejected (REASON_*); items whose bit is 1 get REASON_OK without device work.
+        bitmap None explains every item.  recovered: the recovered address of the items that got as far as recovery, else zero."""
+        items = np.ascontiguousarray(items)
+        assert items.dtype == ITEM_DTYPE
+        n = len(items)
+        arena_np = np.frombuffer(arena, dtype=np.uint8) if isinstance(arena, (bytes, bytearray)) else np.ascontiguousarray(arena, dtype=np.uint8)
+        ng = 0 if groups is None else len(groups)
+        if groups is not None:
+            groups = np.ascontiguousarray(groups)
+            assert groups.dtype == GROUP_DTYPE
+        if bitmap is not None:
+            bitmap = np.ascontiguousarray(bitmap, dtype=np.uint32)
+            if len(bitmap) < (n + 31) // 32:
+                raise ValueError("bitmap needs (n + 31) // 32 words")
+        reasons = np.zeros(max(1, n), dtype=np.uint8)
+        recovered = np.zeros((max(1, n), 20), dtype=np.uint8)
+        self._check(self.lib.ibft_explain_batch(self.handle, _ptr(items) if n else None, n, _ptr(arena_np) if len(arena_np) else None,
+                                                len(arena_np), _ptr(groups) if ng else None, ng, _ptr(bitmap), _ptr(reasons),
+                                                _ptr(recovered)))
+        return reasons[:n], recovered[:n]
 
     def verify_submit(self, items, arena, groups, bitmap, results, recovered=None):
         """Async variant; caller owns (and keeps alive) the output arrays until wait()."""

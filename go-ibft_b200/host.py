@@ -22,6 +22,7 @@ CB_VALID_VALIDATOR = CFUNCTYPE(c_int, POINTER(c_uint8), c_size_t)
 CB_PROPOSER = CFUNCTYPE(c_int, POINTER(c_uint8), c_size_t, c_uint64, c_uint64)
 CB_PROPOSAL_HASH = CFUNCTYPE(c_int, POINTER(c_uint8), c_size_t, c_int, POINTER(c_uint8), c_size_t, c_int)
 CB_SEAL = CFUNCTYPE(c_int, POINTER(c_uint8), c_size_t, c_int, POINTER(c_uint8), c_size_t, POINTER(c_uint8), c_size_t, c_int)
+CB_REJECT = CFUNCTYPE(None, c_void_p, c_uint8, c_uint64, POINTER(c_uint8), c_size_t, POINTER(c_uint8), c_size_t, c_uint8, POINTER(c_uint8))
 
 
 class Callbacks(ctypes.Structure):
@@ -58,6 +59,12 @@ def load_host() -> ctypes.CDLL:
         lib.ibfthost_set_wire_frames.restype = None
         lib.ibfthost_gpu_frames_handed_back.argtypes = [c_void_p]
         lib.ibfthost_gpu_frames_handed_back.restype = c_uint64
+        lib.ibfthost_set_reject_hook.argtypes = [c_void_p, CB_REJECT, c_void_p]
+        lib.ibfthost_set_reject_hook.restype = None
+        lib.ibfthost_gpu_rejects.argtypes = [c_void_p, c_uint32]
+        lib.ibfthost_gpu_rejects.restype = c_uint64
+        lib.ibfthost_gpu_explain_calls.argtypes = [c_void_p]
+        lib.ibfthost_gpu_explain_calls.restype = c_uint64
         lib.ibfthost_set_state.argtypes = [c_void_p, c_uint64, c_uint64, c_int, c_char_p, c_size_t]
         lib.ibfthost_get_state_name.argtypes = [c_void_p]
         for f in ("ibfthost_store_add", "ibfthost_add_message", "ibfthost_is_acceptable", "ibfthost_is_valid_validator"):
@@ -189,6 +196,24 @@ class HostContext:
 
     def set_wire_frames(self, on: bool):
         self.lib.ibfthost_set_wire_frames(self.ctx, int(on))
+
+    def set_reject_hook(self, fn):
+        """GpuVerifier::onReject: fn(kind, height, message, from_, reason, recovered) once per rejected item -- kind IBFT_KIND_PAYLOAD /
+        _WIRE (IsValidValidator: message = PayloadNoSig / the raw frame) or _SEAL (IsValidCommittedSeal: message = the proposal
+        hash), reason REASON_*, recovered = the recovered address (20 bytes, zero when recovery was not reached).  None removes it."""
+        if fn is None:
+            self._reject_cb = None
+            self.lib.ibfthost_set_reject_hook(self.ctx, CB_REJECT(), None)
+            return
+        self._reject_cb = CB_REJECT(lambda _u, kind, h, m, mn, f, fn_, reason, rec: fn(kind, h, _bytes(m, mn), _bytes(f, fn_), reason,
+                                                                                        _bytes(rec, 20)))
+        self.lib.ibfthost_set_reject_hook(self.ctx, self._reject_cb, None)
+
+    def gpu_rejects(self, reason: int) -> int:
+        return int(self.lib.ibfthost_gpu_rejects(self.ctx, reason))
+
+    def gpu_explain_calls(self) -> int:
+        return int(self.lib.ibfthost_gpu_explain_calls(self.ctx))
 
     def gpu_frames_handed_back(self) -> int:
         return int(self.lib.ibfthost_gpu_frames_handed_back(self.ctx))

@@ -129,6 +129,22 @@ void ibfthost_set_incremental_quorum(ibfthost_ctx* c, int on) { c->ibft->increme
 void ibfthost_set_wire_frames(ibfthost_ctx* c, int on) { if (c->gpu) c->gpu->use_wire_frames = on != 0; }
 uint64_t ibfthost_gpu_frames_handed_back(ibfthost_ctx* c) { return c->gpu ? c->gpu->frames_handed_back() : 0; }
 
+// GpuVerifier::onReject: fn(user, kind, height, message, from, reason, recovered20) once per rejected item (see verifier.hpp);
+// fn = NULL removes the hook.  Set it before the context is used from several threads.
+typedef void (*cb_on_reject)(void* user, uint8_t kind, uint64_t height, const uint8_t* message, size_t mlen, const uint8_t* from,
+                             size_t flen, uint8_t reason, const uint8_t* recovered20);
+void ibfthost_set_reject_hook(ibfthost_ctx* c, cb_on_reject fn, void* user) {
+  if (!c->gpu) return;
+  if (!fn) { c->gpu->onReject = nullptr; return; }
+  c->gpu->onReject = [fn, user](const GpuVerifier::Rejection& x) {
+    fn(user, x.kind, x.height, (const uint8_t*)x.message.data(), x.message.size(), (const uint8_t*)x.from.data(), x.from.size(), x.reason,
+       (const uint8_t*)x.recovered.data());
+  };
+}
+// rejections reported with `reason` (IBFT_REASON_*), and the explain calls made for them
+uint64_t ibfthost_gpu_rejects(ibfthost_ctx* c, uint32_t reason) { return c->gpu && reason < 256 ? c->gpu->rejects((uint8_t)reason) : 0; }
+uint64_t ibfthost_gpu_explain_calls(ibfthost_ctx* c) { return c->gpu ? c->gpu->explain_calls() : 0; }
+
 // state.view / state.name / state.proposalMessage
 int ibfthost_set_state(ibfthost_ctx* c, uint64_t height, uint64_t round, int state_name, const uint8_t* proposal_wire, size_t len) {
   c->ibft->state.view = View{height, round};

@@ -242,7 +242,9 @@ class GpuVerifier : public Verifier {
       for (auto& m : msgs)
         if (m) visit(*m);
     }
-    verify_pending(batch, nullptr);
+    std::vector<ExplainCall> explain;
+    verify_pending(batch, nullptr, onReject ? &explain : nullptr);
+    report_rejects(explain);
   }
 
   // Re-verification of the >= Q committed seals of an imported block (Backend.InsertProposal, core/backend.go:78-81; the same
@@ -264,11 +266,33 @@ class GpuVerifier : public Verifier {
       }
     }
     std::vector<int8_t> verdicts;
-    verify_pending(batch, &verdicts);
+    std::vector<ExplainCall> explain;
+    verify_pending(batch, &verdicts, onReject ? &explain : nullptr);
     std::vector<bool> valid(seals.size(), false);
     for (size_t i = 0; i < seals.size(); i++) valid[i] = where[i] == -2 || (where[i] >= 0 && verdicts[(size_t)where[i]] == 1);
+    report_rejects(explain);
     return valid;
   }
+
+  // Reject reasons (opt-in).  With onReject set, every device verify call that rejected any item is followed by ONE
+  // ibft_explain_batch call over those items, and onReject runs once per rejected item with the reason (IBFT_REASON_*) and the
+  // recovered address: what polygon-edge's IsValidValidator logs ("ecrecover failed", "signer does not match From", "signer not
+  // in the validator set").  It runs after the verdicts are published, outside the coalescer's locks, on the thread that made the
+  // device call (the ingress leader, or the caller of Prefetch / VerifyCommittedSeals).  Set it before the verifier is shared.
+  // Without it nothing changes: no explain call is made.  Not reported: frames the device hands back (their re-submission is
+  // explained if rejected), items of a height whose validator table is not resident (the host rejects those, the device accepts
+  // their signature), and the items of a device call that failed.
+  struct Rejection {
+    uint8_t kind;     // IBFT_KIND_PAYLOAD or IBFT_KIND_WIRE: IsValidValidator; IBFT_KIND_SEAL: IsValidCommittedSeal
+    uint64_t height;  // the message's height (a seal: the running sequence's)
+    Bytes message;    // PAYLOAD: PayloadNoSig; WIRE: the raw frame; SEAL: the proposal hash
+    Bytes from;       // the expected signer: msg.From / seal.Signer
+    uint8_t reason;   // IBFT_REASON_*
+    Bytes recovered;  // 20 bytes: the recovered signer, zero when recovery was not reached
+  };
+  std::function<void(const Rejection&)> onReject;
+  uint64_t rejects(uint8_t reason) const { return reject_counts_[reason].load(); }  // rejections reported with each reason
+  uint64_t explain_calls() const { return explain_calls_.load(); }
 
   uint64_t device_calls() const { return device_calls_.load(); }
   uint64_t items_verified() const { return items_verified_.load(); }
@@ -304,6 +328,16 @@ class GpuVerifier : public Verifier {
   std::atomic<uint64_t> current_height_{0};
   uint64_t epoch_ = 0;  // bumped by SetValidators: verdicts computed against a replaced table are not cached
   std::atomic<uint64_t> device_calls_{0}, items_verified_{0}, frames_handed_back_{0}, ingress_requests_{0}, ingress_flushes_{0};
+  std::atomic<uint64_t> reject_counts_[256] = {}, explain_calls_{0};
+  // one device call with rejected items, kept for its explain call (onReject)
+  struct ExplainCall {
+    std::vector<ibft_sig_item> items;
+    Bytes arena;
+    std::vector<ibft_group_desc> groups;
+    std::vector<uint32_t> bitmap;  // the call's verdicts, with the bits of the items not to report set
+    std::vector<uint32_t> index;   // item of each rejection
+    std::vector<Rejection> rejected;
+  };
   // ingress coalescer
   std::mutex ing_mu_;
   std::deque<std::shared_ptr<Req>> ing_queue_;
@@ -386,6 +420,7 @@ class GpuVerifier : public Verifier {
     req->p = std::move(p);
     std::unique_lock<std::mutex> lk(ing_mu_);
     ing_queue_.push_back(req);
+    std::vector<ExplainCall> explain;  // the rejections of the flushes this caller led, reported once it holds no lock
     while (!req->done) {
       // the first leader starts at once; a second one (while a flush is already on the device) only for a queue worth a launch of
       // its own -- otherwise the newcomers keep piling up behind the flush in flight and go up together when it returns
@@ -415,7 +450,7 @@ class GpuVerifier : public Verifier {
         if (ins.second) batch.push_back(taken[i]->p);
       }
       std::vector<int8_t> verdicts;
-      verify_pending(batch, &verdicts);
+      verify_pending(batch, &verdicts, onReject ? &explain : nullptr);
       ingress_flushes_++;
       lk.lock();
       for (size_t i = 0; i < taken.size(); i++) {
@@ -426,12 +461,38 @@ class GpuVerifier : public Verifier {
       ing_leaders_--;
       if (!ing_queue_.empty()) ing_queue_.front()->cv.notify_one();  // somebody is waiting: hand the lead over
     }
+    lk.unlock();
+    report_rejects(explain);
     return req->result;
+  }
+
+  // one explain call per recorded device call; onReject per rejected item
+  void report_rejects(std::vector<ExplainCall>& calls) {
+    for (auto& c : calls) {
+      const uint32_t n = (uint32_t)c.items.size();
+      std::vector<uint8_t> reasons(n), rec((size_t)n * 20);
+      int rc = ibft_explain_batch(engine_, c.items.data(), n, (const uint8_t*)c.arena.data(), c.arena.size(), c.groups.data(),
+                                  (uint32_t)c.groups.size(), c.bitmap.data(), reasons.data(), rec.data());
+      explain_calls_++;
+      if (rc != IBFT_OK) {
+        std::lock_guard<std::mutex> lk(state_mu_);
+        error_ = ibft_last_error();
+        continue;
+      }
+      for (size_t k = 0; k < c.rejected.size(); k++) {
+        Rejection& x = c.rejected[k];
+        x.reason = reasons[c.index[k]];
+        x.recovered.assign((const char*)rec.data() + (size_t)c.index[k] * 20, 20);
+        reject_counts_[x.reason]++;
+        onReject(x);
+      }
+    }
   }
 
   // One device call per engine-capacity chunk of the batch; groups = distinct heights (validator tables).
   // verdicts (optional): per batch entry 1 = valid, 0 = invalid, -1 = no verdict (the device call failed).
-  void verify_pending(std::vector<Pending>& batch, std::vector<int8_t>* verdicts) {
+  // explain (optional): the device calls that rejected items, with those items (onReject).
+  void verify_pending(std::vector<Pending>& batch, std::vector<int8_t>* verdicts, std::vector<ExplainCall>* explain = nullptr) {
     if (verdicts) verdicts->assign(batch.size(), -1);
     if (batch.empty() || !engine_) return;
     std::map<uint32_t, uint64_t> slot_height;
@@ -503,6 +564,7 @@ class GpuVerifier : public Verifier {
         items_verified_ += n;
         std::vector<Pending> redo;
         std::vector<size_t> redo_of;
+        ExplainCall ec;
         {
           std::lock_guard<std::mutex> lk(state_mu_);
           const bool fresh = epoch == epoch_;  // the tables this batch was checked against are still the resident ones
@@ -524,12 +586,35 @@ class GpuVerifier : public Verifier {
             }
             if (fresh) cache_[p.key] = pass;
             if (verdicts) (*verdicts)[pos + i] = pass ? 1 : 0;
+            if (explain && !((bitmap[i >> 5] >> (i & 31)) & 1u)) {
+              Rejection x{};
+              x.kind = p.item.kind;
+              x.height = p.height;
+              if (p.item.kind == IBFT_KIND_WIRE) {
+                x.message.assign(p.wire_root->data() + p.wire_off, p.wire_len);
+                if (p.fallback_payload_msg) x.from = p.fallback_payload_msg->from;
+              } else {
+                x.message = p.item.kind == IBFT_KIND_SEAL ? Bytes((const char*)p.item.digest, 32) : p.payload;
+                x.from.assign((const char*)p.item.signer, 20);
+              }
+              ec.index.push_back((uint32_t)i);
+              ec.rejected.push_back(std::move(x));
+            }
           }
+        }
+        if (explain && !ec.rejected.empty()) {
+          // only the reported items are explained: every other bit is set
+          ec.bitmap.assign(bitmap.size(), 0xFFFFFFFFu);
+          for (uint32_t i : ec.index) ec.bitmap[i >> 5] &= ~(1u << (i & 31));
+          ec.items.assign(items.begin(), items.begin() + n);
+          ec.arena = arena;
+          ec.groups = groups;
+          explain->push_back(std::move(ec));
         }
         if (!redo.empty()) {
           frames_handed_back_ += redo.size();
           std::vector<int8_t> rv;
-          verify_pending(redo, &rv);
+          verify_pending(redo, &rv, explain);
           if (verdicts)
             for (size_t k = 0; k < redo.size(); k++) (*verdicts)[redo_of[k]] = rv[k];
         }

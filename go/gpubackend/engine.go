@@ -177,20 +177,15 @@ func packItem(p *C.ibft_sig_item, it Item, arena *[]byte) bool {
 	return true
 }
 
-// VerifyBatch runs ONE device call for all items and returns one verdict per item.  A failed launch returns an error and
-// NO verdicts (callers treat that as "not valid yet", never as true).  Go memory is only read during the call: the ABI
-// copies into engine-owned pinned staging.
-func (e *Engine) VerifyBatch(items []Item) ([]bool, error) {
-	n := len(items)
-	if n == 0 {
-		return nil, nil
-	}
-	packed := make([]C.ibft_sig_item, n)
-	var arena []byte
-	groups := []C.ibft_group_desc{}
+// packBatch marshals items into packed tuples, their arena, and one group per distinct Height (the slot of the height's resident
+// table, or IBFT_NO_TABLE); noTable marks the groups of heights without a resident table.
+func (e *Engine) packBatch(items []Item) (packed []C.ibft_sig_item, arena []byte, groups []C.ibft_group_desc, noTable map[uint16]bool) {
+	packed = make([]C.ibft_sig_item, len(items))
+	groups = []C.ibft_group_desc{}
 	groupOf := map[uint64]uint16{}
-	noTable := map[uint16]bool{} // groups whose height has no resident table: verdict forced to false
+	noTable = map[uint16]bool{} // groups whose height has no resident table: verdict forced to false
 	e.mu.RLock()
+	defer e.mu.RUnlock()
 	for i, it := range items {
 		p := &packed[i]
 		if !packItem(p, it, &arena) {
@@ -212,20 +207,37 @@ func (e *Engine) VerifyBatch(items []Item) ([]bool, error) {
 		}
 		p.group = C.uint16_t(g)
 	}
-	e.mu.RUnlock()
+	return packed, arena, groups, noTable
+}
+
+func arenaPtr(arena []byte) *C.uint8_t {
+	if len(arena) == 0 {
+		return nil
+	}
+	return (*C.uint8_t)(unsafe.Pointer(&arena[0]))
+}
+
+func groupsPtr(groups []C.ibft_group_desc) *C.ibft_group_desc {
+	if len(groups) == 0 {
+		return nil
+	}
+	return &groups[0]
+}
+
+// VerifyBatch runs ONE device call for all items and returns one verdict per item.  A failed launch returns an error and
+// NO verdicts (callers treat that as "not valid yet", never as true).  Go memory is only read during the call: the ABI
+// copies into engine-owned pinned staging.
+func (e *Engine) VerifyBatch(items []Item) ([]bool, error) {
+	n := len(items)
+	if n == 0 {
+		return nil, nil
+	}
+	packed, arena, groups, noTable := e.packBatch(items)
 	bitmap := make([]uint32, (n+31)/32)
-	var ap *C.uint8_t
-	if len(arena) > 0 {
-		ap = (*C.uint8_t)(unsafe.Pointer(&arena[0]))
-	}
-	var gp *C.ibft_group_desc
-	if len(groups) > 0 {
-		gp = &groups[0]
-	}
 	// _ex: everything comes back with the call itself (a goroutine may change OS threads between two cgo calls, so the
 	// "last call" getters are not usable from Go)
-	rc := C.ibft_verify_batch_ex(e.h, &packed[0], C.uint32_t(n), ap, C.size_t(len(arena)), gp, C.uint32_t(len(groups)),
-		(*C.uint32_t)(unsafe.Pointer(&bitmap[0])), nil, nil, nil, nil, 0)
+	rc := C.ibft_verify_batch_ex(e.h, &packed[0], C.uint32_t(n), arenaPtr(arena), C.size_t(len(arena)), groupsPtr(groups),
+		C.uint32_t(len(groups)), (*C.uint32_t)(unsafe.Pointer(&bitmap[0])), nil, nil, nil, nil, 0)
 	if rc != C.IBFT_OK {
 		return nil, fmt.Errorf("ibft_verify_batch_ex: %w", lastError())
 	}
@@ -234,6 +246,78 @@ func (e *Engine) VerifyBatch(items []Item) ([]bool, error) {
 		out[i] = bitmap[i/32]>>(uint(i)%32)&1 == 1 && !noTable[uint16(packed[i].group)]
 	}
 	return out, nil
+}
+
+// Reason says why the device rejected a signature check (include/ibft_verify.h IBFT_REASON_*).  When several apply, the first
+// in this order is given: it is the order in which the verify pipeline decides.
+type Reason uint8
+
+const (
+	ReasonOK             Reason = C.IBFT_REASON_OK
+	ReasonNoGroup        Reason = C.IBFT_REASON_NO_GROUP
+	ReasonMalformed      Reason = C.IBFT_REASON_MALFORMED
+	ReasonNeedsHost      Reason = C.IBFT_REASON_NEEDS_HOST
+	ReasonBadV           Reason = C.IBFT_REASON_BAD_V
+	ReasonRRange         Reason = C.IBFT_REASON_R_RANGE
+	ReasonSRange         Reason = C.IBFT_REASON_S_RANGE
+	ReasonRNotX          Reason = C.IBFT_REASON_R_NOT_X
+	ReasonNoKey          Reason = C.IBFT_REASON_NO_KEY
+	ReasonSignerMismatch Reason = C.IBFT_REASON_SIGNER_MISMATCH
+	ReasonNotValidator   Reason = C.IBFT_REASON_NOT_VALIDATOR
+	ReasonInconsistent   Reason = C.IBFT_REASON_INCONSISTENT
+)
+
+func (r Reason) String() string {
+	switch r {
+	case ReasonOK:
+		return "ok"
+	case ReasonNoGroup:
+		return "no group"
+	case ReasonMalformed:
+		return "malformed"
+	case ReasonNeedsHost:
+		return "frame needs the host"
+	case ReasonBadV:
+		return "recovery id not 0 or 1"
+	case ReasonRRange:
+		return "r out of range"
+	case ReasonSRange:
+		return "s out of range"
+	case ReasonRNotX:
+		return "r is not an abscissa"
+	case ReasonNoKey:
+		return "recovered point at infinity"
+	case ReasonSignerMismatch:
+		return "signer does not match"
+	case ReasonNotValidator:
+		return "signer not in the validator set"
+	case ReasonInconsistent:
+		return "inconsistent"
+	}
+	return fmt.Sprintf("reason(%d)", uint8(r))
+}
+
+// ExplainBatch says why each item is rejected (ibft_explain_batch over every item, grouped as VerifyBatch groups them): one
+// Reason and the recovered address (20 bytes, zero when recovery was not reached) per item.  An item of a height whose table
+// is not resident gets ReasonOK when its signature is good: VerifyBatch rejects it on the host, not on the device.
+func (e *Engine) ExplainBatch(items []Item) ([]Reason, [][]byte, error) {
+	n := len(items)
+	if n == 0 {
+		return nil, nil, nil
+	}
+	packed, arena, groups, _ := e.packBatch(items)
+	reasons := make([]byte, n)
+	rec := make([]byte, n*20)
+	rc := C.ibft_explain_batch(e.h, &packed[0], C.uint32_t(n), arenaPtr(arena), C.size_t(len(arena)), groupsPtr(groups),
+		C.uint32_t(len(groups)), nil, (*C.uint8_t)(unsafe.Pointer(&reasons[0])), (*C.uint8_t)(unsafe.Pointer(&rec[0])))
+	if rc != C.IBFT_OK {
+		return nil, nil, fmt.Errorf("ibft_explain_batch: %w", lastError())
+	}
+	out, addrs := make([]Reason, n), make([][]byte, n)
+	for i := range out {
+		out[i], addrs[i] = Reason(reasons[i]), rec[20*i:20*i+20]
+	}
+	return out, addrs, nil
 }
 
 // Quorum rules of a Group (include/ibft_verify.h IBFT_QUORUM_*): which of go-ibft's per-message-type decisions

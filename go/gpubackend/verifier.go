@@ -33,6 +33,12 @@ type Verifier struct {
 	// SURVEY.md §8c on the device.  Also the place to hash ONE multi-megabyte proposal on a host core (DESIGN.md §3.3).
 	ProposalHashFn func(raw []byte, round uint64) [32]byte
 
+	// OnReject (optional) is called once per signature check the device rejected, with the reason and the recovered address (20
+	// bytes, zero when recovery was not reached): after every device call that rejected items, one ExplainBatch call over them.
+	// It runs after the verdicts are published and outside the verifier's locks.  Set it before the verifier is shared; nil
+	// (the default) makes no extra device call.  Items of a height whose table is not resident are not reported.
+	OnReject func(msg Item, reason Reason, recovered []byte)
+
 	// ingress coalescer knobs (see lookupOrCoalesce)
 	IngressMaxBatch int
 	IngressMinBatch int
@@ -197,9 +203,37 @@ func (v *Verifier) lookupOrCoalesce(it Item, key string) bool {
 		}
 		v.ingLeader = false
 		v.ingCond.Broadcast()
+		v.ingMu.Unlock()
+		v.reportRejects(items, res)
+		v.ingMu.Lock()
 	}
 	v.ingMu.Unlock()
 	return req.result
+}
+
+// reportRejects: one ExplainBatch call over the items a device call rejected, then OnReject for each
+func (v *Verifier) reportRejects(items []Item, res []bool) {
+	if v.OnReject == nil || res == nil {
+		return
+	}
+	var rejected []Item
+	for i, ok := range res {
+		if !ok {
+			rejected = append(rejected, items[i])
+		}
+	}
+	if len(rejected) == 0 {
+		return
+	}
+	reasons, recovered, err := v.Eng.ExplainBatch(rejected)
+	if err != nil {
+		return
+	}
+	for i, r := range reasons {
+		if r != ReasonOK { // ReasonOK: rejected on the host (no resident table), not by the device
+			v.OnReject(rejected[i], r, recovered[i])
+		}
+	}
 }
 
 // IsValidValidator: signer of msg.Signature over Keccak-256(PayloadNoSig) == msg.From and From is a validator at
@@ -296,5 +330,5 @@ func (v *Verifier) Prefetch(msgs []*proto.IbftMessage, withSeals bool) {
 	for _, m := range msgs {
 		visit(m)
 	}
-	v.verifyBatch(items, keys)
+	v.reportRejects(items, v.verifyBatch(items, keys))
 }

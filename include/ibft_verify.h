@@ -40,11 +40,12 @@ extern "C" {
                                 IbftMessage.PayloadNoSig() (messages/proto/helper.go:13-27) */
 #define IBFT_KIND_SEAL 2     /* `digest` holds proposalHash; z = Keccak-256(proposalHash || 0x02) -- IsValidCommittedSeal
                                 (0x02 = MessageType_COMMIT, messages/proto/messages.proto:10) */
-#define IBFT_KIND_WIRE 3      /* arena slice = the COMPLETE wire encoding of a PREPARE / COMMIT IbftMessage (a raw gossip frame).  The device
-                                finds From, Signature and the signed bytes itself: for a canonically encoded frame PayloadNoSig
-                                (messages/proto/helper.go:13-27) is the frame minus its field-3 TLV.  r/s/v/signer/digest of the tuple are
-                                ignored.  Frames that are not canonical, or carry a nested payload (PREPREPARE / ROUND_CHANGE), get verdict 0
-                                and item status IBFT_ITEM_NEEDS_HOST: the host re-submits those as IBFT_KIND_PAYLOAD. */
+#define IBFT_KIND_WIRE 3      /* arena slice = the COMPLETE wire encoding of an IbftMessage of any of the four types (a raw gossip frame).
+                                The device finds From, Signature and the signed bytes itself: for a canonically encoded frame PayloadNoSig
+                                (messages/proto/helper.go:13-27) is the frame minus its field-3 TLV.  It walks the whole frame, nested
+                                PREPREPARE / ROUND_CHANGE certificates included, and checks its encoding.  r/s/v/signer/digest of the tuple
+                                are ignored.  Frames that are not canonical get verdict 0 and item status IBFT_ITEM_NEEDS_HOST: the host
+                                re-submits those as IBFT_KIND_PAYLOAD. */
 #define IBFT_KIND_WIRE_SEAL 4 /* same frame; checks the committed seal instead: commitData.committedSeal over
                                 Keccak-256(commitData.proposalHash || 0x02), signer = From (IsValidCommittedSeal on the frame) */
 #define IBFT_KIND_PAYLOAD2 5  /* z = Keccak-256(arena[payload_off .. +payload_len] || arena[off2 .. +len2]) with off2 = u64 little-endian in
@@ -61,6 +62,24 @@ extern "C" {
 #define IBFT_ITEM_NEEDS_HOST 1  /* IBFT_KIND_WIRE*: frame not canonical / not a flat PREPARE or COMMIT; verdict bit is 0, re-submit as KIND_PAYLOAD */
 
 #define IBFT_NO_TABLE 0xFFFFu /* ibft_group_desc.table_slot: skip the validator-set membership test */
+
+/* Why an item was rejected (ibft_explain_batch), one byte per item.  When several apply, the first in this order wins: it is the
+ * order in which the verify pipeline decides. */
+#define IBFT_REASON_OK 0              /* the item verifies */
+#define IBFT_REASON_NO_GROUP 1        /* item.group >= n_groups (only when the call has groups) */
+#define IBFT_REASON_MALFORMED 2       /* IBFT_KIND_INVALID or an unknown kind; a payload span (or the second span of PAYLOAD2) outside
+                                         the arena; a canonical frame without a 20-byte From, a View (WIRE) or a 65-byte signature;
+                                         a WIRE_SEAL frame that is not a COMMIT with a 32-byte proposalHash and a 65-byte seal */
+#define IBFT_REASON_NEEDS_HOST 3      /* a non-canonical frame: exactly the items with status IBFT_ITEM_NEEDS_HOST */
+#define IBFT_REASON_BAD_V 4           /* v is not 0 or 1 */
+#define IBFT_REASON_R_RANGE 5         /* r = 0 or r >= n */
+#define IBFT_REASON_S_RANGE 6         /* s = 0 or s >= n */
+#define IBFT_REASON_R_NOT_X 7         /* r^3 + 7 is not a square mod p: no curve point has abscissa r */
+#define IBFT_REASON_NO_KEY 8          /* the recovered point is the point at infinity */
+#define IBFT_REASON_SIGNER_MISMATCH 9 /* the recovered address is not the expected signer (From / seal signer) */
+#define IBFT_REASON_NOT_VALIDATOR 10  /* the recovered address is the expected signer, but it is not in the group's validator table
+                                         (never for an IBFT_NO_TABLE group) */
+#define IBFT_REASON_INCONSISTENT 255  /* the explain pass accepts an item whose given verdict bit is 0: a bug, never expected */
 
 /* One signature check = one packed 128-byte tuple: (r, s, v, hash) + the expected signer.
  * Serves both IsValidValidator(msg) (core/backend.go:41-45: signer of msg.Signature over the payload
@@ -199,6 +218,7 @@ int ibft_engine_device_info(ibft_engine* e, ibft_device_info* out);
  *                                  any failure returns its status with every output untouched.  A call takes the small lane of
  *                                  every device when the whole call fits it, else the bulk lane, locked in device-list order.
  *                                  The results are byte for byte those of a single-device engine.
+ *   ibft_explain_batch             the lead answers (the tables are replicated, and the items to explain are few).
  *   ibft_last_item_status,         the most recent completed call: statuses assembled from the shards, the merged voted sets,
  *   ibft_get_voted_bitmap,         handed-back summed over the devices that call used.
  *   ibft_debug_known_handed_back
@@ -262,6 +282,25 @@ int ibft_verify_batch_ex(ibft_engine* e, const ibft_sig_item* items, uint32_t n,
 
 /* Per-item status (IBFT_ITEM_*) of the most recent completed ibft_verify_batch / ibft_verify_wait on this engine. */
 int ibft_last_item_status(ibft_engine* e, uint8_t* status_out, uint32_t n);
+
+/* Why items were rejected: a separate, opt-in pass that decides the rejected items again, one thread each, and says at which
+ * step each one failed (IBFT_REASON_*) -- what polygon-edge's IsValidValidator separates in its logs ("ecrecover failed",
+ * "signer does not match From", "signer not in the validator set").  The verify calls and their kernels are untouched by it.
+ *   items, arena, groups: the inputs of a verify call, against the same validator tables
+ *   bitmap: that call's verdict bitmap, (n+31)/32 words, or NULL.  An item whose bit is 1 gets IBFT_REASON_OK without any device
+ *           work; only the items whose bit is 0 are staged (compacted on the host; the arena goes up whole, as spans point into
+ *           it) and decided again.  NULL explains every item (tests and tools).
+ *   reasons_out: n bytes.  recovered_out: NULL, or n x 20 bytes receiving the recovered address of the items that got as far as
+ *           recovery (IBFT_REASON_SIGNER_MISMATCH, _NOT_VALIDATOR, and _OK when explained); zero for every other item.
+ * Every reason is the recover path's decision: the key registry is never consulted or taught.  IBFT_REASON_INCONSISTENT marks
+ * an item the pass accepts although its given bit is 0.  Errors are those of the verify calls (IBFT_ERR_NO_TABLE for a group
+ * whose slot holds another height, IBFT_ERR_CAPACITY beyond max_items / max_payload_bytes / max_groups, IBFT_ERR_INVALID_ARG for
+ * a null output or a bad quorum rule); on failure every output is untouched.  The call takes a lane as a host-buffer verify
+ * call does (the small lane when the explained items and the arena fit it, else the bulk lane) and never waits for the other
+ * lane; it is one launch, and none when no bit is 0. */
+int ibft_explain_batch(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                       const ibft_group_desc* groups, uint32_t n_groups, const uint32_t* bitmap, uint8_t* reasons_out,
+                       uint8_t* recovered_out);
 
 /* Asynchronous variant: same arguments; inputs are copied into engine-owned pinned staging before the call
  * returns (cgo rule: no Go pointer is retained).  ibft_verify_poll returns IBFT_OK with *done = 0/1;
