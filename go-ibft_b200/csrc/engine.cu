@@ -23,6 +23,7 @@
 #include <string>
 #include <thread>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "../../include/ibft_verify.h"
@@ -1499,6 +1500,37 @@ k_adopt_entries(uint32_t* __restrict__ key_ref, uint32_t n, uint32_t* __restrict
     key_ref[v] = r & ~IBFT_KEY_REF_FRESH;
   }
 }
+// Multi-device engines: take the keys another device of the engine has learned.  src_state / src_xy: a copy of that device's
+// state and keys of entries [0, n).  The sub-engines number their entries alike (they take every registry-changing call in the
+// same order), so entry r names the same address on both -- except after a replication rolled back part way, when it may not:
+// key_matches_address against this device's own address of entry r refuses such a key, and the entry learns by recovery.  An
+// adopted key is written as learn_key writes a recovered one (first writer wins, every writer stores the same key), so the
+// kernel may run beside the verify kernels of any lane; `adopted` counts the keys this launch took.
+__global__ void __launch_bounds__(256)
+k_adopt_peer_keys(const uint32_t* __restrict__ src_state, const uint32_t* __restrict__ src_xy, uint32_t n, uint32_t* state,
+                  uint32_t* key_xy, const uint8_t* __restrict__ addr, uint32_t* learn_count, uint32_t* adopted) {
+  const uint32_t r = blockIdx.x * 256 + threadIdx.x;
+  if (r >= n) return;
+  const uint32_t ss = src_state[r];
+  if (!(ss == IBFT_KEY_LEARNED || ss == IBFT_KEY_READY || ss == IBFT_KEY_EVICTED) || state[r] != IBFT_KEY_UNKNOWN) return;
+  fe x, y;
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    x.v[i] = src_xy[16 * (size_t)r + i];
+    y.v[i] = src_xy[16 * (size_t)r + 8 + i];
+  }
+  if (!key_matches_address(x, y, addr + 20 * (size_t)r)) return;
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    key_xy[16 * (size_t)r + i] = x.v[i];
+    key_xy[16 * (size_t)r + 8 + i] = y.v[i];
+  }
+  __threadfence();
+  if (atomicCAS(&state[r], IBFT_KEY_UNKNOWN, IBFT_KEY_LEARNED) == IBFT_KEY_UNKNOWN) {
+    atomicAdd(learn_count, 1u);
+    atomicAdd(adopted, 1u);
+  }
+}
 #endif
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1598,6 +1630,7 @@ __global__ void k_debug_op(int op, const uint8_t* a, const uint8_t* b, const uin
       }
       break;
     }
+    case IBFT_DBG_KEY_ADDRESS: o[0] = key_matches_address(fe_from_be(pa), fe_from_be(pb), c + 64 * (size_t)i) ? 1 : 0; break;
     default: debug_arith_op(op, pa, pb, o, c ? c + 64 * (size_t)i : nullptr); break;
   }
 }
@@ -1705,6 +1738,8 @@ struct key_registry {
   uint32_t capacity = 0;                 // entries that state / key_xy / the chunk-pointer array can hold
   uint32_t* d_state = nullptr;           // capacity words
   uint32_t* d_key_xy = nullptr;          // capacity x 16 words
+  uint8_t* d_addr = nullptr;             // capacity x 20 bytes: the address of each entry handed out (k_adopt_peer_keys checks
+                                         // an adopted key against it)
   uint32_t** d_chunks = nullptr;         // capacity / IBFT_KEY_CHUNK (rounded up) chunk base pointers
   uint32_t* d_learn_count = nullptr;     // keys learned so far (learn_key)
   uint32_t* h_learn_count = nullptr;     // pinned
@@ -1712,7 +1747,7 @@ struct key_registry {
   std::vector<uint32_t*> chunks;         // host copy of the allocated chunk pointers
   uint32_t used = 0;                     // entries [0, used) have been handed out at least once (high-water mark)
   std::unordered_map<addr20, uint32_t, addr20_hash> by_addr;
-  std::vector<addr20> addr_of;           // address of each entry in use
+  std::vector<addr20> addr_of;           // address of each entry in use (a retired entry keeps its last one, here and in d_addr)
   std::vector<uint32_t> refs;            // reference count of each entry
   std::vector<uint32_t> free_list;       // retired entries, reused before the high-water mark moves
   // Bounded registry (ibft_set_key_table_budget, for the rest of the engine's life): `chunks` is a pool of budget.max_tables
@@ -1815,6 +1850,7 @@ struct ibft_engine {
   // above; a view is the borrowed diagnostics handle of one of them (ibft_engine_sub)
   struct multi_engine* multi = nullptr;
   ibft_engine* view_of = nullptr;
+  bool coordinated = false;  // a sub-engine of a multi-device engine: its coordinator shares and refreshes the learned keys
 };
 // Entry points of a coordinator or a view (defined with ibft_engine_create_multi at the end of this file)
 static int multi_refused(ibft_engine* e, const char* fn);
@@ -1956,7 +1992,7 @@ static void engine_free(ibft_engine* e) {
   cudaFree(e->d_ctable);
   for (auto c : e->reg.chunks) cudaFree(c);
   cudaFree(e->reg.d_tab); cudaFree(e->reg.d_used);
-  cudaFree(e->reg.d_state); cudaFree(e->reg.d_key_xy); cudaFree(e->reg.d_chunks); cudaFree(e->reg.d_learn_count);
+  cudaFree(e->reg.d_state); cudaFree(e->reg.d_key_xy); cudaFree(e->reg.d_addr); cudaFree(e->reg.d_chunks); cudaFree(e->reg.d_learn_count);
   cudaFreeHost(e->reg.h_learn_count);
   cudaFree(e->d_slots);
   if (e->hash_stream) cudaStreamDestroy(e->hash_stream);
@@ -2019,6 +2055,7 @@ static int engine_alloc(ibft_engine* e) {
     const size_t n_chunks = (cap + IBFT_KEY_CHUNK - 1) / IBFT_KEY_CHUNK;
     CU(cudaMalloc(&R.d_state, std::max<size_t>(cap, 1) * 4));
     CU(cudaMalloc(&R.d_key_xy, std::max<size_t>(cap, 1) * 64));
+    CU(cudaMalloc(&R.d_addr, std::max<size_t>(cap, 1) * 20));
     CU(cudaMalloc(&R.d_chunks, std::max<size_t>(n_chunks, 1) * sizeof(uint32_t*)));
     CU(cudaMemset(R.d_chunks, 0, std::max<size_t>(n_chunks, 1) * sizeof(uint32_t*)));
     CU(cudaMalloc(&R.d_learn_count, 4));
@@ -2533,8 +2570,16 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
   if (s.d_key_ref) {
     // upload key_ref; entries new to their address are reset to unknown before any kernel can read them through this table
     cudaError_t ce = cudaMemcpy(s.d_key_ref, s.key_ref.data(), (size_t)n * 4, cudaMemcpyHostToDevice);
-    bool adopt = false;
-    for (uint32_t v = 0; v < n && !adopt; v++) adopt = (s.key_ref[v] & IBFT_KEY_REF_FRESH) != 0;
+    uint32_t lo = UINT32_MAX, hi = 0;  // the entries new to their address lie in [lo, hi)
+    for (uint32_t v = 0; v < n; v++)
+      if (s.key_ref[v] & IBFT_KEY_REF_FRESH) {
+        lo = std::min(lo, s.key_ref[v] & ~IBFT_KEY_REF_FRESH);
+        hi = std::max(hi, (s.key_ref[v] & ~IBFT_KEY_REF_FRESH) + 1);
+      }
+    const bool adopt = lo < hi;
+    static_assert(sizeof(addr20) == 20, "addr_of is uploaded as packed 20-byte addresses");
+    if (ce == cudaSuccess && adopt)  // the others of [lo, hi) hold their address already
+      ce = cudaMemcpy(e->reg.d_addr + 20 * (size_t)lo, e->reg.addr_of[lo].b, 20 * (size_t)(hi - lo), cudaMemcpyHostToDevice);
     if (ce == cudaSuccess && adopt) {
       k_adopt_entries<<<(n + 255) / 256, 256>>>(s.d_key_ref, n, e->reg.d_state, e->reg.bounded ? e->reg.d_tab : nullptr);
       e->launches++;
@@ -2585,24 +2630,24 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
 // Key registry upkeep: build the comb tables of the keys learned since the last call -- one claim / build / publish pass over
 // the engine's registry, whichever tables the keys were learned through.  Cheap when nothing is new (one 4-byte read).
 // ibft_verify_batch / ibft_verify_wait call it on their way out; callers of the device-resident entry points call it between
-// rounds.  n_ready_out: the members of the resident tables whose key is known, summed over the tables.
-static int refresh_key_tables_locked(ibft_engine* e, lane* L, uint32_t* n_ready_out) {
+// rounds.  n_ready_out: the members of the resident tables whose key is known, summed over the tables.  The caller holds
+// keys_mu; the work goes on stream st.
+static int refresh_key_tables_held(ibft_engine* e, cudaStream_t st, uint32_t* n_ready_out) {
   uint32_t total = 0;
 #if IBFT_WC > 0
   if ((e->p.flags & IBFT_FLAG_KEY_CACHE) && e->reg.d_state) {
     key_registry& R = e->reg;
-    std::lock_guard<std::mutex> kl(e->keys_mu);
     CU(cudaSetDevice(e->p.device));
-    CU(cudaMemcpyAsync(R.h_learn_count, R.d_learn_count, 4, cudaMemcpyDeviceToHost, L->stream));
-    CU(cudaStreamSynchronize(L->stream));
+    CU(cudaMemcpyAsync(R.h_learn_count, R.d_learn_count, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
     const uint32_t learned = *R.h_learn_count;
     bool build = learned != R.built_count && R.used;
     if (R.bounded && build) {
       // the other lane's kernels may be running: only FREE slots are handed out here, to the keys learned since the last
       // reclaim point (LEARNED without a slot), in ascending address order
       std::vector<uint32_t> state(R.used), fresh;
-      CU(cudaMemcpyAsync(state.data(), R.d_state, (size_t)R.used * 4, cudaMemcpyDeviceToHost, L->stream));
-      CU(cudaStreamSynchronize(L->stream));
+      CU(cudaMemcpyAsync(state.data(), R.d_state, (size_t)R.used * 4, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
       for (uint32_t r = 0; r < R.used; r++)
         if (state[r] == IBFT_KEY_LEARNED && R.refs[r] > 0 && R.budget.table[r] == ibft::kNoTable) fresh.push_back(r);
       std::sort(fresh.begin(), fresh.end(), [&](uint32_t a, uint32_t b) { return memcmp(R.addr_of[a].b, R.addr_of[b].b, 20) < 0; });
@@ -2611,11 +2656,11 @@ static int refresh_key_tables_locked(ibft_engine* e, lane* L, uint32_t* n_ready_
         const uint32_t t = R.budget.take_free(r);
         if (t == ibft::kNoTable) break;
         if (!pool_reserve(R, t, &grew)) { R.budget.drop(r); break; }  // the pool cannot grow: builds stop at what it holds
-        CU(cudaMemcpyAsync(R.d_tab + r, &R.budget.table[r], 4, cudaMemcpyHostToDevice, L->stream));
+        CU(cudaMemcpyAsync(R.d_tab + r, &R.budget.table[r], 4, cudaMemcpyHostToDevice, st));
         assigned = true;
       }
-      if (grew) CU(cudaMemcpyAsync(R.d_chunks, R.chunks.data(), R.chunks.size() * sizeof(uint32_t*), cudaMemcpyHostToDevice, L->stream));
-      CU(cudaStreamSynchronize(L->stream));  // the host copies above read pageable memory that changes on the next call
+      if (grew) CU(cudaMemcpyAsync(R.d_chunks, R.chunks.data(), R.chunks.size() * sizeof(uint32_t*), cudaMemcpyHostToDevice, st));
+      CU(cudaStreamSynchronize(st));  // the host copies above read pageable memory that changes on the next call
       R.built_count = learned;
       build = assigned;
     }
@@ -2625,21 +2670,21 @@ static int refresh_key_tables_locked(ibft_engine* e, lane* L, uint32_t* n_ready_
       // before any refresh ran) gets its table built once for nothing -- 17 threads -- and is reset when it is reused.  A
       // bounded registry builds only the entries that hold a slot.
       const uint32_t* tab = R.bounded ? R.d_tab : nullptr;
-      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, L->stream>>>(R.d_state, tab, R.used, IBFT_KEY_LEARNED, IBFT_KEY_BUILDING);
-      k_build_keytabs<<<(uint32_t)(((size_t)R.used * IBFT_KEYTAB_POSITIONS + 63) / 64), 64, 0, L->stream>>>(R.d_state, R.d_key_xy,
+      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, st>>>(R.d_state, tab, R.used, IBFT_KEY_LEARNED, IBFT_KEY_BUILDING);
+      k_build_keytabs<<<(uint32_t)(((size_t)R.used * IBFT_KEYTAB_POSITIONS + 63) / 64), 64, 0, st>>>(R.d_state, R.d_key_xy,
                                                                                                           tab, R.d_chunks, R.used);
-      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, L->stream>>>(R.d_state, tab, R.used, IBFT_KEY_BUILDING, IBFT_KEY_READY);
+      k_keytabs_step<<<(R.used + 255) / 256, 256, 0, st>>>(R.d_state, tab, R.used, IBFT_KEY_BUILDING, IBFT_KEY_READY);
       R.build_due = false;
       e->launches += 3;
       CU(cudaGetLastError());
       R.built_count = learned;
       // the tables are complete before anybody can launch the next round on another stream
-      CU(cudaStreamSynchronize(L->stream));
+      CU(cudaStreamSynchronize(st));
     }
     if (n_ready_out && R.used) {
       std::vector<uint32_t> state(R.used);
-      CU(cudaMemcpyAsync(state.data(), R.d_state, (size_t)R.used * 4, cudaMemcpyDeviceToHost, L->stream));
-      CU(cudaStreamSynchronize(L->stream));
+      CU(cudaMemcpyAsync(state.data(), R.d_state, (size_t)R.used * 4, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
       for (const slot_host& s : e->slots)
         if (s.valid)
           for (uint32_t r : s.key_ref) total += state[r] != IBFT_KEY_UNKNOWN;
@@ -2648,6 +2693,10 @@ static int refresh_key_tables_locked(ibft_engine* e, lane* L, uint32_t* n_ready_
 #endif
   if (n_ready_out) *n_ready_out = total;
   return IBFT_OK;
+}
+static int refresh_key_tables_locked(ibft_engine* e, lane* L, uint32_t* n_ready_out) {
+  std::lock_guard<std::mutex> kl(e->keys_mu);
+  return refresh_key_tables_held(e, L->stream, n_ready_out);
 }
 extern "C" int ibft_refresh_key_tables(ibft_engine* e, uint32_t* n_keys_out) {
   if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
@@ -3079,7 +3128,8 @@ static int wait_locked(ibft_engine* e, lane* L) {
   }
   if (pc.n_groups) memcpy(pc.results_out, L->h_results, (size_t)pc.n_groups * sizeof(ibft_group_result));
   e->last_lane.store((int)(L - e->lanes));
-  if (e->p.flags & IBFT_FLAG_KEY_CACHE) return refresh_key_tables_locked(e, L, nullptr);  // new keys -> tables, for the next call
+  // new keys -> tables, for the next call (a multi-device engine's coordinator does it once it has shared the keys)
+  if ((e->p.flags & IBFT_FLAG_KEY_CACHE) && !e->coordinated) return refresh_key_tables_locked(e, L, nullptr);
   return IBFT_OK;
 }
 
@@ -3678,7 +3728,10 @@ extern "C" int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* w
 extern "C" int ibft_debug_op(ibft_engine* e, int op, const uint8_t* a, const uint8_t* b, const uint8_t* c, uint32_t n,
                              uint8_t* out, uint32_t out_stride) {
   e = diag_engine(e);
-  if (!e || !a || !out || n == 0 || (op == IBFT_DBG_RFC6979 && (!b || !c))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  if (!e || !a || !out || n == 0 || ((op == IBFT_DBG_RFC6979 || op == IBFT_DBG_KEY_ADDRESS) && (!b || !c))) {
+    set_err("null argument");
+    return IBFT_ERR_INVALID_ARG;
+  }
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
   CU(cudaSetDevice(e->p.device));
@@ -3750,6 +3803,14 @@ struct multi_engine {
   std::vector<uint8_t> last_status;
   uint32_t last_used = 0;
   std::vector<multi_table> tables;
+  // key sharing (IBFT_FLAG_KEY_CACHE; all empty otherwise), guarded by every device's keys_mu.  Per device: a stream for key
+  // upkeep (a call that ran on the lead alone holds no lane of the others), a scratch of 17 words per registry entry plus one
+  // (another device's state words, then its keys, then the adoption counter), and the value of its learn counter the last
+  // share step accounted for
+  std::vector<cudaStream_t> key_stream;
+  std::vector<uint32_t*> key_scratch;
+  std::vector<uint32_t> key_seen;
+  uint32_t* h_key_counts = nullptr;  // pinned, 2 words per device: learn counter, keys adopted
 };
 
 static int multi_refused(ibft_engine* e, const char* fn) {
@@ -3904,6 +3965,141 @@ static int multi_submit_locked(ibft_engine* E, int kind, uint32_t used, const ib
   return IBFT_OK;
 }
 
+// Key sharing.  Every device learns the keys of its own shards; after each host-buffer call the devices whose learn counter
+// moved since the last share step are the sources, and every other device adopts their keys: a peer copy of the source's state
+// and keys of the entries in use into the destination's scratch (with or without peer access, and on a repeated ordinal), then
+// k_adopt_peer_keys, which checks each key against the destination's own address of the entry.  Then every device builds the
+// tables of its new keys -- after the adoption, so that a bounded registry hands its free slots to the keys learned on any
+// device, in address order, as a single-device engine does.
+
+// every device's keys_mu, in device-list order (taken after any lane: nobody waits for a lane while holding one)
+struct multi_keys_lock {
+  std::vector<std::unique_lock<std::mutex>> lk;
+  explicit multi_keys_lock(multi_engine* M) { for (ibft_engine* s : M->subs) lk.emplace_back(s->keys_mu); }
+};
+// every lane of every device, device by device in list order, lanes in index order (the reclaim points)
+struct multi_all_lanes_lock {
+  std::vector<std::unique_lock<std::mutex>> lk;
+  explicit multi_all_lanes_lock(multi_engine* M) {
+    for (ibft_engine* s : M->subs)
+      for (lane& L : s->lanes) lk.emplace_back(L.mu);
+  }
+};
+
+// The adoption (caller holds every keys_mu).  Afterwards a device's baseline is its counter as read here plus the keys it
+// adopted: adopted keys are not sent back as new, and keys a concurrent call learns meanwhile go out with the next step.
+static int multi_adopt_keys(multi_engine* M) {
+#if IBFT_WC > 0
+  const uint32_t n_dev = (uint32_t)M->subs.size();
+  uint32_t* h = M->h_key_counts;
+  for (uint32_t k = 0; k < n_dev; k++) {
+    CU(cudaSetDevice(M->subs[k]->p.device));
+    CU(cudaMemcpyAsync(h + 2 * k, M->subs[k]->reg.d_learn_count, 4, cudaMemcpyDeviceToHost, M->key_stream[k]));
+  }
+  std::vector<uint32_t> src;
+  for (uint32_t k = 0; k < n_dev; k++) {
+    CU(cudaSetDevice(M->subs[k]->p.device));
+    CU(cudaStreamSynchronize(M->key_stream[k]));
+    if (h[2 * k] != M->key_seen[k]) src.push_back(k);
+  }
+  if (src.empty()) return IBFT_OK;
+  for (uint32_t d = 0; d < n_dev; d++) {
+    ibft_engine* D = M->subs[d];
+    key_registry& R = D->reg;
+    cudaStream_t ks = M->key_stream[d];
+    uint32_t* sc = M->key_scratch[d];
+    uint32_t* adopted = sc + 17 * (size_t)R.capacity;
+    h[2 * d + 1] = 0;
+    CU(cudaSetDevice(D->p.device));
+    CU(cudaMemsetAsync(adopted, 0, 4, ks));
+    for (uint32_t k : src) {
+      const ibft_engine* S = M->subs[k];
+      const uint32_t n = std::min(S->reg.used, R.used);
+      if (k == d || n == 0) continue;
+      // state first: a key the state copy shows as learned was written before that state (learn_key's fence)
+      CU(cudaMemcpyPeerAsync(sc, D->p.device, S->reg.d_state, S->p.device, (size_t)n * 4, ks));
+      CU(cudaMemcpyPeerAsync(sc + R.capacity, D->p.device, S->reg.d_key_xy, S->p.device, (size_t)n * 64, ks));
+      k_adopt_peer_keys<<<(n + 255) / 256, 256, 0, ks>>>(sc, sc + R.capacity, n, R.d_state, R.d_key_xy, R.d_addr, R.d_learn_count,
+                                                        adopted);
+      D->launches++;
+      CU(cudaGetLastError());
+    }
+    CU(cudaMemcpyAsync(h + 2 * d + 1, adopted, 4, cudaMemcpyDeviceToHost, ks));
+  }
+  for (uint32_t d = 0; d < n_dev; d++) {
+    CU(cudaSetDevice(M->subs[d]->p.device));
+    CU(cudaStreamSynchronize(M->key_stream[d]));
+    M->key_seen[d] = h[2 * d] + h[2 * d + 1];
+  }
+#else
+  (void)M;
+#endif
+  return IBFT_OK;
+}
+
+// every device builds the tables of the keys it learned or adopted (caller holds every keys_mu); a device with nothing new
+// since its last refresh costs nothing
+static int multi_refresh_keys(multi_engine* M) {
+  for (uint32_t k = 0; k < M->subs.size(); k++) {
+    ibft_engine* s = M->subs[k];
+    if (M->key_seen[k] == s->reg.built_count && !(s->reg.bounded && s->reg.build_due)) continue;
+    int rc = refresh_key_tables_held(s, M->key_stream[k], nullptr);
+    if (rc != IBFT_OK) return rc;
+  }
+  return IBFT_OK;
+}
+
+// the share step that closes every host-buffer call
+static int multi_share_keys(multi_engine* M) {
+  if (M->key_stream.empty()) return IBFT_OK;
+  multi_keys_lock kl(M);
+  int rc = multi_adopt_keys(M);
+  return rc != IBFT_OK ? rc : multi_refresh_keys(M);
+}
+
+// A reclaim point of a bounded registry (caller holds every lane of every device, devices drained): every device takes the used
+// flags of all, matched by address, so that every budget ranks the keys by their use on any device.  The flags only rank keys:
+// no device check is needed.
+static int multi_merge_used_flags(multi_engine* M) {
+#if IBFT_WC > 0
+  if (M->key_stream.empty() || !M->subs[0]->reg.bounded) return IBFT_OK;
+  std::unordered_set<addr20, addr20_hash> hot;
+  std::vector<std::vector<uint8_t>> used(M->subs.size());
+  for (size_t k = 0; k < M->subs.size(); k++) {
+    const key_registry& R = M->subs[k]->reg;
+    used[k].assign(R.used, 0);
+    CU(cudaSetDevice(M->subs[k]->p.device));
+    if (R.used) CU(cudaMemcpy(used[k].data(), R.d_used, R.used, cudaMemcpyDeviceToHost));
+    for (const auto& kv : R.by_addr)
+      if (used[k][kv.second]) hot.insert(kv.first);
+  }
+  for (size_t k = 0; k < M->subs.size(); k++) {
+    const key_registry& R = M->subs[k]->reg;
+    for (const auto& kv : R.by_addr) used[k][kv.second] |= hot.count(kv.first) ? 1 : 0;
+    CU(cudaSetDevice(M->subs[k]->p.device));
+    if (R.used) CU(cudaMemcpy(R.d_used, used[k].data(), R.used, cudaMemcpyHostToDevice));
+  }
+#else
+  (void)M;
+#endif
+  return IBFT_OK;
+}
+
+// before the sub-engines' own reclaim points (ibft_set_validators, ibft_set_key_table_budget): merge the used flags.  With a
+// call pending nothing is merged: the sub-engines refuse the call themselves.
+static int multi_before_reclaim(multi_engine* M) {
+  if (M->key_stream.empty() || !M->subs[0]->reg.bounded) return IBFT_OK;
+  multi_all_lanes_lock lk(M);
+  for (ibft_engine* s : M->subs)
+    for (lane& L : s->lanes)
+      if (L.pending.active) return IBFT_OK;
+  for (ibft_engine* s : M->subs) {
+    CU(cudaSetDevice(s->p.device));
+    CU(cudaDeviceSynchronize());
+  }
+  return multi_merge_used_flags(M);
+}
+
 // Waits for a call of multi_submit_locked (same lanes held) and, once every device has succeeded, writes the caller's buffers.
 static int multi_wait_locked(ibft_engine* E, int kind, multi_call& mc, uint8_t* status_out, uint32_t* voted_out,
                              uint32_t voted_stride_words) {
@@ -3953,6 +4149,9 @@ static int multi_wait_locked(ibft_engine* E, int kind, multi_call& mc, uint8_t* 
     M->last_used = mc.used;
     if (status_out && mc.n) memcpy(status_out, M->last_status.data(), mc.n);
   }
+  // new keys -> every device, then tables, for the next call; a failure here is reported as a single engine reports its refresh
+  int rc = multi_share_keys(M);
+  if (rc != IBFT_OK) return rc;
   return copy_voted(lead, L0, mc.n_groups, mc.results_out != nullptr, voted_out, voted_stride_words);
 }
 
@@ -4103,8 +4302,10 @@ static int multi_set_validators(ibft_engine* E, uint32_t table_slot, uint64_t he
                                 uint32_t n) {
   multi_engine* M = E->multi;
   std::unique_lock<std::shared_mutex> st(M->state_mu);
+  int rc = multi_before_reclaim(M);
+  if (rc != IBFT_OK) return rc;
   // the lead checks every argument on the host before it touches its device: a refused table leaves every device as it was
-  int rc = ibft_set_validators(M->subs[0], table_slot, height, addrs, powers_be, n);
+  rc = ibft_set_validators(M->subs[0], table_slot, height, addrs, powers_be, n);
   if (rc != IBFT_OK) return rc;
   for (size_t k = 1; k < M->subs.size(); k++) {
     rc = ibft_set_validators(M->subs[k], table_slot, height, addrs, powers_be, n);
@@ -4152,8 +4353,29 @@ static int known_members(ibft_engine* e, std::vector<std::vector<uint8_t>>& know
 static int multi_refresh_key_tables(ibft_engine* E, uint32_t* n_keys_out) {
   multi_engine* M = E->multi;
   std::unique_lock<std::shared_mutex> st(M->state_mu);
-  for (ibft_engine* s : M->subs) {
-    int rc = ibft_refresh_key_tables(s, nullptr);
+  if (M->key_stream.empty()) {
+    for (ibft_engine* s : M->subs) {
+      int rc = ibft_refresh_key_tables(s, nullptr);
+      if (rc != IBFT_OK) return rc;
+    }
+  } else {
+    // adopt first, then (bounded) the reclaim point on every device with the merged flags, then the tables
+    multi_all_lanes_lock lk(M);
+    for (ibft_engine* s : M->subs)
+      if (s->lanes[0].pending.active) { set_err("a submitted call is still pending"); return IBFT_ERR_INVALID_ARG; }
+    multi_keys_lock kl(M);
+    int rc = multi_adopt_keys(M);
+#if IBFT_WC > 0
+    if (rc == IBFT_OK && M->subs[0]->reg.bounded) {
+      for (ibft_engine* s : M->subs) {
+        CU(cudaSetDevice(s->p.device));
+        CU(cudaDeviceSynchronize());
+      }
+      rc = multi_merge_used_flags(M);
+      for (size_t k = 0; k < M->subs.size() && rc == IBFT_OK; k++) rc = budget_reclaim(M->subs[k], M->subs[k]->reg.budget.max_tables);
+    }
+#endif
+    if (rc == IBFT_OK) rc = multi_refresh_keys(M);
     if (rc != IBFT_OK) return rc;
   }
   if (!n_keys_out) return IBFT_OK;
@@ -4173,8 +4395,10 @@ static int multi_refresh_key_tables(ibft_engine* E, uint32_t* n_keys_out) {
 static int multi_set_key_table_budget(ibft_engine* E, uint32_t max_tables) {
   multi_engine* M = E->multi;
   std::unique_lock<std::shared_mutex> st(M->state_mu);
+  int rc = multi_before_reclaim(M);
+  if (rc != IBFT_OK) return rc;
   for (ibft_engine* s : M->subs) {
-    int rc = ibft_set_key_table_budget(s, max_tables);
+    rc = ibft_set_key_table_budget(s, max_tables);
     if (rc != IBFT_OK) return rc;
   }
   return IBFT_OK;
@@ -4201,6 +4425,13 @@ static void multi_destroy(ibft_engine* E) {
       if (M->merged[k]) cudaEventDestroy(M->merged[k]);
     }
   }
+  for (size_t k = 0; k < M->key_stream.size(); k++) {
+    cudaSetDevice(M->subs[k]->p.device);
+    cudaDeviceSynchronize();
+    if (M->key_stream[k]) cudaStreamDestroy(M->key_stream[k]);
+    cudaFree(M->key_scratch[k]);
+  }
+  cudaFreeHost(M->h_key_counts);
   for (ibft_engine* s : M->subs) engine_free(s);
   for (ibft_engine* v : M->views) delete v;
   delete M;
@@ -4247,6 +4478,26 @@ extern "C" int ibft_engine_create_multi(const ibft_engine_params* params, const 
     multi_destroy(E);
     return IBFT_ERR_CUDA;
   }
+  for (ibft_engine* s : M->subs) s->coordinated = true;
+#if IBFT_WC > 0
+  if ((E->p.flags & IBFT_FLAG_KEY_CACHE) && lead->reg.d_state) {
+    const size_t scratch = (17 * (size_t)lead->reg.capacity + 1) * 4;
+    M->key_stream.assign(n_devices, nullptr);
+    M->key_scratch.assign(n_devices, nullptr);
+    M->key_seen.assign(n_devices, 0);
+    ce = cudaHostAlloc(&M->h_key_counts, 8 * (size_t)n_devices, cudaHostAllocPortable);
+    for (uint32_t k = 0; k < n_devices && ce == cudaSuccess; k++) {
+      ce = cudaSetDevice(M->subs[k]->p.device);
+      if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&M->key_stream[k], cudaStreamNonBlocking);
+      if (ce == cudaSuccess) ce = cudaMalloc(&M->key_scratch[k], scratch);
+    }
+    if (ce != cudaSuccess) {
+      set_err("key sharing buffers: %s", cudaGetErrorString(ce));
+      multi_destroy(E);
+      return ce == cudaErrorMemoryAllocation ? IBFT_ERR_CAPACITY : IBFT_ERR_CUDA;
+    }
+  }
+#endif
   *out = E;
   return IBFT_OK;
 }

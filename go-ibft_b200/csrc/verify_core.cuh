@@ -524,6 +524,24 @@ IBFT_HD bool ecrecover_address(const uint8_t* r_be, const uint8_t* s_be, uint8_t
   return ecrecover_address_x(exec_serial{}, r_be, s_be, v, z_be, G, T, addr20, key_out);
 }
 
+// Key registry: whether (x, y) may be the key of the entry of address addr20.  A known-key accept stands for "recovery yields
+// exactly this key", so the signer it names is the entry's address; a key taken from anywhere but a recovery of this engine
+// (another device's registry) has to show that it hashes to that address.  Both coordinates must be in the limb form a
+// recovery stores (fully reduced, < p), the point on the curve, and its address addr20.
+IBFT_HD bool key_matches_address(const fe& x, const fe& y, const uint8_t* addr20) {
+  const fe xn = fe_normalize(x), yn = fe_normalize(y);
+  uint32_t d = 0;
+#pragma unroll
+  for (int i = 0; i < 8; i++) d |= (xn.v[i] ^ x.v[i]) | (yn.v[i] ^ y.v[i]);
+  if (d != 0) return false;
+  if (!fe_equal(fe_sqr(y), fe_add(fe_mul(fe_sqr(x), x), fe_from_u32(7)))) return false;
+  uint8_t a[20];
+  keccak256_xy_address(x, y, a);
+#pragma unroll
+  for (int i = 0; i < 20; i++) d |= (uint32_t)(a[i] ^ addr20[i]);
+  return d == 0;
+}
+
 // Why one item is rejected (ibft_explain_batch): the recover path's decision, step by step, as an IBFT_REASON_* code.  The steps
 // run in the order the verify kernels decide, so the first failing one is the reason.  member(group, signer) is the validator-set
 // test of the kernels (true for a group without a table).  grouped: the call has groups (without, no item is ever of an unknown

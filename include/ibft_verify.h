@@ -168,8 +168,8 @@ typedef struct ibft_engine_params {
  * table (1.39 GB for a 10,000-validator set, however many resident heights list it).  A key learned through any table serves
  * every table that lists the address, including tables set earlier, so a chain that moves to the next height with (mostly) the
  * same validators never recovers their signatures again.  An entry is retired when no resident table lists its address any
- * more: a validator that leaves every table and later rejoins is learned again.  The engine reserves the state and key of
- * (max_table_slots + 1) x max_validators entries at creation (68 bytes each) and allocates comb tables in chunks of 256
+ * more: a validator that leaves every table and later rejoins is learned again.  The engine reserves the state, key and address
+ * of (max_table_slots + 1) x max_validators entries at creation (88 bytes each) and allocates comb tables in chunks of 256
  * entries (34 MiB) as new addresses arrive; ibft_set_validators fails with IBFT_ERR_CAPACITY when the registry cannot grow to
  * hold its table's new addresses, and the slot keeps its previous table.  ibft_set_key_table_budget bounds the comb tables
  * instead: the engine then keeps at most that many, for the keys used most recently, never allocates them in
@@ -225,9 +225,15 @@ int ibft_engine_device_info(ibft_engine* e, ibft_device_info* out);
  *   ibft_keccak256_batch,          rows split the same way; the output bytes are a single-device call's.
  *   ibft_proposal_hash_batch,
  *   ibft_sign_batch, _rfc6979
- *   ibft_refresh_key_tables,       applied to every device (a budget bounds each device's pool).  Key registries stay per device:
- *   ibft_set_key_table_budget,     each learns from the signatures of its shards, with identical verdicts either way.
- *   ibft_set_recover_path          *n_keys_out counts (table, member) pairs whose key is known on at least one device.
+ *   ibft_refresh_key_tables,       applied to every device (a budget bounds each device's pool).  One set of known keys: every
+ *   ibft_set_key_table_budget,     host-buffer call (one on the lead alone included) ends with a share step, in which every
+ *   ibft_set_recover_path          device adopts the keys the others learned since the last step -- each key checked on the
+ *                                  device to be reduced, on the curve and hashing to the entry's address -- and then builds its
+ *                                  tables; ibft_refresh_key_tables runs it too.  So every device knows what a single-device
+ *                                  engine fed the same calls knows, and under a budget every reclaim point ranks the keys by
+ *                                  their use on any device, so that all devices keep the same tables.  Verdicts are identical
+ *                                  either way.  *n_keys_out counts (table, member) pairs whose key is known on at least one
+ *                                  device.
  *   ibft_engine_launch_count       the sum over the devices.
  *   ibft_engine_device_info,       the lead answers; ibft_engine_sub reaches the others.
  *   ibft_probe_int_peak, ibft_debug_*
@@ -488,6 +494,10 @@ int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* wide_mac_per
                                     * || 17 int16 (little-endian) 8-bit digits at 72 */
 #define IBFT_DBG_RFC6979 23        /* out = raw nonce candidate c (before any range check) of ibft_sign_batch_rfc6979 for the key a
                                     * and the digest b; c = the last byte of the 64-byte c operand */
+#define IBFT_DBG_KEY_ADDRESS 24    /* out[0] = 1 when the key (x = a, y = b, taken as given: no reduction) may stand in the key
+                                    * registry entry of the address in the first 20 bytes of c (x, y < p, on the curve, hashing
+                                    * to the address), else 0: the check of a key one device of a multi-device engine adopts
+                                    * from another */
 /* Generator comb tables (builds with IBFT_WC > 0): *wc = window (0 when absent), *entries = entries of one comb position;
  * copies `count` 64-byte entries (x, y as 8 little-endian words each) starting at `first`, positions laid out one after the
  * other: entry p * entries + d1 * (2^wc + 1) + d2 + 2^(wc-1) holds (d1 + d2*lambda) * 2^(wc*p) * G, p = 0..16 (position 0 is
