@@ -2528,6 +2528,14 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
     int c = memcmp(addrs + 20 * (size_t)a, addrs + 20 * (size_t)b, 20);
     return c != 0 ? c < 0 : a < b;
   });
+  // go-ibft keys voting power by address (a map: core/validator_manager.go), so a table cannot list an address twice.  A
+  // duplicate would count its power twice in the quorum and credit its votes to whichever copy the search meets first: refuse it
+  // before anything changes, so the slot keeps its previous table and the key registry its entries
+  for (uint32_t r = 1; r < n; r++)
+    if (memcmp(addrs + 20 * (size_t)order[r - 1], addrs + 20 * (size_t)order[r], 20) == 0) {
+      set_err("validator table lists one address twice: validators %u and %u", order[r - 1], order[r]);
+      return IBFT_ERR_INVALID_ARG;
+    }
   std::vector<uint32_t> keys((size_t)n * 6);
   for (uint32_t r = 0; r < n; r++) {
     const uint8_t* a = addrs + 20 * (size_t)order[r];

@@ -108,7 +108,9 @@ ibfthost_ctx* ibfthost_create_multi(const ibfthost_callbacks* cbs, const uint8_t
 void ibfthost_destroy(ibfthost_ctx* c) { delete c; }
 
 // ValidatorManager.Init(height) with the embedder's GetVotingPowers result: n addresses (concatenated, lens[i] bytes each)
-// and n 32-byte big-endian powers (NULL => 1).  Returns 0 ok, 5 = errVotingPowerNotCorrect, 3 = device error.
+// and n 32-byte big-endian powers (NULL => 1).  Returns 0 ok, 5 = errVotingPowerNotCorrect, 1 = an address listed twice
+// (GetVotingPowers returns a map, which cannot hold one twice), or the engine's status when it refuses the table.  A refused
+// table changes nothing: the context keeps its previous table.
 int ibfthost_set_validators(ibfthost_ctx* c, uint64_t height, const uint8_t* addrs, const uint32_t* lens, const uint8_t* powers_be, uint32_t n) {
   std::vector<Bytes> order;
   std::vector<u320> powers;
@@ -118,8 +120,22 @@ int ibfthost_set_validators(ibfthost_ctx* c, uint64_t height, const uint8_t* add
     off += lens[i];
     powers.push_back(powers_be ? u320::from_be32(powers_be + 32 * (size_t)i) : u320::from_u64(1));
   }
+  // duplicates: a GPU context leaves the 20-byte addresses to the engine (GpuVerifier::SetValidators returns false); the
+  // others -- every address of a callback context -- are checked here
+  std::vector<Bytes> host_only;
+  for (auto& a : order)
+    if (!c->gpu || a.size() != 20) host_only.push_back(a);
+  std::sort(host_only.begin(), host_only.end());
+  if (std::adjacent_find(host_only.begin(), host_only.end()) != host_only.end()) return IBFT_ERR_INVALID_ARG;
+  u320 total;
+  for (auto& p : powers) total.add(p);
+  if (total.is_zero()) return IBFT_ERR_VOTING_POWER;
+  // the device table first: when the engine refuses it, the host ValidatorManager keeps its previous table too
+  if (c->gpu && !c->gpu->SetValidators(height, order, powers)) {
+    int rc = c->gpu->last_set_status();
+    return rc != IBFT_OK ? rc : IBFT_ERR_CUDA;
+  }
   if (!c->vm.SetVotingPowers(order, powers)) return IBFT_ERR_VOTING_POWER;
-  if (c->gpu && !c->gpu->SetValidators(height, order, powers)) return IBFT_ERR_CUDA;
   return IBFT_OK;
 }
 

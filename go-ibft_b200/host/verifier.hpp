@@ -113,6 +113,10 @@ class GpuVerifier : public Verifier {
     return error_;
   }
   ibft_engine* engine() { return engine_; }
+  int last_set_status() const {
+    std::lock_guard<std::mutex> lk(state_mu_);
+    return last_rc_;
+  }
 
   // ValidatorBackend.GetVotingPowers(height) pushed to the device (validator_manager.go:50-57): the table of `height`
   // occupies slot (height mod max_table_slots).  Addresses that are not 20 bytes can never equal a recovered signer and are
@@ -127,17 +131,27 @@ class GpuVerifier : public Verifier {
         for (int j = 7; j >= 0; j--) p.push_back((uint8_t)(powers[i].l[k] >> (8 * j)));
     }
     uint32_t slot = (uint32_t)(height % params_.max_table_slots);
+    bool had_old = false;
+    uint64_t old_height = 0;
     {
       // the slot stops answering for its old height BEFORE the engine swaps the table
       std::lock_guard<std::mutex> lk(state_mu_);
+      auto it = slot_height_.find(slot);
+      if (it != slot_height_.end()) { had_old = true; old_height = it->second; }
       slot_height_.erase(slot);
       epoch_++;
       cache_.clear();
     }
     int rc = ibft_set_validators(engine_, slot, height, a.data(), p.data(), (uint32_t)(a.size() / 20));
     std::lock_guard<std::mutex> lk(state_mu_);
+    last_rc_ = rc;
     if (rc != IBFT_OK) {
       error_ = ibft_last_error();
+      // a refused table (an address listed twice, zero power, over capacity) leaves the engine's slot as it was: it answers for
+      // its old height again when the engine still holds that height there
+      uint64_t q[5], h = 0;
+      uint32_t n = 0;
+      if (had_old && ibft_get_quorum(engine_, slot, q, &h, &n) == IBFT_OK && h == old_height) slot_height_[slot] = old_height;
       return false;
     }
     slot_height_[slot] = height;
@@ -322,6 +336,7 @@ class GpuVerifier : public Verifier {
   ibft_engine_params params_{};
   ibft_engine* engine_ = nullptr;
   std::string error_;
+  int last_rc_ = IBFT_OK;  // status of the last ibft_set_validators call
   std::unordered_map<Bytes, bool> cache_;
   std::unordered_map<Bytes, Bytes> hash_cache_;
   std::map<uint32_t, uint64_t> slot_height_;

@@ -253,7 +253,10 @@ int ibft_engine_sub(ibft_engine* e, uint32_t k, ibft_engine** sub_out);
 /* Replaces ValidatorManager.Init -> Backend.GetVotingPowers(height) (core/validator_manager.go:50-74,
  * core/backend.go via ValidatorBackend :17-20).  addrs: n x 20 bytes in validator-index order;
  * powers_be: n x 32 bytes big-endian (NULL => unit power).  Computes and stores the quorum threshold
- * floor(2*total/3)+1.  Returns IBFT_ERR_VOTING_POWER when the total is zero. */
+ * floor(2*total/3)+1.  Returns IBFT_ERR_VOTING_POWER when the total is zero.  Every address may appear once: go-ibft keys
+ * voting power by address (ValidatorManager.setCurrentVotingPower takes a map[string]*big.Int, core/validator_manager.go:61-74),
+ * so a table that lists an address twice has no go-ibft meaning and is refused with IBFT_ERR_INVALID_ARG (the error names both
+ * validator indices) before anything changes: the slot keeps its previous table and the key registry its entries. */
 int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t height, const uint8_t* addrs,
                         const uint8_t* powers_be, uint32_t n);
 /* Little-endian 320-bit quorum threshold of a slot (for the host-side quorum mirror). */
