@@ -29,6 +29,7 @@
 #include "../../include/ibft_verify.h"
 #include "verify_core.cuh"
 #include "debug_arith.cuh"
+#include "key_share.cuh"
 #include "key_budget.hpp"
 #include "shard_plan.hpp"
 
@@ -72,11 +73,7 @@ struct slot_dev {
   const uint32_t* key_tab;     // per entry: its table slot, or IBFT_KEY_NO_TAB (nullptr: entry r's table is slot r)
   uint8_t* key_used;           // per entry: set by the known-key pass on every lookup; read and cleared at reclaim points
 };
-#define IBFT_KEY_UNKNOWN 0u
-#define IBFT_KEY_LEARNED 1u
-#define IBFT_KEY_READY 2u
-#define IBFT_KEY_BUILDING 3u  // claimed by a table-build pass (refresh_key_tables_locked)
-#define IBFT_KEY_EVICTED 4u   // bounded registry: key known, no table slot (every kernel treats it as LEARNED)
+// entry states IBFT_KEY_UNKNOWN / _LEARNED / _READY / _BUILDING / _EVICTED: key_share.cuh
 #define IBFT_KEY_NO_TAB 0xFFFFFFFFu
 #define IBFT_KEY_CHUNK 256u   // registry entries per comb-table chunk (34 MiB): the pool grows by whole chunks, never by copying
 #define IBFT_KEY_REF_FRESH 0x80000000u  // key_ref mark of an entry new to its address (k_adopt_entries); entries are < 2^31
@@ -1531,6 +1528,101 @@ k_adopt_peer_keys(const uint32_t* __restrict__ src_state, const uint32_t* __rest
     atomicAdd(adopted, 1u);
   }
 }
+
+// Key sharing between engines of separate processes (ibft_key_share_*; block format and decisions in key_share.cuh).
+// ibft_set_validators: an entry given to another address forgets that it was exported (runs before k_adopt_entries clears the
+// marks of the new table's key_ref).
+__global__ void __launch_bounds__(256) k_key_share_forget(const uint32_t* __restrict__ key_ref, uint32_t n, uint32_t* __restrict__ shared) {
+  const uint32_t v = blockIdx.x * 256 + threadIdx.x;
+  if (v < n && (key_ref[v] & IBFT_KEY_REF_FRESH)) shared[key_ref[v] & ~IBFT_KEY_REF_FRESH] = 0;
+}
+// Export: one CTA walks entries [0, n_entries) a thousand at a time and writes a record for each exportable one, in ascending
+// entry order (a block-wide prefix count gives every record its place), until the block holds IBFT_KEY_SHARE_RECORDS.  The state
+// is read before the key: learn_key stores the key, fences, then publishes the state.
+__global__ void __launch_bounds__(1024) k_key_export(const uint32_t* state, uint32_t* __restrict__ shared, const uint32_t* key_xy,
+                                                     const uint8_t* __restrict__ addr, uint32_t n_entries, uint32_t* __restrict__ block) {
+  __shared__ uint32_t s_warp[32];
+  __shared__ uint32_t s_total;
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  uint32_t base_out = 0;
+  for (uint32_t base = 0; base < n_entries && base_out < IBFT_KEY_SHARE_RECORDS; base += 1024) {
+    const uint32_t r = base + tid;
+    const bool pick = r < n_entries && key_share_exportable(*(volatile const uint32_t*)&state[r], shared[r]);
+    const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, pick);
+    if (lane == 0) s_warp[warp] = __popc(ballot);
+    __syncthreads();
+    if (warp == 0) {
+      const uint32_t c = s_warp[lane];
+      uint32_t incl = c;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d);
+        if (lane >= (uint32_t)d) incl += t;
+      }
+      s_warp[lane] = incl - c;
+      if (lane == 31) s_total = incl;
+    }
+    __syncthreads();
+    const uint32_t pos = base_out + s_warp[warp] + __popc(ballot & ((1u << lane) - 1u));
+    if (pick && pos < IBFT_KEY_SHARE_RECORDS) {
+      __threadfence();
+      uint32_t xy[16];
+#pragma unroll
+      for (int i = 0; i < 16; i++) xy[i] = key_xy[16 * (size_t)r + i];
+      key_share_put(block + 1 + IBFT_KEY_SHARE_RECORD_WORDS * pos, addr + 20 * (size_t)r, xy);
+      shared[r] = 1;
+    }
+    base_out = min(IBFT_KEY_SHARE_RECORDS, base_out + s_total);
+    __syncthreads();  // s_warp / s_total are rewritten by the next step
+  }
+  if (tid == 0) block[0] = base_out;
+}
+struct key_share_parts {
+  const uint32_t* part[IBFT_KEY_SHARE_MAX_PARTS];
+};
+// Adopt: one thread per record slot of every block but the engine's own (blockIdx.y = block).  The blocks may lie in peer memory
+// a peer wrote before publishing a flag this device has seen, so they are read with system-scope loads.  The write of an adopted
+// key is learn_key's (first writer wins, every writer stores the same key), so the kernel may run beside the verify kernels;
+// the entry is marked exported, so the key is never sent back.  counts (may be nullptr): { adopted, refused }.
+__global__ void __launch_bounds__(256)
+k_key_adopt(key_share_parts parts, uint32_t self_part, const slot_dev* __restrict__ slots, uint32_t n_slots, uint32_t* state,
+            uint32_t* key_xy, const uint8_t* __restrict__ addr, uint32_t* __restrict__ shared, uint32_t* learn_count,
+            uint32_t* __restrict__ counts) {
+  if (blockIdx.y == self_part) return;
+  const uint32_t* blk = parts.part[blockIdx.y];
+  const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+  const uint32_t count = ld_relaxed_sys(blk);
+  if (count > IBFT_KEY_SHARE_RECORDS) {
+    if (i == 0 && counts != nullptr) atomicAdd(&counts[1], 1u);
+    return;
+  }
+  if (i >= count) return;
+  uint32_t rec[IBFT_KEY_SHARE_RECORD_WORDS];
+#pragma unroll
+  for (int k = 0; k < (int)IBFT_KEY_SHARE_RECORD_WORDS; k++) rec[k] = ld_relaxed_sys(blk + 1 + IBFT_KEY_SHARE_RECORD_WORDS * i + k);
+  auto lookup = [&](uint32_t s, const uint8_t* a) -> int {
+    const slot_dev& sd = slots[s];
+    if (!sd.valid || sd.key_ref == nullptr) return -1;
+    const int v = lookup_validator(sd, a);
+    return v < 0 ? -1 : (int)sd.key_ref[v];
+  };
+  uint32_t r = 0;
+  fe x, y;
+  const uint32_t d = key_share_decide(rec, n_slots, lookup, state, addr, &r, &x, &y);
+  if (d == IBFT_KEY_SHARE_REFUSE && counts != nullptr) atomicAdd(&counts[1], 1u);
+  if (d != IBFT_KEY_SHARE_ADOPT) return;
+#pragma unroll
+  for (int k = 0; k < 8; k++) {
+    key_xy[16 * (size_t)r + k] = x.v[k];
+    key_xy[16 * (size_t)r + 8 + k] = y.v[k];
+  }
+  __threadfence();
+  if (atomicCAS(&state[r], IBFT_KEY_UNKNOWN, IBFT_KEY_LEARNED) == IBFT_KEY_UNKNOWN) {
+    shared[r] = 1;
+    atomicAdd(learn_count, 1u);
+    if (counts != nullptr) atomicAdd(&counts[0], 1u);
+  }
+}
 #endif
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1760,6 +1852,9 @@ struct key_registry {
   uint32_t* d_tab = nullptr;             // capacity words
   uint8_t* d_used = nullptr;             // capacity bytes: used flags of the known-key pass
   bool build_due = false;                // entries admitted at the last reclaim point wait for the next refresh
+  // Key sharing between engines (ibft_key_share_*; allocated by the first such call): per entry, 1 once its key was exported
+  // or adopted (key_share_exportable)
+  uint32_t* d_shared = nullptr;          // capacity words
 };
 
 struct pending_call {
@@ -1991,7 +2086,7 @@ static void engine_free(ibft_engine* e) {
   for (auto& L : e->lanes) lane_free(&L);
   cudaFree(e->d_ctable);
   for (auto c : e->reg.chunks) cudaFree(c);
-  cudaFree(e->reg.d_tab); cudaFree(e->reg.d_used);
+  cudaFree(e->reg.d_tab); cudaFree(e->reg.d_used); cudaFree(e->reg.d_shared);
   cudaFree(e->reg.d_state); cudaFree(e->reg.d_key_xy); cudaFree(e->reg.d_addr); cudaFree(e->reg.d_chunks); cudaFree(e->reg.d_learn_count);
   cudaFreeHost(e->reg.h_learn_count);
   cudaFree(e->d_slots);
@@ -2588,6 +2683,11 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
     static_assert(sizeof(addr20) == 20, "addr_of is uploaded as packed 20-byte addresses");
     if (ce == cudaSuccess && adopt)  // the others of [lo, hi) hold their address already
       ce = cudaMemcpy(e->reg.d_addr + 20 * (size_t)lo, e->reg.addr_of[lo].b, 20 * (size_t)(hi - lo), cudaMemcpyHostToDevice);
+    if (ce == cudaSuccess && adopt && e->reg.d_shared) {
+      k_key_share_forget<<<(n + 255) / 256, 256>>>(s.d_key_ref, n, e->reg.d_shared);
+      e->launches++;
+      ce = cudaGetLastError();
+    }
     if (ce == cudaSuccess && adopt) {
       k_adopt_entries<<<(n + 255) / 256, 256>>>(s.d_key_ref, n, e->reg.d_state, e->reg.bounded ? e->reg.d_tab : nullptr);
       e->launches++;
@@ -2744,6 +2844,79 @@ extern "C" int ibft_set_key_table_budget(ibft_engine* e, uint32_t max_tables) {
   return budget_reclaim(e, std::min(max_tables, e->reg.capacity));
 #else
   (void)max_tables;
+  set_err("library built without a key registry");
+  return IBFT_ERR_INVALID_ARG;
+#endif
+}
+
+// Key sharing between engines of separate processes (include/ibft_verify.h).  Both device calls hold lane 0 while they launch:
+// ibft_set_validators, which changes the tables and the entries' addresses, takes every lane and drains the device first.
+extern "C" int ibft_key_share_words(ibft_engine* e, uint32_t* words_out) {
+  if (!e || !words_out) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  *words_out = IBFT_KEY_SHARE_WORDS;
+  return IBFT_OK;
+}
+// the checks both calls share, and the export marks (zero: nothing exported yet), allocated by the first call; caller holds lane 0
+static int key_share_begin(ibft_engine* e) {
+  if (!(e->p.flags & IBFT_FLAG_KEY_CACHE) || !e->reg.d_state || IBFT_WC == 0) { set_err("engine has no key registry"); return IBFT_ERR_INVALID_ARG; }
+  if (e->lanes[0].pending.active) { set_err("a submitted call is still pending"); return IBFT_ERR_INVALID_ARG; }
+  CU(cudaSetDevice(e->p.device));
+  if (!e->reg.d_shared) {
+    uint32_t* d = nullptr;
+    CU(cudaMalloc(&d, (size_t)e->reg.capacity * 4));
+    if (cudaMemset(d, 0, (size_t)e->reg.capacity * 4) != cudaSuccess) { cudaFree(d); CU(cudaGetLastError()); }
+    e->reg.d_shared = d;
+  }
+  return IBFT_OK;
+}
+extern "C" int ibft_key_share_export_device(ibft_engine* e, void* d_block, void* stream) {
+  IBFT_REFUSE_MULTI(e);
+  if (!e || !d_block) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+#if IBFT_WC > 0
+  lane* L = &e->lanes[0];
+  std::lock_guard<std::mutex> lk(L->mu);
+  int rc = key_share_begin(e);
+  if (rc != IBFT_OK) return rc;
+  const key_registry& R = e->reg;
+  k_key_export<<<1, 1024, 0, stream ? (cudaStream_t)stream : L->stream>>>(R.d_state, R.d_shared, R.d_key_xy, R.d_addr, R.used,
+                                                                          (uint32_t*)d_block);
+  e->launches++;
+  CU(cudaGetLastError());
+  return IBFT_OK;
+#else
+  (void)stream;
+  set_err("library built without a key registry");
+  return IBFT_ERR_INVALID_ARG;
+#endif
+}
+extern "C" int ibft_key_share_adopt_device(ibft_engine* e, const uint64_t* part_ptrs, uint32_t n_parts, uint32_t self_part,
+                                           void* d_counts_out, void* stream) {
+  IBFT_REFUSE_MULTI(e);
+  if (!e || !part_ptrs || n_parts == 0 || n_parts > IBFT_KEY_SHARE_MAX_PARTS || self_part >= n_parts) {
+    set_err("bad argument: %u parts (1 to %u), own part %u", n_parts, IBFT_KEY_SHARE_MAX_PARTS, self_part);
+    return IBFT_ERR_INVALID_ARG;
+  }
+  key_share_parts parts{};
+  for (uint32_t k = 0; k < n_parts; k++) {
+    if (k != self_part && part_ptrs[k] == 0) { set_err("key block %u is null", k); return IBFT_ERR_INVALID_ARG; }
+    parts.part[k] = (const uint32_t*)(uintptr_t)part_ptrs[k];
+  }
+#if IBFT_WC > 0
+  lane* L = &e->lanes[0];
+  std::lock_guard<std::mutex> lk(L->mu);
+  int rc = key_share_begin(e);
+  if (rc != IBFT_OK) return rc;
+  cudaStream_t st = stream ? (cudaStream_t)stream : L->stream;
+  if (d_counts_out) CU(cudaMemsetAsync(d_counts_out, 0, 8, st));
+  key_registry& R = e->reg;
+  k_key_adopt<<<dim3(IBFT_KEY_SHARE_RECORDS / 256, n_parts), 256, 0, st>>>(parts, self_part, e->d_slots, e->p.max_table_slots, R.d_state,
+                                                                          R.d_key_xy, R.d_addr, R.d_shared, R.d_learn_count,
+                                                                          (uint32_t*)d_counts_out);
+  e->launches++;
+  CU(cudaGetLastError());
+  return IBFT_OK;
+#else
+  (void)d_counts_out; (void)stream;
   set_err("library built without a key registry");
   return IBFT_ERR_INVALID_ARG;
 #endif

@@ -45,6 +45,7 @@ EXPORTS = [
     "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_sign_batch_rfc6979", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_set_key_table_budget", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
     "ibft_debug_wtable", "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
     "ibft_engine_create_multi", "ibft_engine_device_count", "ibft_engine_sub", "ibft_explain_batch",
+    "ibft_key_share_words", "ibft_key_share_export_device", "ibft_key_share_adopt_device",
 ]
 
 
@@ -113,6 +114,9 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.ibft_exchange_close.argtypes = [c_void_p, c_void_p]
     lib.ibft_exchange_free.argtypes = [c_void_p, c_void_p]
     lib.ibft_exchange_clear.argtypes = [c_void_p, c_void_p, c_uint32, c_uint32, c_void_p]
+    lib.ibft_key_share_words.argtypes = [c_void_p, POINTER(c_uint32)]
+    lib.ibft_key_share_export_device.argtypes = [c_void_p, c_void_p, c_void_p]
+    lib.ibft_key_share_adopt_device.argtypes = [c_void_p, c_void_p, c_uint32, c_uint32, c_void_p, c_void_p]
     lib.ibft_get_voted_bitmap.argtypes = [c_void_p, c_uint32, c_void_p, c_uint32]
     lib.ibft_keccak256_batch.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_uint32, c_void_p]
     lib.ibft_proposal_hash_batch.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]
@@ -403,6 +407,22 @@ class Engine:
 
     def exchange_clear(self, d_buf: int, word_off: int, words: int, stream: int = 0):
         self._check(self.lib.ibft_exchange_clear(self.handle, c_void_p(d_buf), word_off, words, stream or None))
+
+    def key_share_words(self) -> int:
+        """u32 words of one key block (ibft_key_share_words)"""
+        w = c_uint32(0)
+        self._check(self.lib.ibft_key_share_words(self.handle, ctypes.byref(w)))
+        return int(w.value)
+
+    def key_share_export_device(self, d_block: int, stream: int = 0):
+        """write the keys learned by recovery since the last export into the key block at d_block (ibft_key_share_export_device)"""
+        self._check(self.lib.ibft_key_share_export_device(self.handle, c_void_p(d_block), stream or None))
+
+    def key_share_adopt_device(self, part_ptrs, self_part: int, d_counts: int = 0, stream: int = 0):
+        """adopt the checked keys of every key block in part_ptrs but part_ptrs[self_part]; d_counts (u32[2], optional) receives
+        (adopted, refused) (ibft_key_share_adopt_device).  Call refresh_key_tables() afterwards to build their tables."""
+        arr = (c_uint64 * len(part_ptrs))(*[int(p) for p in part_ptrs])
+        self._check(self.lib.ibft_key_share_adopt_device(self.handle, arr, len(part_ptrs), self_part, d_counts or None, stream or None))
 
     def voted_bitmap(self, group: int, n_validators: int) -> np.ndarray:
         words = np.zeros((n_validators + 31) // 32, dtype=np.uint32)

@@ -42,6 +42,7 @@ def all_gather_bitmap(local_words: torch.Tensor, n: int, world: int) -> torch.Te
 import numpy as np  # noqa: E402
 
 _KINDS_WITH_PAYLOAD = (1, 3, 4, 5)  # IBFT_KIND_PAYLOAD, _WIRE, _WIRE_SEAL, _PAYLOAD2 (include/ibft_verify.h)
+_KEY_RECORDS, _KEY_MAX_PARTS = 1024, 256  # IBFT_KEY_SHARE_RECORDS, IBFT_KEY_SHARE_MAX_PARTS (include/ibft_verify.h)
 
 
 def rebase_shard(items: np.ndarray, arena: np.ndarray, lo: int, hi: int):
@@ -104,6 +105,11 @@ class ShardedVerifier:
     The descriptors are bound as given, quorum rule and proposer included (Engine.groups(..., rule=, proposer=)): both exchanges
     return go-ibft's per-message-type decision (HasPrepareQuorum for PREPARE groups, one valid message for PREPREPARE groups).
 
+    Key registry (engine flag key_cache): a rank only recovers the signers whose items land in its shard.  Call share_keys()
+    between rounds and every rank also knows the keys the other ranks learned, so from the next round on no rank recovers a
+    validator any rank already knows.  A caller that never calls it sees no change, except that a p2p-mode rank with a key
+    registry exports its new keys into its exchange buffer every round (see share_keys).
+
     Peer-memory exchange: when a peer does not publish its round within the kernel's bounded wait, finish() raises RuntimeError,
     and so does every later round of this verifier -- the timeout flag is never cleared.  Rebuild the verifiers of all ranks
     after a timeout: the parity alternation only guarantees that a peer has finished reading this rank's buffer of round e when
@@ -143,10 +149,23 @@ class ShardedVerifier:
         self.items_base = self.d_items.data_ptr() - self.lo * 128
         self.bitmap_base = self.d_local.data_ptr() - (self.lo // 32) * 4
         self.exchange = exchange
+        # key sharing (share_keys): each rank sends key_blocks blocks of key_words words per step, enough for a whole validator
+        # table (a rank that learned more keys sends the rest at the next step); key_words = 0 when the engine has no key registry
+        self.key_words = engine.key_share_words() if engine.params.flags & 1 else 0
+        self.key_blocks = -(-engine.params.max_validators // _KEY_RECORDS)
+        kw = self.key_blocks * self.key_words                             # words per rank and step
+        if self.key_words:
+            n_calls = -(-(world - 1) * self.key_blocks // (_KEY_MAX_PARTS - 1)) if world > 1 else 1
+            self.d_key_counts = torch.zeros(2 * n_calls, dtype=torch.int32, device=dev)
+            self.h_key_counts = torch.zeros(2 * n_calls, dtype=torch.int32).pin_memory()
+            if exchange != "p2p":
+                self.d_keys = torch.zeros(kw, dtype=torch.int32, device=dev)
+                self.d_keys_all = torch.zeros(world * kw, dtype=torch.int32, device=dev)
         if exchange == "p2p":
             self.wpr = (self.per + self.W + 63) // 64 * 64                   # words per rank and parity
-            # [2][wpr] words, then the two flags: an engine-owned cudaMalloc block whose IPC handle the peers open on THEIR device
-            self.xbuf_ptr, handle = engine.exchange_alloc(2 * self.wpr + 64)
+            # [2][wpr] words, then the two flags (64 words), then with a key registry [2][kw] words of key blocks: an engine-owned
+            # cudaMalloc block whose IPC handle the peers open on THEIR device
+            self.xbuf_ptr, handle = engine.exchange_alloc(2 * self.wpr + 64 + 2 * kw)
             self.epoch = 0
             self.d_full = torch.zeros(world * self.per, dtype=torch.int32, device=dev)
             self.d_timeout = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -188,6 +207,8 @@ class ShardedVerifier:
                 self.e.verify_device(self.items_base, self.n, self.d_arena.data_ptr(), self.h_arena.numel(), self.lo, self.hi,
                                      base - (self.lo // 32) * 4, 0, st)
             self.e.quorum_mark_device(self.items_base, self.n, self.lo, self.hi, base - (self.lo // 32) * 4, base + self.per * 4, st)
+            if self.key_words:
+                self._export_keys(self._key_region(self.xbuf_ptr, par), st)
             self.e.quorum_exchange_device(self.peer_ptrs, self.rank, self.wpr, self.per, self.epoch, self.d_full.data_ptr(),
                                           self.d_results.data_ptr(), self.d_timeout.data_ptr(), st)
             nres = self.d_results.numel()
@@ -238,3 +259,55 @@ class ShardedVerifier:
     def run(self):
         self.enqueue()
         return self.finish()
+
+    def _key_region(self, xbuf_ptr: int, par: int) -> int:
+        """device address of a rank's key blocks of parity `par` in its exchange buffer"""
+        return xbuf_ptr + (2 * self.wpr + 64 + par * self.key_blocks * self.key_words) * 4
+
+    def _export_keys(self, region: int, st: int):
+        for j in range(self.key_blocks):             # each export takes the next (up to) 1,024 keys not yet exported
+            self.e.key_share_export_device(region + 4 * j * self.key_words, st)
+
+    def share_keys(self) -> tuple[int, int]:
+        """Between rounds, after finish(): every rank takes the validator keys the other ranks learned by recovery, each checked on
+        its device (the key must hash to the address it claims), then builds their comb tables.  Collective: every rank calls it.
+        Returns (keys adopted, records refused) of this rank.
+
+        Each rank sends key_blocks key blocks per step, enough for every validator of a full table; keys beyond that go at the
+        next step.  nccl: export this rank's new keys into its blocks, one all_gather_into_tensor of every rank's blocks, adopt,
+        on self.stream.  p2p: each round's enqueue() exports into this rank's key blocks of the round's parity, before the
+        exchange kernel publishes the round's flag; here the rank adopts from the peers' blocks of that parity, which its
+        exchange kernel has seen published.
+        The read is safe for the same reason the exchange's is: a peer rewrites parity p only in round e + 2, after it has seen
+        this rank's flag of round e + 1, which this rank publishes after the adoption (same stream).  Keys a rank exported in a
+        round that was not followed by share_keys() are not sent again; the peers learn them by recovery."""
+        if not self.key_words:
+            raise RuntimeError("share_keys needs an engine with the key registry (key_cache=True)")
+        st = self.stream.cuda_stream
+        if self.exchange == "p2p":
+            self.stream.synchronize()
+            nres = self.d_results.numel() + 4 * self.world * self.per
+            if self.epoch and int(self.h_out[nres:].numpy().view(np.uint32)[0]):
+                raise RuntimeError("peer-memory exchange: a peer did not publish its round in time")
+            regions = [self._key_region(p, self.epoch & 1) for p in self.peer_ptrs]
+        else:
+            regions = [self.d_keys_all.data_ptr() + 4 * k * self.key_blocks * self.key_words for k in range(self.world)]
+        blocks = [[reg + 4 * j * self.key_words for j in range(self.key_blocks)] for reg in regions]
+        peers = [b for k in range(self.world) if k != self.rank for b in blocks[k]]
+        own = blocks[self.rank][0]
+        with torch.cuda.stream(self.stream):
+            if self.exchange != "p2p":
+                self._export_keys(self.d_keys.data_ptr(), st)
+                if self.world > 1:
+                    dist.all_gather_into_tensor(self.d_keys_all, self.d_keys)
+                else:
+                    self.d_keys_all.copy_(self.d_keys)
+            # own block first, as the skipped part: at most IBFT_KEY_SHARE_MAX_PARTS - 1 peer blocks per call
+            per_call = _KEY_MAX_PARTS - 1
+            for j, i in enumerate(range(0, max(len(peers), 1), per_call)):
+                self.e.key_share_adopt_device([own] + peers[i: i + per_call], 0, self.d_key_counts.data_ptr() + 8 * j, st)
+            self.h_key_counts.copy_(self.d_key_counts, non_blocking=True)
+        self.stream.synchronize()        # the adopted keys are in the registry before the refresh reads its learn counter
+        self.e.refresh_key_tables()
+        c = self.h_key_counts.numpy().reshape(-1, 2).sum(axis=0)
+        return int(c[0]), int(c[1])

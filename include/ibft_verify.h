@@ -443,6 +443,34 @@ int ibft_set_recover_path(ibft_engine* e, int path);
  * entry points call it between rounds.  No-op (0 keys) when the flag is off. */
 int ibft_refresh_key_tables(ibft_engine* e, uint32_t* n_keys_out);
 
+/* Key sharing between engines of separate processes (IBFT_FLAG_KEY_CACHE), e.g. the ranks of a sharded verifier, each of
+ * which only recovers the signers whose items land in its shard.  Between rounds, on every rank:
+ *   1. ibft_key_share_export_device writes the keys this engine learned by recovery since its last export into a key block;
+ *   2. the caller exchanges the blocks (an all-gather, or peer memory);
+ *   3. ibft_key_share_adopt_device takes the peers' keys, each checked on the device before it enters the registry;
+ *   4. ibft_refresh_key_tables builds their tables (adopted keys fall under ibft_set_key_table_budget like learned ones).
+ * Key block: IBFT_KEY_SHARE_WORDS u32 words.  Word 0 = the record count (at most IBFT_KEY_SHARE_RECORDS), then the records
+ * of IBFT_KEY_SHARE_RECORD_WORDS words each: the 20-byte address in 5 words (byte 4k + j in byte j of word k), then x and y as
+ * 8 little-endian words each.  Records name addresses, not registry entries, so the ranks need not number their entries alike.
+ *   - Export: entries in ascending entry order, at most IBFT_KEY_SHARE_RECORDS; a rank that learned more sends the rest at its
+ *     next export.  A key taken by adoption is never exported; an entry ibft_set_validators gives to another address is
+ *     exported again once it learns its new key.
+ *   - Adopt: every block part_ptrs[k] (device addresses as seen from this process: a gathered tensor or mapped peer memory),
+ *     except part_ptrs[self_part].  A record whose address no resident table lists is dropped.  The key must be fully reduced,
+ *     on the curve and hash to the address, or it is refused; a valid key of an entry that has none is written as a recovery
+ *     writes it.  A block whose count exceeds IBFT_KEY_SHARE_RECORDS is refused whole (one refusal).  d_counts_out (u32[2],
+ *     may be NULL) receives { keys adopted, records refused }.  The kernel may run beside verify kernels.
+ * Both run on `stream` (NULL: the engine's own).  IBFT_ERR_INVALID_ARG without IBFT_FLAG_KEY_CACHE, on a multi-device engine,
+ * while a submitted call is pending, or for more than IBFT_KEY_SHARE_MAX_PARTS parts. */
+#define IBFT_KEY_SHARE_RECORDS 1024u
+#define IBFT_KEY_SHARE_RECORD_WORDS 21u
+#define IBFT_KEY_SHARE_WORDS 21568u /* 1 + 1024 x 21, padded to a multiple of 64 */
+#define IBFT_KEY_SHARE_MAX_PARTS 256u
+int ibft_key_share_words(ibft_engine* e, uint32_t* words_out);
+int ibft_key_share_export_device(ibft_engine* e, void* d_block, void* stream);
+int ibft_key_share_adopt_device(ibft_engine* e, const uint64_t* part_ptrs, uint32_t n_parts, uint32_t self_part, void* d_counts_out,
+                                void* stream);
+
 /* Key registry (IBFT_FLAG_KEY_CACHE): hold at most max_tables comb tables (136 KiB each) from now on.  The call is opt-in and
  * puts the engine in bounded mode for the rest of its life; the value may be changed again at any time (0 keeps every key
  * learned but builds no table: every signature takes the recover path).  In bounded mode:
