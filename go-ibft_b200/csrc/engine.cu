@@ -1278,6 +1278,79 @@ k_explain(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// Reject reasons of device-resident items (ibft_explain_batch_device), in two launches per chunk of a shard.
+// k_explain_compact: one thread per item of [lo, hi) (lo a multiple of 32, so each warp reads one bitmap word).  A one bit gets
+// IBFT_REASON_OK and a zero address; the zero bits are appended to worklist[1..] with one atomic per warp (order is free: every
+// output is written by index), and their number is added to worklist[0] and to *count (when given).
+// ------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_explain_compact(const uint32_t* __restrict__ bitmap, uint32_t lo, uint32_t hi, uint8_t* __restrict__ reasons,
+                  uint8_t* __restrict__ recovered, uint32_t* __restrict__ worklist, uint32_t* __restrict__ count) {
+  const uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t lane = threadIdx.x & 31u;
+  bool zero = false;
+  if (i < hi) {
+    const bool one = (__ldg(bitmap + (i >> 5)) >> lane) & 1u;
+    zero = !one;
+    if (one) {
+      reasons[i] = IBFT_REASON_OK;
+      if (recovered)
+#pragma unroll
+        for (int k = 0; k < 20; k++) recovered[(size_t)i * 20 + k] = 0;
+    }
+  }
+  const uint32_t m = __ballot_sync(0xFFFFFFFFu, zero);
+  if (m == 0) return;
+  uint32_t base = 0;
+  if (lane == 0) {
+    base = atomicAdd(worklist, (uint32_t)__popc(m));
+    if (count) atomicAdd(count, (uint32_t)__popc(m));
+  }
+  base = __shfl_sync(0xFFFFFFFFu, base, 0);
+  if (zero) worklist[1 + base + __popc(m & ((1u << lane) - 1u))] = i;
+}
+
+// k_explain_list: k_explain over the worklist of k_explain_compact, launched for the most items the list can hold (the count is
+// on the device); threads beyond it leave at once, as in k_recover's worklist mode.  Every listed item has verdict bit 0, so an
+// item the pass accepts is IBFT_REASON_INCONSISTENT.  recovered may be null.
+template <bool WIDE>
+__global__ void __launch_bounds__(32)
+k_explain_list(const ibft_sig_item* __restrict__ items, const uint8_t* __restrict__ arena, size_t arena_len,
+               const ibft_group_desc* __restrict__ groups, uint32_t n_groups, const slot_dev* __restrict__ slots, uint32_t n_slots,
+               const uint32_t* __restrict__ ctable, const uint32_t* __restrict__ wtable, const uint32_t* __restrict__ worklist,
+               uint8_t* __restrict__ reasons, uint8_t* __restrict__ recovered) {
+  extern __shared__ uint32_t s_rtab[];
+  const uint32_t k = blockIdx.x * 32 + threadIdx.x;
+  if (k >= worklist[0]) return;
+  const uint32_t i = worklist[1 + k];
+  ibft_sig_item it;
+  const uint4* src = reinterpret_cast<const uint4*>(items + i);
+  uint4* w = reinterpret_cast<uint4*>(&it);
+#pragma unroll
+  for (int j = 0; j < 8; j++) w[j] = __ldg(src + j);
+  gtab_view G{g_gtable};
+  G.comb = ctable;
+  G.wide = WIDE ? wtable : nullptr;
+  rtab_view T{s_rtab + threadIdx.x, 32u};
+  auto member = [&](uint32_t group, const uint8_t* signer) {
+    int v;
+    uint32_t slot;
+    return group_member(groups, n_groups, slots, n_slots, group, signer, &v, &slot);
+  };
+  uint8_t addr[20];
+  uint8_t why;
+#if IBFT_GEN_WIDE > 0
+  if (WIDE) why = explain_item(exec_serial_wide{}, it, arena, arena_len, groups != nullptr, n_groups, G, T, member, addr);
+  else
+#endif
+    why = explain_item(exec_serial{}, it, arena, arena_len, groups != nullptr, n_groups, G, T, member, addr);
+  reasons[i] = why == IBFT_REASON_OK ? (uint8_t)IBFT_REASON_INCONSISTENT : why;
+  if (recovered)
+#pragma unroll
+    for (int j = 0; j < 20; j++) recovered[(size_t)i * 20 + j] = addr[j];
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // hash-only batch (IsValidProposalHash)
 // ------------------------------------------------------------------------------------------------------------
 __global__ void k_keccak_batch(const uint8_t* __restrict__ arena, size_t arena_len, const uint32_t* __restrict__ offs,
@@ -1934,6 +2007,10 @@ struct ibft_engine {
   uint32_t* d_ctable = nullptr;  // combined generator table (IBFT_WC > 0)
   uint32_t* d_wtable = nullptr;  // wide generator comb of the device (IBFT_GEN_WIDE > 0), shared; nullptr when it did not fit
   cudaFuncAttributes recover_attr{};
+  // ibft_explain_batch_device: [0] = count, [1..max_items] = the zero bits of one chunk of a shard; explain_ev = its last use
+  // (calls may arrive on different streams)
+  uint32_t* d_explain_wl = nullptr;
+  cudaEvent_t explain_ev = nullptr;
   // hashing (ibft_keccak256_batch / ibft_proposal_hash_batch): own lock, own stream, own grow-only scratch -- a hash call
   // never waits for a verify call and never allocates on the per-call path
   std::mutex hash_mu;
@@ -2090,6 +2167,8 @@ static void engine_free(ibft_engine* e) {
   cudaFree(e->reg.d_state); cudaFree(e->reg.d_key_xy); cudaFree(e->reg.d_addr); cudaFree(e->reg.d_chunks); cudaFree(e->reg.d_learn_count);
   cudaFreeHost(e->reg.h_learn_count);
   cudaFree(e->d_slots);
+  cudaFree(e->d_explain_wl);
+  if (e->explain_ev) cudaEventDestroy(e->explain_ev);
   if (e->hash_stream) cudaStreamDestroy(e->hash_stream);
   cudaFree(e->hs_arena); cudaFreeHost(e->hs_h_arena); cudaFree(e->hs_meta); cudaFreeHost(e->hs_h_meta);
   delete e;
@@ -2159,6 +2238,8 @@ static int engine_alloc(ibft_engine* e) {
   }
   CU(cudaMalloc(&e->d_slots, (size_t)p.max_table_slots * sizeof(slot_dev)));
   CU(cudaMemset(e->d_slots, 0, (size_t)p.max_table_slots * sizeof(slot_dev)));
+  CU(cudaMalloc(&e->d_explain_wl, ((size_t)p.max_items + 1) * 4));
+  CU(cudaEventCreateWithFlags(&e->explain_ev, cudaEventDisableTiming));
   e->slots.resize(p.max_table_slots);
   e->slots_shadow.assign(p.max_table_slots, slot_dev{});
   CU(cudaMemcpyToSymbol(g_gtable, IBFT_GTABLE, sizeof(uint32_t) * IBFT_GTAB_ENTRY_WORDS * IBFT_GTAB_ENTRIES));
@@ -3533,6 +3614,47 @@ extern "C" int ibft_verify_batch_device(ibft_engine* e, const void* d_items, uin
   return launch_recover(e, L, (const ibft_sig_item*)d_items, n, (const uint8_t*)d_arena, arena_len, shard_lo, shard_hi,
                         L->last_groups.empty() ? nullptr : L->d_groups, (uint32_t)L->last_groups.size(), (uint32_t*)d_bitmap,
                         (uint8_t*)d_recovered, st);
+}
+
+extern "C" int ibft_explain_batch_device(ibft_engine* e, const void* d_items, uint32_t n, const void* d_arena, size_t arena_len,
+                                         uint32_t shard_lo, uint32_t shard_hi, const void* d_bitmap, void* d_reasons, void* d_recovered,
+                                         void* d_count_out, void* stream) {
+  IBFT_REFUSE_MULTI(e);
+  if (!e || (n && (!d_items || !d_bitmap || !d_reasons)) || (arena_len && !d_arena)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  if (shard_hi > n || shard_lo > shard_hi || (shard_lo & 31) || ((shard_hi & 31) && shard_hi != n)) {
+    set_err("shard [%u,%u) of %u must be 32-aligned", shard_lo, shard_hi, n);
+    return IBFT_ERR_INVALID_ARG;
+  }
+  lane* L = &e->lanes[0];
+  std::lock_guard<std::mutex> lk(L->mu);
+  CU(cudaSetDevice(e->p.device));
+  cudaStream_t st = stream ? (cudaStream_t)stream : L->stream;
+  uint32_t* count = (uint32_t*)d_count_out;
+  if (count) CU(cudaMemsetAsync(count, 0, 4, st));
+  if (shard_hi == shard_lo) return IBFT_OK;
+  // membership as ibft_verify_batch_device decides it: the bound groups, or none
+  const uint32_t n_groups = (uint32_t)L->last_groups.size();
+  const ibft_group_desc* groups = n_groups ? L->d_groups : nullptr;
+  auto kernel = e->d_wtable != nullptr ? k_explain_list<true> : k_explain_list<false>;
+  uint32_t* wl = e->d_explain_wl;
+  CU(cudaStreamWaitEvent(st, e->explain_ev, 0));
+  // chunks of max_items, a multiple of 32 (ibft_engine_create rounds it up), so that every chunk starts on a bitmap word
+  const uint32_t chunk = e->p.max_items;
+  for (uint32_t lo = shard_lo; lo < shard_hi; lo += std::min(chunk, shard_hi - lo)) {
+    const uint32_t cnt = std::min(chunk, shard_hi - lo);
+    CU(cudaMemsetAsync(wl, 0, 4, st));
+    k_explain_compact<<<(cnt + 255) / 256, 256, 0, st>>>((const uint32_t*)d_bitmap, lo, lo + cnt, (uint8_t*)d_reasons,
+                                                         (uint8_t*)d_recovered, wl, count);
+    e->launches++;
+    CU(cudaGetLastError());
+    kernel<<<(cnt + 31) / 32, 32, 32 * IBFT_RTAB_WORDS * 4, st>>>((const ibft_sig_item*)d_items, (const uint8_t*)d_arena, arena_len, groups,
+                                                                  n_groups, e->d_slots, e->p.max_table_slots, e->d_ctable, e->d_wtable, wl,
+                                                                  (uint8_t*)d_reasons, (uint8_t*)d_recovered);
+    e->launches++;
+    CU(cudaGetLastError());
+  }
+  CU(cudaEventRecord(e->explain_ev, st));
+  return IBFT_OK;
 }
 
 // binds the groups used by the device-resident entry points (copied to the engine's device buffers)

@@ -44,7 +44,7 @@ EXPORTS = [
     "ibft_exchange_alloc", "ibft_exchange_open", "ibft_exchange_close", "ibft_exchange_free", "ibft_exchange_clear",
     "ibft_get_voted_bitmap", "ibft_keccak256_batch", "ibft_proposal_hash_batch", "ibft_sign_batch", "ibft_sign_batch_rfc6979", "ibft_engine_launch_count", "ibft_set_recover_path", "ibft_refresh_key_tables", "ibft_set_key_table_budget", "ibft_probe_int_peak", "ibft_debug_op", "ibft_debug_ctable",
     "ibft_debug_wtable", "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
-    "ibft_engine_create_multi", "ibft_engine_device_count", "ibft_engine_sub", "ibft_explain_batch",
+    "ibft_engine_create_multi", "ibft_engine_device_count", "ibft_engine_sub", "ibft_explain_batch", "ibft_explain_batch_device",
     "ibft_key_share_words", "ibft_key_share_export_device", "ibft_key_share_adopt_device",
 ]
 
@@ -104,6 +104,8 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
     lib.ibft_verify_wait.argtypes = [c_void_p]
     lib.ibft_bind_groups.argtypes = [c_void_p, c_void_p, c_uint32]
     lib.ibft_verify_batch_device.argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_size_t, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p]
+    lib.ibft_explain_batch_device.argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_size_t, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p,
+                                              c_void_p, c_void_p]
     lib.ibft_quorum_reduce_device.argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p]
     lib.ibft_quorum_partial_words.argtypes = [c_void_p, POINTER(c_uint32)]
     lib.ibft_quorum_mark_device.argtypes = [c_void_p, c_void_p, c_uint32, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p]
@@ -366,6 +368,14 @@ class Engine:
                       d_recovered: int = 0, stream: int = 0):
         self._check(self.lib.ibft_verify_batch_device(self.handle, d_items, n, d_arena or None, arena_len, lo, hi, d_bitmap,
                                                       d_recovered or None, stream or None))
+
+    def explain_device(self, d_items: int, n: int, d_arena: int, arena_len: int, lo: int, hi: int, d_bitmap: int, d_reasons: int,
+                       d_recovered: int = 0, d_count: int = 0, stream: int = 0):
+        """ibft_explain_batch_device: writes bytes [lo, hi) of d_reasons (REASON_*: OK for a one bit of d_bitmap, the reason for a
+        zero bit) and, when given, rows [lo, hi) of d_recovered (20 bytes each); d_count (u32, optional) receives the number of zero
+        bits explained.  Pointers are indexed by global item number, as in verify_device; enqueues only."""
+        self._check(self.lib.ibft_explain_batch_device(self.handle, d_items or None, n, d_arena or None, arena_len, lo, hi, d_bitmap or None,
+                                                       d_reasons or None, d_recovered or None, d_count or None, stream or None))
 
     def quorum_reduce_device(self, d_items: int, n: int, d_bitmap: int, n_groups: int, d_results: int, stream: int = 0):
         self._check(self.lib.ibft_quorum_reduce_device(self.handle, d_items, n, d_bitmap, None, n_groups, d_results, stream or None))

@@ -72,6 +72,45 @@ def rebase_shard(items: np.ndarray, arena: np.ndarray, lo: int, hi: int):
     return local, local_arena
 
 
+def explain_block_bytes(n: int, world: int) -> int:
+    """bytes of one rank's explain block: P = shard_words(n, world) * 32 reason bytes, then P x 20 recovered-address bytes (a
+    rank's shard padded to P items, so that the blocks of ranks 0.. all-gathered in rank order list items 0.. in order)"""
+    return shard_words(n, world) * 32 * 21
+
+
+def explain_shard(engine, block: torch.Tensor, n: int, world: int, rank: int, d_items: int, d_arena: int, arena_len: int,
+                  d_bitmap: int, stream: int = 0):
+    """Enqueue engine.explain_device over this rank's shard with its outputs in `block` (explain_block_bytes(n, world) bytes):
+    the reason and address pointers are rebased by the shard's first item, as the device calls index by global item number.
+    d_items and d_bitmap are the rebased pointers the rank's verify call took.  Bytes of the padding are never written."""
+    lo, hi = shard_bounds(n, world, rank)
+    if hi > lo:
+        P = shard_words(n, world) * 32
+        base = block.data_ptr()
+        engine.explain_device(d_items, n, d_arena, arena_len, lo, hi, d_bitmap, base - lo, base + P - 20 * lo, 0, stream)
+
+
+def gather_explain_blocks(block: torch.Tensor, out: torch.Tensor, world: int) -> torch.Tensor:
+    """Collective: every rank's explain block in rank order, in `out` (world blocks); the block itself at world 1."""
+    if world == 1:
+        return block
+    dist.all_gather_into_tensor(out, block)
+    return out
+
+
+def explain_rows(blocks: np.ndarray, n: int, world: int, rank: int | None = None):
+    """(reasons uint8[m], recovered uint8[m, 20]) out of explain blocks: with rank, `blocks` is that rank's block and m its
+    shard's length; without, `blocks` is every rank's block in rank order (the all-gather) and m = n."""
+    P = shard_words(n, world) * 32
+    b = np.asarray(blocks, dtype=np.uint8).reshape(-1, 21 * P)
+    reasons, rec = b[:, :P].reshape(-1), b[:, P:].reshape(-1, 20)
+    m = n
+    if rank is not None:
+        lo, hi = shard_bounds(n, world, rank)
+        m = hi - lo
+    return reasons[:m].copy(), rec[:m].copy()
+
+
 def open_peer_buffers(engine, world: int, rank: int, own_ptr: int, own_handle: bytes) -> list:
     """Collective: exchange the CUDA IPC handles of the ranks' exchange buffers and map every peer's buffer on this rank's device
     (engine.exchange_open).  Returns the per-rank device addresses (own_ptr at `rank`).  Either every rank succeeds or every rank
@@ -259,6 +298,28 @@ class ShardedVerifier:
     def run(self):
         self.enqueue()
         return self.finish()
+
+    def explain(self, gather: bool = False):
+        """After finish(): why this rank's items of the round were rejected, decided again on the device (Engine.explain_device
+        on self.stream, against the round's own verdict words: the local words in nccl mode, the rank's words of the assembled
+        bitmap in p2p mode).  Returns host arrays (reasons uint8[hi - lo], recovered uint8[hi - lo, 20]) of the shard -- REASON_OK
+        for an accepted item, REASON_NEEDS_HOST for a non-canonical raw frame to re-submit through the host path.
+        gather=True is collective (every rank calls it): one all-gather of the ranks' reasons and addresses, and every rank
+        returns all n items, what Engine.explain_batch returns for the whole batch and its bitmap."""
+        if not hasattr(self, "d_explain"):                 # allocated on the first call, reused by every later round
+            nb = explain_block_bytes(self.n, self.world)
+            dev = self.d_items.device
+            self.d_explain = torch.zeros(nb, dtype=torch.uint8, device=dev)
+            self.d_explain_all = torch.zeros(self.world * nb, dtype=torch.uint8, device=dev) if self.world > 1 else self.d_explain
+            self.h_explain = torch.zeros(self.world * nb, dtype=torch.uint8).pin_memory()
+        bitmap = self.d_full.data_ptr() if self.exchange == "p2p" else self.bitmap_base
+        with torch.cuda.stream(self.stream):
+            explain_shard(self.e, self.d_explain, self.n, self.world, self.rank, self.items_base, self.d_arena.data_ptr(),
+                          self.h_arena.numel(), bitmap, self.stream.cuda_stream)
+            src = gather_explain_blocks(self.d_explain, self.d_explain_all, self.world) if gather else self.d_explain
+            self.h_explain[: src.numel()].copy_(src, non_blocking=True)
+        self.stream.synchronize()
+        return explain_rows(self.h_explain[: src.numel()].numpy(), self.n, self.world, None if gather else self.rank)
 
     def _key_region(self, xbuf_ptr: int, par: int) -> int:
         """device address of a rank's key blocks of parity `par` in its exchange buffer"""

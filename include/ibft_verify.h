@@ -237,7 +237,7 @@ int ibft_engine_device_info(ibft_engine* e, ibft_device_info* out);
  *   ibft_engine_launch_count       the sum over the devices.
  *   ibft_engine_device_info,       the lead answers; ibft_engine_sub reaches the others.
  *   ibft_probe_int_peak, ibft_debug_*
- *   ibft_bind_groups, ibft_verify_batch_device, ibft_quorum_*_device, ibft_exchange_*
+ *   ibft_bind_groups, ibft_verify_batch_device, ibft_explain_batch_device, ibft_quorum_*_device, ibft_exchange_*
  *                                  IBFT_ERR_INVALID_ARG: they take device pointers of one device.  Across processes or nodes, or
  *                                  with device-resident buffers, use one engine per device (go-ibft_b200/sharding.py). */
 int ibft_engine_create_multi(const ibft_engine_params* params, const int32_t* devices, uint32_t n_devices, ibft_engine** out);
@@ -329,6 +329,28 @@ int ibft_bind_groups(ibft_engine* e, const ibft_group_desc* groups, uint32_t n_g
  * be multiples of 32 or equal to n) -- the multi-GPU path all-gathers the bitmap words afterwards. */
 int ibft_verify_batch_device(ibft_engine* e, const void* d_items, uint32_t n, const void* d_arena, size_t arena_len,
                              uint32_t shard_lo, uint32_t shard_hi, void* d_bitmap, void* d_recovered, void* stream);
+
+/* ibft_explain_batch for device-resident items: why each item of [shard_lo, shard_hi) whose verdict bit is 0 was rejected,
+ * without a host round trip of tuples or verdicts.  Every pointer is a DEVICE pointer on the engine's device, indexed by global
+ * item number as in ibft_verify_batch_device (item i, bit i of d_bitmap, byte i of d_reasons, bytes 20*i.. of d_recovered);
+ * the shard rules are the same (both bounds multiples of 32, or shard_hi == n).  Enqueues only, on `stream` (NULL = engine
+ * stream); the caller synchronises it.
+ *   d_bitmap     the verdict bitmap of the verify call over the same items (ibft_verify_batch_device's words of the shard).
+ *   d_reasons    only bytes [shard_lo, shard_hi) are written: IBFT_REASON_OK for a one bit; for a zero bit the reason the
+ *                recover path gives (IBFT_REASON_NEEDS_HOST included: re-submit those items through the host path), or
+ *                IBFT_REASON_INCONSISTENT if it accepts the item.
+ *   d_recovered  NULL, or the recovered address of the items that got as far as recovery, zero for every other item of the shard.
+ *   d_count_out  NULL, or one device uint32 receiving the number of items explained (the zero bits of the shard).
+ * Membership comes from the groups bound by ibft_bind_groups, as ibft_verify_batch_device decides it; with none bound, no item
+ * is IBFT_REASON_NO_GROUP or _NOT_VALIDATOR.  Every reason is the recover path's decision: the key registry is never consulted
+ * or taught.  The zero bits are compacted on the device (k_explain_compact) and explained one thread each (k_explain_list),
+ * in chunks of at most max_items (rounded up to a multiple of 32 at engine creation): two launches per chunk, none for an empty
+ * shard; the worklist is engine-owned, so a shard larger than max_items needs no host synchronisation either.
+ * Errors, with nothing enqueued and every output untouched: IBFT_ERR_INVALID_ARG for a null pointer, a misaligned shard, a
+ * multi-device engine or a sub-engine view. */
+int ibft_explain_batch_device(ibft_engine* e, const void* d_items, uint32_t n, const void* d_arena, size_t arena_len,
+                              uint32_t shard_lo, uint32_t shard_hi, const void* d_bitmap, void* d_reasons, void* d_recovered,
+                              void* d_count_out, void* stream);
 
 /* Device-resident quorum reduction over a complete (all-gathered) bitmap: resolves each item's signer to its
  * validator index, ORs the per-group voted sets and reduces voting power against the threshold.
