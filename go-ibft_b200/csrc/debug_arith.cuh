@@ -56,6 +56,23 @@ IBFT_HD bool debug_arith_op(int op, const uint8_t* a, const uint8_t* b, uint8_t*
       rfc6979_candidate(a, zm, c[63], o);
       return true;
     }
+    case IBFT_DBG_FE_FUSED: {
+      if (c == nullptr) return false;
+      const fe x = fe_from_be(a), y = fe_from_be(b), z = fe_from_be(c);
+      fe r;
+      switch (c[63]) {
+        case 0: r = fe_mul3(x); break;
+        case 1: r = fe_sub_shl<1>(x, y); break;
+        case 2: r = fe_sub_shl<3>(x, y); break;
+        case 3: r = fe_sub_sub_dbl(x, y, z); break;
+        case 4: r = fe_dbl_sub_sub(x, y, z); break;
+        case 5: r = fe_sub_signed(x, y, false); break;
+        case 6: r = fe_sub_signed(x, y, true); break;
+        default: return false;
+      }
+      fe_to_be(r, o);
+      return true;
+    }
     default: return false;
   }
 }

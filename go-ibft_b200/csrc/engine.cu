@@ -4031,7 +4031,7 @@ extern "C" int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* w
 extern "C" int ibft_debug_op(ibft_engine* e, int op, const uint8_t* a, const uint8_t* b, const uint8_t* c, uint32_t n,
                              uint8_t* out, uint32_t out_stride) {
   e = diag_engine(e);
-  if (!e || !a || !out || n == 0 || ((op == IBFT_DBG_RFC6979 || op == IBFT_DBG_KEY_ADDRESS) && (!b || !c))) {
+  if (!e || !a || !out || n == 0 || ((op == IBFT_DBG_RFC6979 || op == IBFT_DBG_KEY_ADDRESS || op == IBFT_DBG_FE_FUSED) && (!b || !c))) {
     set_err("null argument");
     return IBFT_ERR_INVALID_ARG;
   }

@@ -89,16 +89,10 @@ IBFT_PT jac jac_double_body(const jac& p) {
   fe b = DSQR(p.y);
   fe c = DSQR(b);
 #endif
-  fe t = fe_add(p.x, b);
-  t = DSQR(t);
-  t = fe_sub(t, a);
-  t = fe_sub(t, c);
-  fe d = fe_dbl(t);
-  fe e = fe_add(fe_dbl(a), a);
-  fe f = DSQR(e);
-  r.x = fe_sub(f, fe_dbl(d));
-  fe c8 = fe_dbl(fe_dbl(fe_dbl(c)));
-  r.y = fe_sub(DMUL(e, fe_sub(d, r.x)), c8);
+  const fe d = fe_dbl_sub_sub(DSQR(fe_add(p.x, b)), a, c);  // D = 2 ((X + B)^2 - A - C)
+  const fe e = fe_mul3(a);
+  r.x = fe_sub_shl<1>(DSQR(e), d);                          // X3 = E^2 - 2D
+  r.y = fe_sub_shl<3>(DMUL(e, fe_sub(d, r.x)), c);          // Y3 = E (D - X3) - 8C
   r.z = fe_dbl(DMUL(p.y, p.z));
   r.inf = p.inf;
   return r;
@@ -186,7 +180,8 @@ __device__ __forceinline__ jac jac_double(const jac& p) {
 IBFT_PT jac jac_double(const jac& p) { return jac_double_body(p); }
 #endif
 
-// p + (qx, qy) with q affine (never infinity): 8M + 3S.  h_out (optional): Z3 / Z1 of the generic case (= H), 1 otherwise.
+// p + (qx, qy), or p + (qx, -qy) when neg_q, with q affine (never infinity): 8M + 3S.  h_out (optional): Z3 / Z1 of the
+// generic case (= H), 1 otherwise.
 // OPT-IN -DIBFT_MADD_7M4S: madd-2007-bl, 7M + 4S -- Z3 = (Z1 + H)^2 - Z1Z1 - HH = 2 Z1 H trades the multiplication Z1 H for a
 // squaring, and X3, Y3 carry the matching factors 4 and 8 (I = 4 HH, r = 2 (S2 - Y1)); h_out is then 2H.  Slower on an H100
 // (DESIGN.md §3.1): the seven extra additions cost more issue slots and code than the 28 wide MACs it saves.
@@ -228,8 +223,9 @@ __device__ __noinline__ jac33 jac_madd_v(jac24 in, fe qx, fe qy) {
   o.w[32] = flag;
   return o;
 }
-__device__ __forceinline__ jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, fe* h_out = nullptr) {
+__device__ __forceinline__ jac jac_add_affine(const jac& p, const fe& qx, const fe& qy_in, bool neg_q = false, fe* h_out = nullptr) {
   jac r;
+  const fe qy = neg_q ? fe_neg(qy_in) : qy_in;
   if (h_out) *h_out = fe_from_u32(1);
   if (p.inf) {
     r.x = qx;
@@ -258,13 +254,13 @@ __device__ __forceinline__ jac jac_add_affine(const jac& p, const fe& qx, const 
   return r;
 }
 #else
-IBFT_PT jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, fe* h_out = nullptr) {
+IBFT_PT jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, bool neg_q = false, fe* h_out = nullptr) {
   jac r;
   if (h_out) *h_out = fe_from_u32(1);
   if (p.inf) {
     IBFT_BRANCH(IBFT_BR_ADD_INF);
     r.x = qx;
-    r.y = qy;
+    r.y = neg_q ? fe_neg(qy) : qy;
     r.z = fe_from_u32(1);
     r.inf = false;
     return r;
@@ -273,7 +269,7 @@ IBFT_PT jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, fe* h_out =
   fe u2 = PMUL(qx, z1z1);
   fe s2 = PMUL(PMUL(qy, p.z), z1z1);
   fe h = fe_sub(u2, p.x);
-  fe rr = fe_sub(s2, p.y);
+  fe rr = fe_sub_signed(s2, p.y, neg_q);  // the sign of -Q folded into r = +-S2 - Y1
   if (fe_is_zero(h)) {
     if (fe_is_zero(rr)) {
       IBFT_BRANCH(IBFT_BR_ADD_DBL);
@@ -302,7 +298,7 @@ IBFT_PT jac jac_add_affine(const jac& p, const fe& qx, const fe& qy, fe* h_out =
 #else
   fe hhh = PMUL(h, hh);
   fe v = PMUL(p.x, hh);
-  r.x = fe_sub(fe_sub(PSQR(rr), hhh), fe_dbl(v));
+  r.x = fe_sub_sub_dbl(PSQR(rr), hhh, v);
   r.y = fe_sub(PMUL(rr, fe_sub(v, r.x)), PMUL(p.y, hhh));
   r.z = PMUL(p.z, h);
   r.inf = false;
@@ -715,7 +711,7 @@ IBFT_HD fe ecmult_build_rtable_globalz(const aff& R, const rtab_view& T) {
   for (int m = 1; m < 8; m++) {
     fe h;
     if (m == 1) { t = jac_double(t); h = t.z; }  // Z of R is 1
-    else t = jac_add_affine(t, R.x, R.y, &h);
+    else t = jac_add_affine(t, R.x, R.y, false, &h);
     T.store(m, t.x, t.y);
     zr[m] = h;
   }
@@ -801,9 +797,8 @@ IBFT_HD jac ecmult_streams(const ecmult_digits& dg, const gtab_view& G, const rt
         neg = (d < 0) != dg.kneg[s];
       }
       if (use_beta) x = fe_mul(x, beta);  // lambda * (x, y) = (beta x, y)
-      if (neg) y = fe_neg(y);
       IBFT_OPCOUNT(IBFT_OP_WIN_ADD);
-      acc = jac_add_affine(acc, x, y);
+      acc = jac_add_affine(acc, x, y, neg);
     }
   }
   return acc;
@@ -876,8 +871,7 @@ IBFT_HD jac ecmult_streams_known(const ecmult_digits& dg, const gtab_view& G, co
         if (s == 1) x = fe_mul(x, beta);
         neg = (d < 0) != dg.kneg[s];
       }
-      if (neg) y = fe_neg(y);
-      acc = jac_add_affine(acc, x, y);
+      acc = jac_add_affine(acc, x, y, neg);
     }
   }
   return acc;
@@ -903,9 +897,8 @@ IBFT_HD jac ecmult_gen_comb(const ecmult_digits& dg, const gtab_view& G) {
     if (neg) { d1 = -d1; d2 = -d2; }
     fe x, y;
     G.load_comb_pos(jg, d1, d2, x, y);
-    if (neg) y = fe_neg(y);
     IBFT_OPCOUNT(IBFT_OP_COMB_ADD);
-    acc = jac_add_affine(acc, x, y);
+    acc = jac_add_affine(acc, x, y, neg);
   }
   return acc;
 }
@@ -951,9 +944,8 @@ IBFT_HD jac ecmult_gen_wide(const ecmult_digits& dg, const gtab_view& G) {
     if (d == 0) continue;
     fe x, y;
     G.load_gen_wide(j, d < 0 ? -d : d, x, y);
-    if (d < 0) y = fe_neg(y);
     IBFT_OPCOUNT(IBFT_OP_COMB_ADD);
-    acc = jac_add_affine(acc, x, y);
+    acc = jac_add_affine(acc, x, y, d < 0);
   }
   return acc;
 }

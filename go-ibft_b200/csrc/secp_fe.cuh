@@ -155,19 +155,18 @@ IBFT_FN_ADD fe fe_add(fe a, fe b) {
         "=r"(c)
       : "r"(a.v[0]), "r"(a.v[1]), "r"(a.v[2]), "r"(a.v[3]), "r"(a.v[4]), "r"(a.v[5]), "r"(a.v[6]), "r"(a.v[7]),
         "r"(b.v[0]), "r"(b.v[1]), "r"(b.v[2]), "r"(b.v[3]), "r"(b.v[4]), "r"(b.v[5]), "r"(b.v[6]), "r"(b.v[7]));
-  // fold the carry: 2^256 = 2^32 + 977 (mod p)
-  uint32_t k = c * IBFT_PC, c2;
+  // fold the carry: 2^256 = 2^32 + 977 (mod p).  The carry is 0 or 1, so c * 977 is a mask and an AND on the ALU pipe, not an
+  // IMAD on the FMA pipe, which the multiplier bodies keep busy.
+  uint32_t k = (0u - c) & IBFT_PC, c2;
   asm("add.cc.u32 %0,%0,%9;\n\taddc.cc.u32 %1,%1,%10;\n\taddc.cc.u32 %2,%2,0;\n\taddc.cc.u32 %3,%3,0;\n\t"
       "addc.cc.u32 %4,%4,0;\n\taddc.cc.u32 %5,%5,0;\n\taddc.cc.u32 %6,%6,0;\n\taddc.cc.u32 %7,%7,0;\n\t"
       "addc.u32 %8,0,0;"
       : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2]), "+r"(r.v[3]), "+r"(r.v[4]), "+r"(r.v[5]), "+r"(r.v[6]), "+r"(r.v[7]),
         "=r"(c2)
       : "r"(k), "r"(c));
-  // a second wrap leaves a value < 2^34, so the last fold cannot ripple past limb 2
-  uint32_t k2 = c2 * IBFT_PC;
-  asm("add.cc.u32 %0,%0,%3;\n\taddc.cc.u32 %1,%1,%4;\n\taddc.u32 %2,%2,0;"
-      : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2])
-      : "r"(k2), "r"(c2));
+  // a second wrap leaves a value < 2^34 (limb 1 < 4), so the last fold cannot ripple past limb 1
+  uint32_t k2 = (0u - c2) & IBFT_PC;
+  asm("add.cc.u32 %0,%0,%2;\n\taddc.u32 %1,%1,%3;" : "+r"(r.v[0]), "+r"(r.v[1]) : "r"(k2), "r"(c2));
 #else
   uint64_t c = 0;
   for (int i = 0; i < 8; i++) {
@@ -176,7 +175,7 @@ IBFT_FN_ADD fe fe_add(fe a, fe b) {
     c >>= 32;
   }
   uint32_t k = (uint32_t)c;
-  uint64_t d = (uint64_t)r.v[0] + k * IBFT_PC;
+  uint64_t d = (uint64_t)r.v[0] + ((0u - k) & IBFT_PC);
   r.v[0] = (uint32_t)d;
   d >>= 32;
   d += (uint64_t)r.v[1] + k;
@@ -188,13 +187,10 @@ IBFT_FN_ADD fe fe_add(fe a, fe b) {
     d >>= 32;
   }
   uint32_t k2 = (uint32_t)d;
-  d = (uint64_t)r.v[0] + k2 * IBFT_PC;
+  d = (uint64_t)r.v[0] + ((0u - k2) & IBFT_PC);
   r.v[0] = (uint32_t)d;
   d >>= 32;
-  d += (uint64_t)r.v[1] + k2;
-  r.v[1] = (uint32_t)d;
-  d >>= 32;
-  r.v[2] += (uint32_t)d;
+  r.v[1] += (uint32_t)d + k2;
 #endif
   return r;
 }
@@ -210,19 +206,17 @@ IBFT_FN_ADD fe fe_sub(fe a, fe b) {
         "=r"(c)
       : "r"(a.v[0]), "r"(a.v[1]), "r"(a.v[2]), "r"(a.v[3]), "r"(a.v[4]), "r"(a.v[5]), "r"(a.v[6]), "r"(a.v[7]),
         "r"(b.v[0]), "r"(b.v[1]), "r"(b.v[2]), "r"(b.v[3]), "r"(b.v[4]), "r"(b.v[5]), "r"(b.v[6]), "r"(b.v[7]));
-  // c = 0 or 0xFFFFFFFF (borrow).  a-b+2^256 = a-b+C (mod p)  =>  subtract C on borrow.
-  uint32_t m = c & 1u, k = m * IBFT_PC, c2;
+  // c = 0 or 0xFFFFFFFF (borrow).  a-b+2^256 = a-b+C (mod p)  =>  subtract C on borrow.  The borrow is a mask: C's words are ANDs.
+  uint32_t m = c & 1u, k = c & IBFT_PC, c2;
   asm("sub.cc.u32 %0,%0,%9;\n\tsubc.cc.u32 %1,%1,%10;\n\tsubc.cc.u32 %2,%2,0;\n\tsubc.cc.u32 %3,%3,0;\n\t"
       "subc.cc.u32 %4,%4,0;\n\tsubc.cc.u32 %5,%5,0;\n\tsubc.cc.u32 %6,%6,0;\n\tsubc.cc.u32 %7,%7,0;\n\t"
       "subc.u32 %8,0,0;"
       : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2]), "+r"(r.v[3]), "+r"(r.v[4]), "+r"(r.v[5]), "+r"(r.v[6]), "+r"(r.v[7]),
         "=r"(c2)
       : "r"(k), "r"(m));
-  // a second borrow leaves a value >= 2^256 - 2^34: subtracting C again cannot ripple past limb 2
-  uint32_t m2 = c2 & 1u, k2 = m2 * IBFT_PC;
-  asm("sub.cc.u32 %0,%0,%3;\n\tsubc.cc.u32 %1,%1,%4;\n\tsubc.u32 %2,%2,0;"
-      : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2])
-      : "r"(k2), "r"(m2));
+  // a second borrow leaves a value >= 2^256 - 2^34 (limb 1 >= 2^32 - 4): subtracting C again cannot ripple past limb 1
+  uint32_t m2 = c2 & 1u, k2 = c2 & IBFT_PC;
+  asm("sub.cc.u32 %0,%0,%2;\n\tsubc.u32 %1,%1,%3;" : "+r"(r.v[0]), "+r"(r.v[1]) : "r"(k2), "r"(m2));
 #else
   int64_t c = 0;
   for (int i = 0; i < 8; i++) {
@@ -231,7 +225,7 @@ IBFT_FN_ADD fe fe_sub(fe a, fe b) {
     c >>= 32;  // arithmetic shift: 0 or -1
   }
   uint32_t m = (uint32_t)(-c);
-  int64_t d = (int64_t)r.v[0] - (int64_t)(m * IBFT_PC);
+  int64_t d = (int64_t)r.v[0] - (int64_t)((0u - m) & IBFT_PC);
   r.v[0] = (uint32_t)d;
   d >>= 32;
   d += (int64_t)r.v[1] - (int64_t)m;
@@ -243,19 +237,172 @@ IBFT_FN_ADD fe fe_sub(fe a, fe b) {
     d >>= 32;
   }
   uint32_t m2 = (uint32_t)(-d);
-  d = (int64_t)r.v[0] - (int64_t)(m2 * IBFT_PC);
+  d = (int64_t)r.v[0] - (int64_t)((0u - m2) & IBFT_PC);
   r.v[0] = (uint32_t)d;
   d >>= 32;
-  d += (int64_t)r.v[1] - (int64_t)m2;
-  r.v[1] = (uint32_t)d;
-  d >>= 32;
-  r.v[2] += (uint32_t)d;
+  r.v[1] += (uint32_t)d - m2;
 #endif
   return r;
 }
 
 IBFT_HD fe fe_neg(const fe& a) { return fe_sub(fe_zero(), a); }
 IBFT_HD fe fe_dbl(const fe& a) { return fe_add(a, a); }
+
+// ------------------------------------------------------------------------------------------------
+// fused small linear combinations of the group law (3A, 2 (T - A - C), F - 2D, M - 8C, R^2 - HHH - 2V, +-S2 - Y1)
+// ------------------------------------------------------------------------------------------------
+// Chained fe_add / fe_sub fold after every step: a carry chain over the limbs plus a fold chain each.  These keep one signed
+// accumulator word above the eight limbs instead, take one chain per operand (funnel shifts for the small multiples) and fold
+// once.  Same contract as fe_add / fe_sub: any inputs < 2^256, a result < 2^256 congruent mod p.
+struct fe9 {
+  uint32_t v[8];
+  uint32_t t;  // value = v + t * 2^256, t a small signed word (two's complement)
+};
+IBFT_HD fe9 fe9_from(const fe& a) {
+  fe9 r;
+#pragma unroll
+  for (int i = 0; i < 8; i++) r.v[i] = a.v[i];
+  r.t = 0;
+  return r;
+}
+// a * 2^S, S = 1..3
+template <int S>
+IBFT_HD fe9 fe9_shl(const fe& a) {
+  fe9 r;
+  r.v[0] = a.v[0] << S;
+#pragma unroll
+  for (int i = 1; i < 8; i++) r.v[i] = (a.v[i] << S) | (a.v[i - 1] >> (32 - S));
+  r.t = a.v[7] >> (32 - S);
+  return r;
+}
+template <int S>
+IBFT_HD fe9 fe9_shl(const fe9& a) {
+  fe r;
+#pragma unroll
+  for (int i = 0; i < 8; i++) r.v[i] = a.v[i];
+  fe9 o = fe9_shl<S>(r);
+  o.t |= a.t << S;
+  return o;
+}
+// x += b, x -= b, x -= b9
+IBFT_HD void fe9_add(fe9& x, const fe& b) {
+#if IBFT_PTX
+  asm("add.cc.u32 %0,%0,%9;\n\taddc.cc.u32 %1,%1,%10;\n\taddc.cc.u32 %2,%2,%11;\n\taddc.cc.u32 %3,%3,%12;\n\t"
+      "addc.cc.u32 %4,%4,%13;\n\taddc.cc.u32 %5,%5,%14;\n\taddc.cc.u32 %6,%6,%15;\n\taddc.cc.u32 %7,%7,%16;\n\t"
+      "addc.u32 %8,%8,0;"
+      : "+r"(x.v[0]), "+r"(x.v[1]), "+r"(x.v[2]), "+r"(x.v[3]), "+r"(x.v[4]), "+r"(x.v[5]), "+r"(x.v[6]), "+r"(x.v[7]), "+r"(x.t)
+      : "r"(b.v[0]), "r"(b.v[1]), "r"(b.v[2]), "r"(b.v[3]), "r"(b.v[4]), "r"(b.v[5]), "r"(b.v[6]), "r"(b.v[7]));
+#else
+  uint64_t c = 0;
+  for (int i = 0; i < 8; i++) {
+    c += (uint64_t)x.v[i] + b.v[i];
+    x.v[i] = (uint32_t)c;
+    c >>= 32;
+  }
+  x.t += (uint32_t)c;
+#endif
+}
+IBFT_HD void fe9_sub(fe9& x, const fe& b, uint32_t bt = 0) {
+#if IBFT_PTX
+  asm("sub.cc.u32 %0,%0,%9;\n\tsubc.cc.u32 %1,%1,%10;\n\tsubc.cc.u32 %2,%2,%11;\n\tsubc.cc.u32 %3,%3,%12;\n\t"
+      "subc.cc.u32 %4,%4,%13;\n\tsubc.cc.u32 %5,%5,%14;\n\tsubc.cc.u32 %6,%6,%15;\n\tsubc.cc.u32 %7,%7,%16;\n\t"
+      "subc.u32 %8,%8,%17;"
+      : "+r"(x.v[0]), "+r"(x.v[1]), "+r"(x.v[2]), "+r"(x.v[3]), "+r"(x.v[4]), "+r"(x.v[5]), "+r"(x.v[6]), "+r"(x.v[7]), "+r"(x.t)
+      : "r"(b.v[0]), "r"(b.v[1]), "r"(b.v[2]), "r"(b.v[3]), "r"(b.v[4]), "r"(b.v[5]), "r"(b.v[6]), "r"(b.v[7]), "r"(bt));
+#else
+  int64_t c = 0;
+  for (int i = 0; i < 8; i++) {
+    c += (int64_t)x.v[i] - (int64_t)b.v[i];
+    x.v[i] = (uint32_t)c;
+    c >>= 32;  // 0 or -1
+  }
+  x.t += (uint32_t)c - bt;
+#endif
+}
+IBFT_HD void fe9_sub(fe9& x, const fe9& b) {
+  fe lo;
+#pragma unroll
+  for (int i = 0; i < 8; i++) lo.v[i] = b.v[i];
+  fe9_sub(x, lo, b.t);
+}
+// x + e mod p, |t| <= 8, e <= 1: one chain adds t * (2^32 + 977) + e (2^256 = 2^32 + 977 mod p) as a 256-bit two's-complement
+// word, whose carry leaves a top t2 in {-1, 0, 1}.  t2 = 1 leaves a value below |t| (2^32 + 977) + 1 < 2^36, t2 = -1 one at or
+// above 2^256 - 2^36: adding t2 (2^32 + 977) to the low two limbs cannot ripple further.
+IBFT_HD fe fe9_fold(const fe9& x, uint32_t e = 0) {
+  fe r;
+#pragma unroll
+  for (int i = 0; i < 8; i++) r.v[i] = x.v[i];
+  const uint32_t s = (uint32_t)((int32_t)x.t >> 31);
+  const uint32_t lo = x.t * IBFT_PC + e, hi = x.t + s;  // (t (2^32 + 977) + e) mod 2^64; the words above it are s
+  uint32_t t2;
+#if IBFT_PTX
+  asm("add.cc.u32 %0,%0,%9;\n\taddc.cc.u32 %1,%1,%10;\n\taddc.cc.u32 %2,%2,%11;\n\taddc.cc.u32 %3,%3,%11;\n\t"
+      "addc.cc.u32 %4,%4,%11;\n\taddc.cc.u32 %5,%5,%11;\n\taddc.cc.u32 %6,%6,%11;\n\taddc.cc.u32 %7,%7,%11;\n\t"
+      "addc.u32 %8,%11,0;"
+      : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2]), "+r"(r.v[3]), "+r"(r.v[4]), "+r"(r.v[5]), "+r"(r.v[6]), "+r"(r.v[7]), "=r"(t2)
+      : "r"(lo), "r"(hi), "r"(s));
+  const uint32_t lo2 = t2 * IBFT_PC, hi2 = t2 + (uint32_t)((int32_t)t2 >> 31);
+  asm("add.cc.u32 %0,%0,%2;\n\taddc.u32 %1,%1,%3;" : "+r"(r.v[0]), "+r"(r.v[1]) : "r"(lo2), "r"(hi2));
+#else
+  uint64_t c = (uint64_t)r.v[0] + lo;
+  r.v[0] = (uint32_t)c;
+  c >>= 32;
+  c += (uint64_t)r.v[1] + hi;
+  r.v[1] = (uint32_t)c;
+  c >>= 32;
+  for (int i = 2; i < 8; i++) {
+    c += (uint64_t)r.v[i] + s;
+    r.v[i] = (uint32_t)c;
+    c >>= 32;
+  }
+  t2 = (uint32_t)c + s;
+  const uint32_t lo2 = t2 * IBFT_PC, hi2 = t2 + (uint32_t)((int32_t)t2 >> 31);
+  c = (uint64_t)r.v[0] + lo2;
+  r.v[0] = (uint32_t)c;
+  c >>= 32;
+  r.v[1] += (uint32_t)c + hi2;
+#endif
+  return r;
+}
+
+// 3a (t in [0, 2])
+IBFT_HD fe fe_mul3(const fe& a) {
+  fe9 x = fe9_shl<1>(a);
+  fe9_add(x, a);
+  return fe9_fold(x);
+}
+// a - 2^S b, S = 1..3 (t in [-2^S, 0])
+template <int S>
+IBFT_HD fe fe_sub_shl(const fe& a, const fe& b) {
+  fe9 x = fe9_from(a);
+  fe9_sub(x, fe9_shl<S>(b));
+  return fe9_fold(x);
+}
+// a - b - 2c (t in [-3, 0])
+IBFT_HD fe fe_sub_sub_dbl(const fe& a, const fe& b, const fe& c) {
+  fe9 x = fe9_from(a);
+  fe9_sub(x, b);
+  fe9_sub(x, fe9_shl<1>(c));
+  return fe9_fold(x);
+}
+// 2 (a - b - c) (t in [-4, 1])
+IBFT_HD fe fe_dbl_sub_sub(const fe& a, const fe& b, const fe& c) {
+  fe9 x = fe9_from(a);
+  fe9_sub(x, b);
+  fe9_sub(x, c);
+  return fe9_fold(fe9_shl<1>(x));
+}
+// a - b, or -a - b when neg: -a = ~a + 1 - 2^256, the complement read as a 9-limb value with top -1 and the + 1 added by the
+// fold (t in [-2, 0])
+IBFT_HD fe fe_sub_signed(const fe& a, const fe& b, bool neg) {
+  const uint32_t m = neg ? 0xFFFFFFFFu : 0u;
+  fe9 x;
+#pragma unroll
+  for (int i = 0; i < 8; i++) x.v[i] = a.v[i] ^ m;
+  x.t = m;
+  fe9_sub(x, b);
+  return fe9_fold(x, m & 1u);
+}
 
 // canonical representative in [0, p)
 IBFT_HD fe fe_normalize(const fe& a) {

@@ -26,7 +26,7 @@ QUORUM_DEFAULT, QUORUM_PREPREPARE, QUORUM_PREPARE = 0, 1, 2
 PROPOSER_NONE, PROPOSER_UNSET = 0xFFFFFFFF, 0xFFFFFFFE
 DBG = dict(FE_MUL=1, FE_SQR=2, FE_INV=3, FE_SQRT=4, SC_MUL=5, SC_INV=6, ECMULT=7, FE_ADD=8, FE_SUB=9, GLV=10,
            FE_MUL_RAW=11, FE_SQR_RAW=12, FE_ADD_RAW=13, FE_SUB_RAW=14, FE_NORMALIZE=15, FE_EQUAL=16, FE_SQRN=17, FE_SQRT_INV=18,
-           SC_ADD=19, SC_NEG=20, SC_REDUCE_ONCE=21, SC_DIGITS=22, RFC6979=23, KEY_ADDRESS=24)
+           SC_ADD=19, SC_NEG=20, SC_REDUCE_ONCE=21, SC_DIGITS=22, RFC6979=23, KEY_ADDRESS=24, FE_FUSED=25)
 
 # numpy mirrors of the ABI structs
 ITEM_DTYPE = np.dtype([

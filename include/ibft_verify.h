@@ -551,6 +551,9 @@ int ibft_probe_int_peak(ibft_engine* e, double* imad_per_s, double* wide_mac_per
                                     * registry entry of the address in the first 20 bytes of c (x, y < p, on the curve, hashing
                                     * to the address), else 0: the check of a key one device of a multi-device engine adopts
                                     * from another */
+#define IBFT_DBG_FE_FUSED 25       /* out = one fused linear combination of the group law, raw; c = a third operand (32 bytes) and
+                                    * the selector in c[63]: 0 = 3a, 1 = a - 2b, 2 = a - 8b, 3 = a - b - 2c, 4 = 2 (a - b - c),
+                                    * 5 = a - b and 6 = -a - b (the sign-selected subtraction of the mixed addition) */
 /* Generator comb tables (builds with IBFT_WC > 0): *wc = window (0 when absent), *entries = entries of one comb position;
  * copies `count` 64-byte entries (x, y as 8 little-endian words each) starting at `first`, positions laid out one after the
  * other: entry p * entries + d1 * (2^wc + 1) + d2 + 2^(wc-1) holds (d1 + d2*lambda) * 2^(wc*p) * G, p = 0..16 (position 0 is
