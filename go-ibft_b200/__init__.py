@@ -8,4 +8,5 @@ from .engine import (Engine, EngineError, GROUP_DTYPE, ITEM_DTYPE, KIND_DIGEST, 
                      NO_TABLE, PROPOSER_NONE, PROPOSER_UNSET, QUORUM_DEFAULT, QUORUM_PREPARE, QUORUM_PREPREPARE, RESULT_DTYPE,
                      REASON_BAD_V, REASON_INCONSISTENT, REASON_MALFORMED, REASON_NEEDS_HOST, REASON_NO_GROUP, REASON_NO_KEY,
                      REASON_NOT_VALIDATOR, REASON_OK, REASON_R_NOT_X, REASON_R_RANGE, REASON_S_RANGE, REASON_SIGNER_MISMATCH,
-                     group_descs, load_library)
+                     group_descs, load_library,
+                     GROUP_HASH_DTYPE, HASH_COMMIT, HASH_PREPARE, HASH_UNBOUND, group_hashes)

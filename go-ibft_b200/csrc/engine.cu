@@ -28,6 +28,7 @@
 
 #include "../../include/ibft_verify.h"
 #include "verify_core.cuh"
+#include "group_hash.cuh"
 #include "debug_arith.cuh"
 #include "key_share.cuh"
 #include "key_budget.hpp"
@@ -39,6 +40,7 @@ using namespace ibft;
 
 static_assert(sizeof(ibft_sig_item) == 128, "packed item must be 128 bytes");
 static_assert(sizeof(ibft_group_desc) == 16, "group descriptor must be 16 bytes");
+static_assert(sizeof(ibft_group_hash) == 48, "group hash binding must be 48 bytes");
 static_assert(IBFT_GTABLE_WG == IBFT_WG, "regenerate secp_gtable.inc (tools/gen_tables.py) for this IBFT_WG");
 
 #define IBFT_BLOCK 128
@@ -1049,6 +1051,42 @@ __global__ void k_quorum_mark(const ibft_sig_item* __restrict__ items, uint32_t 
   if (v >= 0) atomicOr(&voted[gdev[g].voted_off + ((uint32_t)v >> 5)], 1u << (v & 31));
 }
 
+// k_quorum_mark for calls in which a group is bound to the accepted proposal's hash (ibft_group_hash): an item of a bound group
+// counts -- enters the voted set and the valid count -- only when it names the bound hash (item_names_hash, group_hash.cuh); an
+// item of an unbound group counts when its verdict bit is set, as in k_quorum_mark.  counted (nullptr: not wanted) receives one
+// bit per item of [lo, hi), each by an atomic bit update, so that shards may share a bitmap whatever their bounds.  A separate
+// kernel: k_quorum_mark and the recover kernels' fused marking stay as they are, and the recover kernels run without a vote sink
+// when a call binds hashes (DESIGN.md §3.2).
+__global__ void k_quorum_mark_hashed(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __restrict__ arena,
+                                     size_t arena_len, const uint32_t* __restrict__ bitmap, const ibft_group_desc* __restrict__ groups,
+                                     const ibft_group_hash* __restrict__ ghash, const group_dev* __restrict__ gdev, uint32_t n_groups,
+                                     const slot_dev* __restrict__ slots, uint32_t n_slots, uint32_t* __restrict__ voted,
+                                     uint32_t* __restrict__ n_valid, uint32_t* __restrict__ counted, uint32_t lo, uint32_t hi) {
+  uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= hi || i >= n) return;
+  const ibft_sig_item* it = items + i;
+  const uint32_t g = it->group;
+  bool c = ((bitmap[i >> 5] >> (i & 31)) & 1u) && g < n_groups;
+  ibft_sig_item local;
+  if (c) {
+    local = *it;
+    const uint32_t mt = ghash != nullptr ? ghash[g].msg_type : IBFT_HASH_UNBOUND;
+    if (mt != IBFT_HASH_UNBOUND) c = item_names_hash(local, arena, arena_len, mt, ghash[g].hash);
+  }
+  if (counted != nullptr) {
+    if (c) atomicOr(&counted[i >> 5], 1u << (i & 31));
+    else atomicAnd(&counted[i >> 5], ~(1u << (i & 31)));
+  }
+  if (!c) return;
+  atomicAdd(&n_valid[g], 1u);
+  uint32_t slot = groups[g].table_slot;
+  if (slot == IBFT_NO_TABLE || slot >= n_slots || !slots[slot].valid) return;
+  uint8_t addr[20];
+  if (!item_signer(local, arena, arena_len, addr)) return;
+  int v = lookup_validator(slots[slot], addr);
+  if (v >= 0) atomicOr(&voted[gdev[g].voted_off + ((uint32_t)v >> 5)], 1u << (v & 31));
+}
+
 // multi-GPU: OR the ranks' partial voted sets and add their valid counts (partial layout: voted words, then one count per group)
 __global__ void k_quorum_merge(const uint32_t* __restrict__ parts, uint32_t n_parts, uint32_t part_stride, uint32_t voted_words,
                                uint32_t n_groups, uint32_t* __restrict__ voted, uint32_t* __restrict__ n_valid) {
@@ -1936,6 +1974,8 @@ struct pending_call {
   uint32_t* bitmap_out = nullptr;
   ibft_group_result* results_out = nullptr;
   uint8_t* recovered_out = nullptr;
+  uint32_t* counted_out = nullptr;
+  bool hashed = false;  // counted bits on the device (a group was bound); else they are the verdict bits
 };
 
 // One LANE = everything a host-buffer verify call needs while it is in flight: streams, events, device buffers, pinned
@@ -1971,6 +2011,8 @@ struct lane {
   uint32_t* d_voted = nullptr;
   uint32_t* d_nvalid = nullptr;
   size_t voted_words_cap = 0;
+  ibft_group_hash* d_ghash = nullptr;  // hash bindings of the groups (ibft_group_hash), when last_hashes is not empty
+  uint32_t* d_counted = nullptr;       // counted bits of a call that binds hashes
   // pinned host staging
   ibft_sig_item* h_items = nullptr;
   uint8_t* h_arena = nullptr;
@@ -1979,8 +2021,11 @@ struct lane {
   ibft_group_desc* h_groups = nullptr;
   group_dev* h_gdev = nullptr;
   ibft_group_result* h_results = nullptr;
+  ibft_group_hash* h_ghash = nullptr;
+  uint32_t* h_counted = nullptr;
   std::vector<group_dev> last_gdev;  // layout of the voted sets of the most recent reduce
   std::vector<ibft_group_desc> last_groups;
+  std::vector<ibft_group_hash> last_hashes;  // hash bindings of last_groups; empty when no group is bound
   pending_call pending;
   uint32_t* d_worklist = nullptr;  // key-registry path: [0] = count, [1..] = indices left to the recover pass
   cudaEvent_t wl_ev[4] = {nullptr, nullptr, nullptr, nullptr};  // last use of each worklist (orders launches that arrive on different streams)
@@ -2032,7 +2077,8 @@ static int multi_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t he
                                 uint32_t n);
 static int multi_verify(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
                         const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
-                        uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words);
+                        uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words,
+                        const ibft_group_hash* ghash = nullptr, uint32_t* counted_out = nullptr);
 static int multi_submit(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
                         const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
                         uint8_t* recovered_out);
@@ -2078,6 +2124,7 @@ static void lane_free(lane* L) {
   cudaFree(L->d_gdev); cudaFree(L->d_results); cudaFree(L->d_voted); cudaFree(L->d_nvalid);
   cudaFreeHost(L->h_items); cudaFreeHost(L->h_arena); cudaFreeHost(L->h_bitmap); cudaFreeHost(L->h_recovered);
   cudaFreeHost(L->h_groups); cudaFreeHost(L->h_gdev); cudaFreeHost(L->h_results);
+  cudaFree(L->d_ghash); cudaFree(L->d_counted); cudaFreeHost(L->h_ghash); cudaFreeHost(L->h_counted);
   if (L->done_ev) cudaEventDestroy(L->done_ev);
   for (auto ev : L->chunk_ev) cudaEventDestroy(ev);
   if (L->copy_stream) cudaStreamDestroy(L->copy_stream);
@@ -2207,6 +2254,10 @@ static int lane_alloc(ibft_engine* e, lane* L, uint32_t cap_items, size_t cap_ar
   CU(cudaHostAlloc(&L->h_groups, (size_t)p.max_groups * sizeof(ibft_group_desc), cudaHostAllocDefault));
   CU(cudaHostAlloc(&L->h_gdev, (size_t)p.max_groups * sizeof(group_dev), cudaHostAllocDefault));
   CU(cudaHostAlloc(&L->h_results, (size_t)p.max_groups * sizeof(ibft_group_result), cudaHostAllocDefault));
+  CU(cudaMalloc(&L->d_ghash, std::max<size_t>(p.max_groups, 1) * sizeof(ibft_group_hash)));
+  CU(cudaMalloc(&L->d_counted, std::max<size_t>(words, 1) * 4));
+  CU(cudaHostAlloc(&L->h_ghash, std::max<size_t>(p.max_groups, 1) * sizeof(ibft_group_hash), cudaHostAllocDefault));
+  CU(cudaHostAlloc(&L->h_counted, std::max<size_t>(words, 1) * 4, cudaHostAllocDefault));
   return IBFT_OK;
 }
 
@@ -3055,6 +3106,28 @@ static int plan_groups(ibft_engine* e, lane* L, const ibft_group_desc* groups, u
   return IBFT_OK;
 }
 
+// Validates the hash bindings of a call's groups (ibft_group_hash); *any_bound = at least one group is bound
+static int check_group_hashes(const ibft_group_desc* groups, uint32_t n_groups, const ibft_group_hash* hashes, bool* any_bound) {
+  *any_bound = false;
+  for (uint32_t g = 0; g < n_groups; g++) {
+    const ibft_group_hash& h = hashes[g];
+    if (h.reserved[0] | h.reserved[1] | h.reserved[2]) { set_err("group hash %u: reserved words must be zero", g); return IBFT_ERR_INVALID_ARG; }
+    if (h.msg_type == IBFT_HASH_UNBOUND) continue;
+    const uint32_t rule = groups[g].flags & IBFT_QUORUM_RULE_MASK;
+    if (h.msg_type != IBFT_HASH_PREPARE && h.msg_type != IBFT_HASH_COMMIT) {
+      set_err("group hash %u: msg_type %u is not PREPARE (1), COMMIT (2) or IBFT_HASH_UNBOUND", g, h.msg_type);
+      return IBFT_ERR_INVALID_ARG;
+    }
+    const bool fits = rule == IBFT_QUORUM_DEFAULT || (rule == IBFT_QUORUM_PREPARE && h.msg_type == IBFT_HASH_PREPARE);
+    if (!fits) {
+      set_err("group %u: quorum rule %u cannot be bound to %s hashes", g, rule, h.msg_type == IBFT_HASH_PREPARE ? "PREPARE" : "COMMIT");
+      return IBFT_ERR_INVALID_ARG;
+    }
+    *any_bound = true;
+  }
+  return IBFT_OK;
+}
+
 static int launch_recover(ibft_engine* e, lane* L, const ibft_sig_item* d_items, uint32_t n, const uint8_t* d_arena, size_t arena_len,
                           uint32_t lo, uint32_t hi, const ibft_group_desc* d_groups, uint32_t n_groups, uint32_t* d_bitmap,
                           uint8_t* d_recovered, cudaStream_t st, uint8_t* d_status = nullptr, int forced_path = IBFT_PATH_AUTO,
@@ -3180,13 +3253,19 @@ static int launch_recover(ibft_engine* e, lane* L, const ibft_sig_item* d_items,
 
 static int launch_quorum(ibft_engine* e, lane* L, const ibft_sig_item* d_items, uint32_t n, const uint8_t* d_arena, size_t arena_len, const uint32_t* d_bitmap,
                          const ibft_group_desc* d_groups, const group_dev* d_gdev, uint32_t n_groups, size_t voted_words,
-                         ibft_group_result* d_results, cudaStream_t st, bool already_marked = false) {
+                         ibft_group_result* d_results, cudaStream_t st, bool already_marked = false,
+                         const ibft_group_hash* d_ghash = nullptr, uint32_t* d_counted = nullptr) {
   if (n_groups == 0) return IBFT_OK;
   if (!already_marked) {
     CU(cudaMemsetAsync(L->d_voted, 0, std::max<size_t>(voted_words, 1) * 4, st));
     CU(cudaMemsetAsync(L->d_nvalid, 0, (size_t)n_groups * 4, st));
   }
-  if (n && !already_marked) {
+  if (n && !already_marked && (d_ghash != nullptr || d_counted != nullptr)) {
+    k_quorum_mark_hashed<<<(n + 255) / 256, 256, 0, st>>>(d_items, n, d_arena, arena_len, d_bitmap, d_groups, d_ghash, d_gdev, n_groups,
+                                                           e->d_slots, e->p.max_table_slots, L->d_voted, L->d_nvalid, d_counted, 0u, n);
+    e->launches++;
+    CU(cudaGetLastError());
+  } else if (n && !already_marked) {
     k_quorum_mark<<<(n + 255) / 256, 256, 0, st>>>(d_items, n, d_arena, arena_len, d_bitmap, d_groups, d_gdev, n_groups, e->d_slots,
                                                     e->p.max_table_slots, L->d_voted, L->d_nvalid, 0u, n);
     e->launches++;
@@ -3219,8 +3298,10 @@ static void stage_copy(void* dst, const void* src, size_t bytes) {
 
 static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
                          const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
-                         ibft_group_result* results_out, uint8_t* recovered_out, bool votes_only = false) {
+                         ibft_group_result* results_out, uint8_t* recovered_out, bool votes_only = false,
+                         const ibft_group_hash* ghash = nullptr, uint32_t* counted_out = nullptr) {
   // votes_only: a shard of a multi-device call -- record the votes, leave the reduce to the coordinator's merge
+  // ghash: the groups' hash bindings, given only when at least one group is bound (checked by check_group_hashes)
   if (L->pending.active) { set_err("a submitted call is still pending; wait for it first"); return IBFT_ERR_INVALID_ARG; }
   if ((n && !items) || (n && !bitmap_out) || (arena_len && !arena) || (n_groups && !groups)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   if (n > L->cap_items || arena_len > L->cap_arena || n_groups > e->p.max_groups) {
@@ -3242,6 +3323,9 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
     L->last_gdev.clear();
     L->last_groups.clear();
   }
+  if (ghash && n_groups) L->last_hashes.assign(ghash, ghash + n_groups);
+  else L->last_hashes.clear();
+  const bool hashed = !L->last_hashes.empty();
   cudaStream_t st = L->stream;
   if (arena_len) {
     if (arena != L->h_arena) memcpy(L->h_arena, arena, arena_len);  // a shard is planned straight into the staging
@@ -3251,12 +3335,17 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
     CU(cudaMemcpyAsync(L->d_groups, L->h_groups, (size_t)n_groups * sizeof(ibft_group_desc), cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(L->d_gdev, L->h_gdev, (size_t)n_groups * sizeof(group_dev), cudaMemcpyHostToDevice, st));
   }
-  // quorum requested: the recover kernels record the votes themselves (no k_quorum_mark pass over the tuples afterwards)
+  if (hashed) {
+    memcpy(L->h_ghash, ghash, (size_t)n_groups * sizeof(ibft_group_hash));
+    CU(cudaMemcpyAsync(L->d_ghash, L->h_ghash, (size_t)n_groups * sizeof(ibft_group_hash), cudaMemcpyHostToDevice, st));
+  }
+  // quorum requested: the recover kernels record the votes themselves (no k_quorum_mark pass over the tuples afterwards) -- unless
+  // a group is bound to a hash, which their fused marking cannot test: k_quorum_mark_hashed marks the counted items afterwards
   vote_sink sink{nullptr, nullptr, nullptr};
-  if (n_groups && (results_out || votes_only)) {
+  if (n_groups && (results_out || votes_only || hashed)) {
     CU(cudaMemsetAsync(L->d_voted, 0, std::max<size_t>(voted_words, 1) * 4, st));
     CU(cudaMemsetAsync(L->d_nvalid, 0, (size_t)n_groups * 4, st));
-    sink = vote_sink{L->d_voted, L->d_nvalid, L->d_gdev};
+    if (!hashed) sink = vote_sink{L->d_voted, L->d_nvalid, L->d_gdev};
   }
   // Tuples go up in chunks: while the recover kernel works on chunk k, the host stages chunk k+1 into pinned memory and the
   // copy engine moves it (two streams + events).  Small batches are a single chunk.
@@ -3347,6 +3436,14 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
       CU(cudaStreamWaitEvent(st, L->lat_ev[k], 0));
     }
   }
+  if (hashed && n) {
+    k_quorum_mark_hashed<<<(n + 255) / 256, 256, 0, st>>>(L->d_items, n, L->d_arena, arena_len, L->d_bitmap, L->d_groups, L->d_ghash, L->d_gdev,
+                                                           n_groups, e->d_slots, e->p.max_table_slots, L->d_voted, L->d_nvalid, L->d_counted,
+                                                           0u, n);
+    e->launches++;
+    CU(cudaGetLastError());
+    if (counted_out) CU(cudaMemcpyAsync(L->h_counted, L->d_counted, (size_t)((n + 31) / 32) * 4, cudaMemcpyDeviceToHost, st));
+  }
   if (n_groups && results_out) {
     rc = launch_quorum(e, L, L->d_items, n, L->d_arena, arena_len, L->d_bitmap, L->d_groups, L->d_gdev, n_groups, voted_words, L->d_results, st,
                        /*already_marked=*/true);
@@ -3365,6 +3462,8 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
   L->pending.bitmap_out = bitmap_out;
   L->pending.results_out = results_out;
   L->pending.recovered_out = recovered_out;
+  L->pending.counted_out = counted_out;
+  L->pending.hashed = hashed;
   return IBFT_OK;
 }
 
@@ -3387,6 +3486,10 @@ static int wait_locked(ibft_engine* e, lane* L) {
     memcpy(pc.bitmap_out, L->h_bitmap, words * 4);
     if (pc.n & 31) pc.bitmap_out[words - 1] &= (1u << (pc.n & 31)) - 1u;
     if (pc.recovered_out) memcpy(pc.recovered_out, L->h_recovered, (size_t)pc.n * 20);
+    if (pc.counted_out) {
+      memcpy(pc.counted_out, pc.hashed ? L->h_counted : L->h_bitmap, words * 4);
+      if (pc.n & 31) pc.counted_out[words - 1] &= (1u << (pc.n & 31)) - 1u;
+    }
   }
   if (pc.n_groups) memcpy(pc.results_out, L->h_results, (size_t)pc.n_groups * sizeof(ibft_group_result));
   e->last_lane.store((int)(L - e->lanes));
@@ -3434,8 +3537,9 @@ static int copy_voted(ibft_engine* e, lane* L, uint32_t n_groups, bool recorded,
 
 static int verify_batch_on_lane(ibft_engine* e, lane* L, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
                                 const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
-                                uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words) {
-  int rc = submit_locked(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out);
+                                uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words,
+                                const ibft_group_hash* ghash = nullptr, uint32_t* counted_out = nullptr) {
+  int rc = submit_locked(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, false, ghash, counted_out);
   if (rc != IBFT_OK) return rc;
   rc = wait_locked(e, L);
   if (rc != IBFT_OK) return rc;
@@ -3469,6 +3573,33 @@ extern "C" int ibft_verify_batch_ex(ibft_engine* e, const ibft_sig_item* items, 
   std::lock_guard<std::mutex> lk(L->mu, std::adopt_lock);
   return verify_batch_on_lane(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, status_out, voted_out,
                               voted_stride_words);
+}
+
+extern "C" int ibft_verify_batch_hashed(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                                        const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
+                                        ibft_group_result* results_out, uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out,
+                                        uint32_t voted_stride_words, const ibft_group_hash* group_hashes, uint32_t* counted_out) {
+  if (!e) { set_err("null engine"); return IBFT_ERR_INVALID_ARG; }
+  if (voted_out && !results_out) { set_err("voted_out needs results_out (votes are recorded only when quorum results are requested)"); return IBFT_ERR_INVALID_ARG; }
+  IBFT_REFUSE_VIEW(e);
+  if (n_groups && !groups) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  bool bound = false;
+  if (group_hashes) {
+    if (n_groups > e->p.max_groups) {
+      set_err("batch (%u groups) exceeds engine capacity (%u)", n_groups, e->p.max_groups);
+      return IBFT_ERR_CAPACITY;
+    }
+    int rc = check_group_hashes(groups, n_groups, group_hashes, &bound);
+    if (rc != IBFT_OK) return rc;
+  }
+  const ibft_group_hash* ghash = bound ? group_hashes : nullptr;  // no group bound: the call is ibft_verify_batch_ex
+  if (e->multi)
+    return multi_verify(e, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, status_out, voted_out,
+                        voted_stride_words, ghash, counted_out);
+  lane* L = acquire_lane(e, n, arena_len);
+  std::lock_guard<std::mutex> lk(L->mu, std::adopt_lock);
+  return verify_batch_on_lane(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, status_out, voted_out,
+                              voted_stride_words, ghash, counted_out);
 }
 
 extern "C" int ibft_last_item_status(ibft_engine* e, uint8_t* status_out, uint32_t n) {
@@ -3678,11 +3809,45 @@ extern "C" int ibft_bind_groups(ibft_engine* e, const ibft_group_desc* groups, u
     L->last_gdev.clear();
     L->last_groups.clear();
   }
+  L->last_hashes.clear();  // new groups: any hash binding was for the previous ones
+  return IBFT_OK;
+}
+
+// binds the groups of the device-resident calls to the accepted proposal's hash (ibft_group_hash); NULL unbinds
+extern "C" int ibft_bind_group_hashes(ibft_engine* e, const ibft_group_hash* hashes, uint32_t n_groups) {
+  IBFT_REFUSE_MULTI(e);
+  if (!e) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
+  lane* L = &e->lanes[0];
+  std::lock_guard<std::mutex> lk(L->mu);
+  if (hashes == nullptr) {
+    L->last_hashes.clear();
+    return IBFT_OK;
+  }
+  if (n_groups != L->last_groups.size()) {
+    set_err("%u hash bindings for %zu bound groups: call ibft_bind_groups with the same groups first", n_groups, L->last_groups.size());
+    return IBFT_ERR_INVALID_ARG;
+  }
+  bool bound = false;
+  int rc = check_group_hashes(L->last_groups.data(), n_groups, hashes, &bound);
+  if (rc != IBFT_OK) return rc;
+  if (!bound) {
+    L->last_hashes.clear();
+    return IBFT_OK;
+  }
+  CU(cudaSetDevice(e->p.device));
+  memcpy(L->h_ghash, hashes, (size_t)n_groups * sizeof(ibft_group_hash));
+  CU(cudaMemcpy(L->d_ghash, L->h_ghash, (size_t)n_groups * sizeof(ibft_group_hash), cudaMemcpyHostToDevice));
+  L->last_hashes.assign(hashes, hashes + n_groups);
   return IBFT_OK;
 }
 
 extern "C" int ibft_quorum_reduce_device(ibft_engine* e, const void* d_items, uint32_t n, const void* d_bitmap,
                                          const void* d_groups, uint32_t n_groups, void* d_results, void* stream) {
+  return ibft_quorum_reduce_device_ex(e, d_items, n, d_bitmap, d_groups, n_groups, d_results, nullptr, stream);
+}
+
+extern "C" int ibft_quorum_reduce_device_ex(ibft_engine* e, const void* d_items, uint32_t n, const void* d_bitmap, const void* d_groups,
+                                            uint32_t n_groups, void* d_results, void* d_counted, void* stream) {
   IBFT_REFUSE_MULTI(e);
   if (!e || !d_results || (n && (!d_items || !d_bitmap))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
@@ -3694,7 +3859,8 @@ extern "C" int ibft_quorum_reduce_device(ibft_engine* e, const void* d_items, ui
   size_t voted_words = 0;
   for (auto& g : L->last_gdev) voted_words += g.n_words;
   return launch_quorum(e, L, (const ibft_sig_item*)d_items, n, L->dev_arena, L->dev_arena_len, (const uint32_t*)d_bitmap, L->d_groups,
-                       L->d_gdev, n_groups, voted_words, (ibft_group_result*)d_results, st);
+                       L->d_gdev, n_groups, voted_words, (ibft_group_result*)d_results, st, false,
+                       L->last_hashes.empty() ? nullptr : L->d_ghash, (uint32_t*)d_counted);
 }
 
 extern "C" int ibft_quorum_partial_words(ibft_engine* e, uint32_t* words_out) {
@@ -3710,6 +3876,11 @@ extern "C" int ibft_quorum_partial_words(ibft_engine* e, uint32_t* words_out) {
 
 extern "C" int ibft_quorum_mark_device(ibft_engine* e, const void* d_items, uint32_t n, uint32_t shard_lo, uint32_t shard_hi,
                                        const void* d_bitmap, void* d_partial, void* stream) {
+  return ibft_quorum_mark_device_ex(e, d_items, n, shard_lo, shard_hi, d_bitmap, d_partial, nullptr, stream);
+}
+
+extern "C" int ibft_quorum_mark_device_ex(ibft_engine* e, const void* d_items, uint32_t n, uint32_t shard_lo, uint32_t shard_hi,
+                                          const void* d_bitmap, void* d_partial, void* d_counted, void* stream) {
   IBFT_REFUSE_MULTI(e);
   if (!e || !d_partial || (n && (!d_items || !d_bitmap))) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   if (shard_hi > n || shard_lo > shard_hi) { set_err("bad shard"); return IBFT_ERR_INVALID_ARG; }
@@ -3723,7 +3894,14 @@ extern "C" int ibft_quorum_mark_device(ibft_engine* e, const void* d_items, uint
   for (auto& g : L->last_gdev) voted_words += g.n_words;
   uint32_t* part = (uint32_t*)d_partial;
   CU(cudaMemsetAsync(part, 0, (voted_words + n_groups) * 4, st));
-  if (shard_hi > shard_lo) {
+  if (shard_hi > shard_lo && (!L->last_hashes.empty() || d_counted != nullptr)) {
+    k_quorum_mark_hashed<<<(shard_hi - shard_lo + 255) / 256, 256, 0, st>>>(
+        (const ibft_sig_item*)d_items, n, L->dev_arena, L->dev_arena_len, (const uint32_t*)d_bitmap, L->d_groups,
+        L->last_hashes.empty() ? nullptr : L->d_ghash, L->d_gdev, n_groups, e->d_slots, e->p.max_table_slots, part, part + voted_words,
+        (uint32_t*)d_counted, shard_lo, shard_hi);
+    e->launches++;
+    CU(cudaGetLastError());
+  } else if (shard_hi > shard_lo) {
     k_quorum_mark<<<(shard_hi - shard_lo + 255) / 256, 256, 0, st>>>((const ibft_sig_item*)d_items, n, L->dev_arena, L->dev_arena_len,
                                                                      (const uint32_t*)d_bitmap, L->d_groups, L->d_gdev, n_groups, e->d_slots,
                                                                      e->p.max_table_slots, part, part + voted_words, shard_lo, shard_hi);
@@ -4081,8 +4259,10 @@ struct multi_call {
   uint32_t* bitmap_out = nullptr;
   ibft_group_result* results_out = nullptr;
   uint8_t* recovered_out = nullptr;
-  std::vector<std::vector<uint32_t>> bitmap;   // each shard's verdict words and recovered addresses, until every device is done
-  std::vector<std::vector<uint8_t>> recovered;
+  uint32_t* counted_out = nullptr;
+  std::vector<std::vector<uint32_t>> bitmap;   // each shard's verdict words, recovered addresses and counted words, until every
+  std::vector<std::vector<uint8_t>> recovered; // device is done
+  std::vector<std::vector<uint32_t>> counted;
 };
 
 // a slot's table as the devices hold it, for the roll-back of a replication that failed part way
@@ -4202,7 +4382,8 @@ static int multi_merge_enqueue(multi_engine* M, int kind, uint32_t used, uint32_
 // caller's buffers here.
 static int multi_submit_locked(ibft_engine* E, int kind, uint32_t used, const ibft_sig_item* items, uint32_t n, const uint8_t* arena,
                                size_t arena_len, const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
-                               ibft_group_result* results_out, uint8_t* recovered_out, multi_call& mc) {
+                               ibft_group_result* results_out, uint8_t* recovered_out, multi_call& mc,
+                               const ibft_group_hash* ghash = nullptr, uint32_t* counted_out = nullptr) {
   multi_engine* M = E->multi;
   ibft_engine* lead = M->subs[0];
   lane* L0 = &lead->lanes[kind];
@@ -4215,8 +4396,10 @@ static int multi_submit_locked(ibft_engine* E, int kind, uint32_t used, const ib
   mc.bitmap_out = bitmap_out;
   mc.results_out = results_out;
   mc.recovered_out = recovered_out;
+  mc.counted_out = counted_out;
   if (used == 1) {  // the lead's own call, as on a single-device engine
-    int rc = submit_locked(lead, L0, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out);
+    int rc = submit_locked(lead, L0, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, false, ghash,
+                           counted_out);
     mc.active = rc == IBFT_OK;
     return rc;
   }
@@ -4236,6 +4419,7 @@ static int multi_submit_locked(ibft_engine* E, int kind, uint32_t used, const ib
   mc.merge = n_groups && results_out;
   mc.bitmap.resize(used);
   mc.recovered.resize(used);
+  mc.counted.resize(used);
   // each device plans its shard into its own pinned staging: large pageable batches are staged on all devices at once
   const bool parallel = (uint64_t)n * sizeof(ibft_sig_item) + arena_len >= (4u << 20);
   int rc = for_devices(used, parallel, [&](uint32_t k) {
@@ -4249,8 +4433,11 @@ static int multi_submit_locked(ibft_engine* E, int kind, uint32_t used, const ib
     copy_runs(arena, runs, L->h_arena);
     mc.bitmap[k].assign((hi - lo + 31) / 32, 0);
     if (recovered_out) mc.recovered[k].assign((size_t)(hi - lo) * 20, 0);
+    if (counted_out) mc.counted[k].assign((hi - lo + 31) / 32, 0);
+    // a bound group's filter runs per shard (k_quorum_mark_hashed), so the partials the lead merges hold counted items only
     return submit_locked(s, L, L->h_items, hi - lo, L->h_arena, len, groups, n_groups, mc.bitmap[k].data(), nullptr,
-                         recovered_out ? mc.recovered[k].data() : nullptr, /*votes_only=*/mc.merge);
+                         recovered_out ? mc.recovered[k].data() : nullptr, /*votes_only=*/mc.merge, ghash,
+                         counted_out ? mc.counted[k].data() : nullptr);
   });
   if (rc == IBFT_OK && mc.merge) rc = multi_merge_enqueue(M, kind, used, n_groups);
   if (rc != IBFT_OK) {  // drain what was enqueued; its outputs go to this call's own buffers
@@ -4438,6 +4625,7 @@ static int multi_wait_locked(ibft_engine* E, int kind, multi_call& mc, uint8_t* 
       if (hi == lo) continue;
       memcpy(mc.bitmap_out + lo / 32, mc.bitmap[k].data(), mc.bitmap[k].size() * 4);
       if (mc.recovered_out) memcpy(mc.recovered_out + (size_t)lo * 20, mc.recovered[k].data(), mc.recovered[k].size());
+      if (mc.counted_out) memcpy(mc.counted_out + lo / 32, mc.counted[k].data(), mc.counted[k].size() * 4);
     }
     if (mc.merge) memcpy(mc.results_out, L0->h_results, (size_t)mc.n_groups * sizeof(ibft_group_result));
   }
@@ -4460,7 +4648,8 @@ static int multi_wait_locked(ibft_engine* E, int kind, multi_call& mc, uint8_t* 
 
 static int multi_verify(ibft_engine* E, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
                         const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
-                        uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words) {
+                        uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words,
+                        const ibft_group_hash* ghash, uint32_t* counted_out) {
   multi_engine* M = E->multi;
   std::shared_lock<std::shared_mutex> st(M->state_mu);
   const lane& small = M->subs[0]->lanes[1];
@@ -4468,7 +4657,8 @@ static int multi_verify(ibft_engine* E, const ibft_sig_item* items, uint32_t n, 
   const uint32_t used = shard_devices(n, (uint32_t)M->subs.size());
   multi_lanes_lock lk(M, kind, used);
   multi_call mc;
-  int rc = multi_submit_locked(E, kind, used, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, mc);
+  int rc = multi_submit_locked(E, kind, used, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, mc, ghash,
+                               counted_out);
   if (rc != IBFT_OK) return rc;
   return multi_wait_locked(E, kind, mc, status_out, voted_out, voted_stride_words);
 }

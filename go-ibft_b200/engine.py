@@ -24,6 +24,8 @@ NO_TABLE = 0xFFFF
 # quorum rule of a group (ibft_group_desc.flags bits 0-1) and the proposer markers of the PREPARE rule (ibft_group_desc.reserved)
 QUORUM_DEFAULT, QUORUM_PREPREPARE, QUORUM_PREPARE = 0, 1, 2
 PROPOSER_NONE, PROPOSER_UNSET = 0xFFFFFFFF, 0xFFFFFFFE
+# hash binding of a group (ibft_group_hash.msg_type): unbound, or the extractor of the group's handler
+HASH_UNBOUND, HASH_PREPARE, HASH_COMMIT = 0xFFFFFFFF, 1, 2
 DBG = dict(FE_MUL=1, FE_SQR=2, FE_INV=3, FE_SQRT=4, SC_MUL=5, SC_INV=6, ECMULT=7, FE_ADD=8, FE_SUB=9, GLV=10,
            FE_MUL_RAW=11, FE_SQR_RAW=12, FE_ADD_RAW=13, FE_SUB_RAW=14, FE_NORMALIZE=15, FE_EQUAL=16, FE_SQRN=17, FE_SQRT_INV=18,
            SC_ADD=19, SC_NEG=20, SC_REDUCE_ONCE=21, SC_DIGITS=22, RFC6979=23, KEY_ADDRESS=24, FE_FUSED=25)
@@ -35,7 +37,8 @@ ITEM_DTYPE = np.dtype([
 ])
 GROUP_DTYPE = np.dtype([("table_slot", "<u2"), ("flags", "<u2"), ("reserved", "<u4"), ("height", "<u8")])
 RESULT_DTYPE = np.dtype([("power", "<u8", 5), ("n_valid", "<u4"), ("n_distinct", "<u4"), ("has_quorum", "<u4"), ("reserved", "<u4")])
-assert ITEM_DTYPE.itemsize == 128 and GROUP_DTYPE.itemsize == 16 and RESULT_DTYPE.itemsize == 56
+GROUP_HASH_DTYPE = np.dtype([("hash", "u1", 32), ("msg_type", "<u4"), ("reserved", "<u4", 3)])
+assert ITEM_DTYPE.itemsize == 128 and GROUP_DTYPE.itemsize == 16 and RESULT_DTYPE.itemsize == 56 and GROUP_HASH_DTYPE.itemsize == 48
 
 EXPORTS = [
     "ibft_abi_version", "ibft_last_error", "ibft_engine_create", "ibft_engine_destroy", "ibft_engine_device_info",
@@ -46,6 +49,7 @@ EXPORTS = [
     "ibft_debug_wtable", "ibft_debug_keytab", "ibft_debug_key_registry", "ibft_debug_known_handed_back",
     "ibft_engine_create_multi", "ibft_engine_device_count", "ibft_engine_sub", "ibft_explain_batch", "ibft_explain_batch_device",
     "ibft_key_share_words", "ibft_key_share_export_device", "ibft_key_share_adopt_device",
+    "ibft_verify_batch_hashed", "ibft_bind_group_hashes", "ibft_quorum_reduce_device_ex", "ibft_quorum_mark_device_ex",
 ]
 
 
@@ -98,6 +102,11 @@ def load_library(path: str | None = None) -> ctypes.CDLL:
         getattr(lib, name).argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_size_t, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p]
     lib.ibft_verify_batch_ex.argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_size_t, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_uint32]
+    lib.ibft_verify_batch_hashed.argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_size_t, c_void_p, c_uint32, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p]
+    lib.ibft_bind_group_hashes.argtypes = [c_void_p, c_void_p, c_uint32]
+    lib.ibft_quorum_reduce_device_ex.argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p]
+    lib.ibft_quorum_mark_device_ex.argtypes = [c_void_p, c_void_p, c_uint32, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.ibft_last_item_status.argtypes = [c_void_p, c_void_p, c_uint32]
     lib.ibft_explain_batch.argtypes = [c_void_p, c_void_p, c_uint32, c_void_p, c_size_t, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p]
     lib.ibft_verify_poll.argtypes = [c_void_p, POINTER(c_int)]
@@ -156,6 +165,19 @@ def group_descs(n_groups: int, slot=0, rule=QUORUM_DEFAULT, proposer=0, slot_hei
         g[i]["flags"] = ru
         g[i]["reserved"] = pr if ru == QUORUM_PREPARE else 0
     return g
+
+
+def group_hashes(n_groups: int, bound: dict | None = None) -> np.ndarray:
+    """n ibft_group_hash records, every group unbound except bound[g] = (msg_type, hash): msg_type HASH_PREPARE or HASH_COMMIT
+    (the extractor of the group's handler) and the accepted proposal's 32-byte hash."""
+    h = np.zeros(n_groups, dtype=GROUP_HASH_DTYPE)
+    h["msg_type"] = HASH_UNBOUND
+    for g, (msg_type, digest) in (bound or {}).items():
+        if len(digest) != 32:
+            raise ValueError("a bound hash is 32 bytes")
+        h[g]["msg_type"] = msg_type
+        h[g]["hash"] = np.frombuffer(bytes(digest), np.uint8)
+    return h
 
 
 class Engine:
@@ -274,8 +296,11 @@ class Engine:
 
     # ---- host-buffer verify (the e2e call)
     def verify_batch_ex(self, items: np.ndarray, arena: bytes | np.ndarray = b"", groups: np.ndarray | None = None,
-                        voted_stride_words: int = 0):
-        """ibft_verify_batch_ex: returns (bitmap, results, status, voted) -- everything from the call itself (concurrent callers)."""
+                        voted_stride_words: int = 0, group_hashes: np.ndarray | None = None):
+        """ibft_verify_batch_ex: returns (bitmap, results, status, voted) -- everything from the call itself (concurrent callers).
+        group_hashes (GROUP_HASH_DTYPE, one per group; see group_hashes()): ibft_verify_batch_hashed -- only the items that name a
+        bound group's hash count toward its results and voted set, and the call returns (bitmap, results, status, voted, counted)
+        with counted = one bit per item that counted (an item of an unbound group: its verdict bit)."""
         items = np.ascontiguousarray(items)
         assert items.dtype == ITEM_DTYPE
         n = len(items)
@@ -288,6 +313,17 @@ class Engine:
         results = np.zeros(ng, dtype=RESULT_DTYPE) if ng else None
         status = np.zeros(max(1, n), dtype=np.uint8)
         voted = np.zeros((ng, voted_stride_words), dtype=np.uint32) if (ng and voted_stride_words) else None
+        if group_hashes is not None:
+            group_hashes = np.ascontiguousarray(group_hashes)
+            if group_hashes.dtype != GROUP_HASH_DTYPE or len(group_hashes) != ng:
+                raise ValueError("group_hashes needs one GROUP_HASH_DTYPE record per group")
+            counted = np.zeros(max(1, (n + 31) // 32), dtype=np.uint32)
+            self._check(self.lib.ibft_verify_batch_hashed(self.handle, _ptr(items) if n else None, n,
+                                                          _ptr(arena_np) if len(arena_np) else None, len(arena_np),
+                                                          _ptr(groups) if ng else None, ng, _ptr(bitmap), _ptr(results), None,
+                                                          _ptr(status), _ptr(voted), voted_stride_words, _ptr(group_hashes) if ng else None,
+                                                          _ptr(counted)))
+            return bitmap[: (n + 31) // 32], results, status[:n], voted, counted[: (n + 31) // 32]
         self._check(self.lib.ibft_verify_batch_ex(self.handle, _ptr(items) if n else None, n,
                                                   _ptr(arena_np) if len(arena_np) else None, len(arena_np),
                                                   _ptr(groups) if ng else None, ng, _ptr(bitmap), _ptr(results), None,
@@ -364,6 +400,18 @@ class Engine:
             groups = np.ascontiguousarray(groups)
         self._check(self.lib.ibft_bind_groups(self.handle, _ptr(groups) if ng else None, ng))
 
+    def bind_group_hashes(self, hashes: np.ndarray | None):
+        """ibft_bind_group_hashes: bind the groups of the device-resident calls (bind_groups first) to the accepted proposal's hash,
+        one GROUP_HASH_DTYPE record per bound group (group_hashes()); None unbinds.  quorum_reduce_device / quorum_mark_device then
+        mark only the items that name their group's hash."""
+        if hashes is None:
+            self._check(self.lib.ibft_bind_group_hashes(self.handle, None, 0))
+            return
+        hashes = np.ascontiguousarray(hashes)
+        if hashes.dtype != GROUP_HASH_DTYPE:
+            raise ValueError("hashes need GROUP_HASH_DTYPE")
+        self._check(self.lib.ibft_bind_group_hashes(self.handle, _ptr(hashes) if len(hashes) else None, len(hashes)))
+
     def verify_device(self, d_items: int, n: int, d_arena: int, arena_len: int, lo: int, hi: int, d_bitmap: int,
                       d_recovered: int = 0, stream: int = 0):
         self._check(self.lib.ibft_verify_batch_device(self.handle, d_items, n, d_arena or None, arena_len, lo, hi, d_bitmap,
@@ -377,7 +425,12 @@ class Engine:
         self._check(self.lib.ibft_explain_batch_device(self.handle, d_items or None, n, d_arena or None, arena_len, lo, hi, d_bitmap or None,
                                                        d_reasons or None, d_recovered or None, d_count or None, stream or None))
 
-    def quorum_reduce_device(self, d_items: int, n: int, d_bitmap: int, n_groups: int, d_results: int, stream: int = 0):
+    def quorum_reduce_device(self, d_items: int, n: int, d_bitmap: int, n_groups: int, d_results: int, stream: int = 0, d_counted: int = 0):
+        """d_counted (device u32 bitmap, optional): receives bits [0, n) -- the items that counted (ibft_quorum_reduce_device_ex)"""
+        if d_counted:
+            self._check(self.lib.ibft_quorum_reduce_device_ex(self.handle, d_items, n, d_bitmap, None, n_groups, d_results, d_counted,
+                                                              stream or None))
+            return
         self._check(self.lib.ibft_quorum_reduce_device(self.handle, d_items, n, d_bitmap, None, n_groups, d_results, stream or None))
 
     def quorum_partial_words(self) -> int:
@@ -385,7 +438,13 @@ class Engine:
         self._check(self.lib.ibft_quorum_partial_words(self.handle, ctypes.byref(w)))
         return int(w.value)
 
-    def quorum_mark_device(self, d_items: int, n: int, lo: int, hi: int, d_bitmap: int, d_partial: int, stream: int = 0):
+    def quorum_mark_device(self, d_items: int, n: int, lo: int, hi: int, d_bitmap: int, d_partial: int, stream: int = 0,
+                           d_counted: int = 0):
+        """d_counted (device u32 bitmap by global item number, optional): receives bits [lo, hi) -- the items of the shard that
+        counted (ibft_quorum_mark_device_ex)"""
+        if d_counted:
+            self._check(self.lib.ibft_quorum_mark_device_ex(self.handle, d_items, n, lo, hi, d_bitmap, d_partial, d_counted, stream or None))
+            return
         self._check(self.lib.ibft_quorum_mark_device(self.handle, d_items, n, lo, hi, d_bitmap, d_partial, stream or None))
 
     def quorum_merge_device(self, d_partials: int, n_parts: int, stride_words: int, d_results: int, stream: int = 0):

@@ -144,6 +144,11 @@ class ShardedVerifier:
     The descriptors are bound as given, quorum rule and proposer included (Engine.groups(..., rule=, proposer=)): both exchanges
     return go-ibft's per-message-type decision (HasPrepareQuorum for PREPARE groups, one valid message for PREPREPARE groups).
 
+    group_hashes (ibft_b200.group_hashes(...), one record per group): every rank binds the PREPARE and COMMIT groups to the accepted
+    proposal's hash (Engine.bind_group_hashes), so each rank marks only the items of its shard that name it and the merged or
+    exchanged decision is go-ibft's handlePrepare / handleCommit decision.  After finish(), `counted` holds the shard's counted
+    bits ((hi - lo + 31) // 32 words, bit i = item lo + i counted): the messages GetValidMessages keeps.
+
     Key registry (engine flag key_cache): a rank only recovers the signers whose items land in its shard.  Call share_keys()
     between rounds and every rank also knows the keys the other ranks learned, so from the next round on no rank recovers a
     validator any rank already knows.  A caller that never calls it sees no change, except that a p2p-mode rank with a key
@@ -156,7 +161,7 @@ class ShardedVerifier:
     """
 
     def __init__(self, engine, n_global: int, groups: np.ndarray, world: int, rank: int, local_items: np.ndarray,
-                 local_arena: np.ndarray, stream=None, exchange: str = "nccl"):
+                 local_arena: np.ndarray, stream=None, exchange: str = "nccl", group_hashes: np.ndarray | None = None):
         """exchange = "nccl": one all_gather_into_tensor + merge kernel (any backend / any topology);
         exchange = "p2p": every rank's words live in a buffer its peers map over NVLink (CUDA IPC, one node, <= 8 ranks) and ONE
         kernel publishes, waits for the peers and merges straight out of peer memory (ibft_quorum_exchange_device)."""
@@ -166,6 +171,9 @@ class ShardedVerifier:
         assert len(local_items) == self.hi - self.lo
         self.groups = groups
         engine.bind_groups(groups)
+        self.hashed = group_hashes is not None
+        if self.hashed:
+            engine.bind_group_hashes(group_hashes)
         self.W = engine.quorum_partial_words()
         self.per = shard_words(n_global, world)
         dev = torch.device("cuda", torch.cuda.current_device())
@@ -187,6 +195,11 @@ class ShardedVerifier:
         # the kernels index tuples and bitmap words by GLOBAL item number: hand them rebased pointers
         self.items_base = self.d_items.data_ptr() - self.lo * 128
         self.bitmap_base = self.d_local.data_ptr() - (self.lo // 32) * 4
+        self.counted = None
+        if self.hashed:  # the shard's counted bits, by global item number as the mark call indexes them
+            self.d_counted = torch.zeros(max(1, self.per), dtype=torch.int32, device=dev)
+            self.h_counted = torch.zeros(max(1, self.per), dtype=torch.int32).pin_memory()
+            self.counted_base = self.d_counted.data_ptr() - (self.lo // 32) * 4
         self.exchange = exchange
         # key sharing (share_keys): each rank sends key_blocks blocks of key_words words per step, enough for a whole validator
         # table (a rank that learned more keys sends the rest at the next step); key_words = 0 when the engine has no key registry
@@ -245,7 +258,10 @@ class ShardedVerifier:
             if self.hi > self.lo:
                 self.e.verify_device(self.items_base, self.n, self.d_arena.data_ptr(), self.h_arena.numel(), self.lo, self.hi,
                                      base - (self.lo // 32) * 4, 0, st)
-            self.e.quorum_mark_device(self.items_base, self.n, self.lo, self.hi, base - (self.lo // 32) * 4, base + self.per * 4, st)
+            self.e.quorum_mark_device(self.items_base, self.n, self.lo, self.hi, base - (self.lo // 32) * 4, base + self.per * 4, st,
+                                      self.counted_base if self.hashed else 0)
+            if self.hashed:
+                self.h_counted.copy_(self.d_counted, non_blocking=True)
             if self.key_words:
                 self._export_keys(self._key_region(self.xbuf_ptr, par), st)
             self.e.quorum_exchange_device(self.peer_ptrs, self.rank, self.wpr, self.per, self.epoch, self.d_full.data_ptr(),
@@ -270,7 +286,9 @@ class ShardedVerifier:
                 self.e.verify_device(self.items_base, self.n, self.d_arena.data_ptr(), self.h_arena.numel(), self.lo, self.hi,
                                      self.bitmap_base, 0, st)
             self.e.quorum_mark_device(self.items_base, self.n, self.lo, self.hi, self.bitmap_base,
-                                      self.d_local.data_ptr() + self.per * 4, st)
+                                      self.d_local.data_ptr() + self.per * 4, st, self.counted_base if self.hashed else 0)
+            if self.hashed:
+                self.h_counted.copy_(self.d_counted, non_blocking=True)
             if self.world > 1:
                 dist.all_gather_into_tensor(self.d_gather, self.d_local)
             else:
@@ -284,6 +302,8 @@ class ShardedVerifier:
 
     def finish(self):
         self.stream.synchronize()
+        if self.hashed:
+            self.counted = self.h_counted.numpy().view(np.uint32)[: (self.hi - self.lo + 31) // 32].copy()
         nres = self.d_results.numel()
         res = self.h_out[:nres].numpy().view(self.result_dtype).copy()
         if self.exchange == "p2p":

@@ -135,6 +135,40 @@ typedef struct ibft_group_desc {
 #define IBFT_PROPOSER_NONE 0xFFFFFFFFu
 #define IBFT_PROPOSER_UNSET 0xFFFFFFFEu
 
+/* A group may be BOUND to the hash of the accepted proposal (state.proposal in go-ibft): then only the items that name that hash
+ * count toward its quorum, as in handlePrepare (core/ibft.go:855-889: IsValidProposalHash(state.proposal, ExtractPrepareHash(m)))
+ * and handleCommit (core/ibft.go:931-967: ExtractCommitHash before IsValidCommittedSeal), whose GetValidMessages
+ * (messages/messages.go:169-199) drops every other message before hasQuorumByMsgType sees the set.  Without a binding a valid
+ * PREPARE or seal over ANY hash counts -- an equivocating validator, a stale round or a competing proposal included -- which is
+ * what a caller that never parses its items (raw frames, device-resident tuples) cannot filter itself.
+ * Binding is opt-in, one entry per group in an array parallel to the groups (ibft_verify_batch_hashed, ibft_bind_group_hashes);
+ * ibft_group_desc is unchanged.  An item of a bound group COUNTS when its verdict bit is 1, its group index is in range and the
+ * hash the group's extractor gets from it is exactly the 32 bound bytes:
+ *   IBFT_KIND_SEAL       digest (the proposalHash the caller extracted); COMMIT-bound groups only, never in a PREPARE-bound one
+ *   IBFT_KIND_WIRE_SEAL  commitData.proposalHash of the frame, which must be a COMMIT; COMMIT-bound groups only
+ *   IBFT_KIND_WIRE       ExtractPrepareHash / ExtractCommitHash of the frame, by msg_type: the frame's type must match and the
+ *                        matching oneof member must be present, otherwise the hash is nil and the item never counts
+ *   IBFT_KIND_PAYLOAD    the same extractors over the PayloadNoSig bytes, decoded as protobuf-go decodes them (the last `type`
+ *                        wins, a later oneof member replaces an earlier one and the same member again merges into it, the last
+ *                        proposalHash wins even when empty, unknown fields and groups are skipped, bytes protobuf-go refuses
+ *                        anywhere in the message give nil)
+ *   any other kind       no hash is knowable: never counts in a bound group
+ * A hash of any length other than 32 never matches.  Items that count feed the voted set, n_valid, n_distinct, power and
+ * has_quorum; the verdict bitmap and every unbound group keep their meaning.  The counted bits (one per item: the items that
+ * counted, and for an item of an unbound group its verdict bit) are what GetValidMessages returns -- the seals to pick for
+ * InsertProposal.  Refused with IBFT_ERR_INVALID_ARG before anything is launched: a msg_type other than 1, 2 or
+ * IBFT_HASH_UNBOUND; a bound group whose quorum rule is IBFT_QUORUM_PREPREPARE, a COMMIT-bound group whose rule is not
+ * IBFT_QUORUM_DEFAULT, a PREPARE-bound group whose rule is not IBFT_QUORUM_DEFAULT or IBFT_QUORUM_PREPARE; non-zero reserved
+ * words (in any entry).  PREPREPARE and ROUND_CHANGE groups stay unbound: go-ibft filters neither by an accepted hash. */
+#define IBFT_HASH_UNBOUND 0xFFFFFFFFu
+#define IBFT_HASH_PREPARE 1u /* ExtractPrepareHash (messages/helpers.go:107-118) */
+#define IBFT_HASH_COMMIT 2u  /* ExtractCommitHash (messages/helpers.go:51-62) */
+typedef struct ibft_group_hash {
+  uint8_t hash[32];     /* the accepted proposal's hash (state.proposal's hash in go-ibft); ignored when unbound */
+  uint32_t msg_type;    /* IBFT_HASH_UNBOUND, IBFT_HASH_PREPARE or IBFT_HASH_COMMIT: the extractor of the group's handler */
+  uint32_t reserved[3]; /* zero */
+} ibft_group_hash;      /* sizeof == 48 */
+
 /* Per-group result of the on-device quorum reduction.
  * power[] is the little-endian 320-bit sum of votingPower over the DISTINCT validators with >= 1 valid
  * item in the group (HasQuorum sums over an address *set*: validator_manager.go:88-92, :147-155); under IBFT_QUORUM_PREPARE
@@ -210,14 +244,15 @@ int ibft_engine_device_info(ibft_engine* e, ibft_device_info* out);
  *                                  those get the slot's previous table back (or the slot unset), so the slot answers as before.
  *   ibft_get_quorum                the lead answers.
  *   ibft_verify_batch, _ex,        split into contiguous shards whose boundaries are multiples of 32 over
- *   _submit / _poll / _wait        min(n_devices, ceil(n / 1,024)) devices.  Each shard gets its own payload arena: the union of
- *                                  the byte ranges its items reference, each byte once, never longer than the call's arena.  Every
+ *   _hashed, _submit / _poll /     min(n_devices, ceil(n / 1,024)) devices.  Each shard gets its own payload arena: the union of
+ *   _wait                          the byte ranges its items reference, each byte once, never longer than the call's arena.  Every
  *                                  device verifies its shard (its kernel chosen for the shard's size) and records its votes; the
  *                                  lead gathers the voted sets and valid counts with peer copies, merges them and decides each
  *                                  group's quorum rule.  The caller's buffers are written only after every device has succeeded;
  *                                  any failure returns its status with every output untouched.  A call takes the small lane of
  *                                  every device when the whole call fits it, else the bulk lane, locked in device-list order.
- *                                  The results are byte for byte those of a single-device engine.
+ *                                  The results are byte for byte those of a single-device engine.  Hash bindings
+ *                                  (ibft_verify_batch_hashed) are applied in every shard, before its votes go to the merge.
  *   ibft_explain_batch             the lead answers (the tables are replicated, and the items to explain are few).
  *   ibft_last_item_status,         the most recent completed call: statuses assembled from the shards, the merged voted sets,
  *   ibft_get_voted_bitmap,         handed-back summed over the devices that call used.
@@ -237,7 +272,8 @@ int ibft_engine_device_info(ibft_engine* e, ibft_device_info* out);
  *   ibft_engine_launch_count       the sum over the devices.
  *   ibft_engine_device_info,       the lead answers; ibft_engine_sub reaches the others.
  *   ibft_probe_int_peak, ibft_debug_*
- *   ibft_bind_groups, ibft_verify_batch_device, ibft_explain_batch_device, ibft_quorum_*_device, ibft_exchange_*
+ *   ibft_bind_groups, ibft_bind_group_hashes, ibft_verify_batch_device, ibft_explain_batch_device, ibft_quorum_*_device(_ex),
+ *   ibft_exchange_*
  *                                  IBFT_ERR_INVALID_ARG: they take device pointers of one device.  Across processes or nodes, or
  *                                  with device-resident buffers, use one engine per device (go-ibft_b200/sharding.py). */
 int ibft_engine_create_multi(const ibft_engine_params* params, const int32_t* devices, uint32_t n_devices, ibft_engine** out);
@@ -288,6 +324,18 @@ int ibft_verify_batch_ex(ibft_engine* e, const ibft_sig_item* items, uint32_t n,
                          const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
                          ibft_group_result* results_out, uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out,
                          uint32_t voted_stride_words);
+
+/* ibft_verify_batch_ex with groups bound to the accepted proposal's hash (ibft_group_hash above):
+ *   group_hashes  NULL (the call is ibft_verify_batch_ex), or n_groups entries, IBFT_HASH_UNBOUND for a group left as it is
+ *   counted_out   NULL, or (n+31)/32 words: bit i = item i counted (for an item of an unbound group: its verdict bit)
+ * bitmap_out, status_out and recovered_out are what ibft_verify_batch_ex writes; results_out and voted_out follow the counted
+ * items.  When at least one group is bound the recover kernels record no votes (their fused marking cannot see the hash) and one
+ * extra launch (k_quorum_mark_hashed) marks the counted items over the tuples.  Multi-device engines apply the filter per shard
+ * and merge as usual. */
+int ibft_verify_batch_hashed(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
+                             const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out, ibft_group_result* results_out,
+                             uint8_t* recovered_out, uint8_t* status_out, uint32_t* voted_out, uint32_t voted_stride_words,
+                             const ibft_group_hash* group_hashes, uint32_t* counted_out);
 
 /* Per-item status (IBFT_ITEM_*) of the most recent completed ibft_verify_batch / ibft_verify_wait on this engine. */
 int ibft_last_item_status(ibft_engine* e, uint8_t* status_out, uint32_t n);
@@ -372,6 +420,23 @@ int ibft_quorum_mark_device(ibft_engine* e, const void* d_items, uint32_t n, uin
                             const void* d_bitmap, void* d_partial, void* stream);
 int ibft_quorum_merge_device(ibft_engine* e, const void* d_partials, uint32_t n_parts, uint32_t part_stride_words,
                              void* d_results, void* stream);
+
+/* Binds the groups of the device-resident calls to the accepted proposal's hash (ibft_group_hash above): HOST array of n_groups
+ * entries, n_groups == the number of groups bound by ibft_bind_groups (call that first; ibft_bind_groups, and every host-buffer
+ * call on the full-capacity lane, which replaces the bound groups, drops the hashes).  NULL unbinds.  From then on
+ * ibft_quorum_reduce_device and ibft_quorum_mark_device mark only the counted items, so the partials, the merge
+ * (ibft_quorum_merge_device) and the peer-memory exchange (ibft_quorum_exchange_device) decide go-ibft's quorum; every rank of a
+ * sharded verifier binds the same hashes.  ibft_verify_batch_device records no votes in any case and is unchanged.  Refusals as
+ * for ibft_verify_batch_hashed, with nothing changed. */
+int ibft_bind_group_hashes(ibft_engine* e, const ibft_group_hash* hashes, uint32_t n_groups);
+/* ibft_quorum_reduce_device / ibft_quorum_mark_device with the counted bits of the items they mark: d_counted NULL, or a DEVICE
+ * bitmap indexed by global item number of which exactly the bits of [0, n) (reduce) or [shard_lo, shard_hi) (mark, any bounds)
+ * are written, each by an atomic bit update, so the ranks of a sharded verifier may write one gathered bitmap.  A counted bit is
+ * the verdict bit for an item of an unbound group (all items while no hashes are bound). */
+int ibft_quorum_reduce_device_ex(ibft_engine* e, const void* d_items, uint32_t n, const void* d_bitmap, const void* d_groups,
+                                 uint32_t n_groups, void* d_results, void* d_counted, void* stream);
+int ibft_quorum_mark_device_ex(ibft_engine* e, const void* d_items, uint32_t n, uint32_t shard_lo, uint32_t shard_hi,
+                               const void* d_bitmap, void* d_partial, void* d_counted, void* stream);
 
 /* The same exchange WITHOUT a library collective (one node, <= 8 ranks): every rank keeps its (bitmap words | partial) in an
  * exchange buffer that its peers have mapped over NVLink (CUDA IPC / peer access; the caller exchanges the handles once).
