@@ -3299,9 +3299,10 @@ static void stage_copy(void* dst, const void* src, size_t bytes) {
 static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
                          const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
                          ibft_group_result* results_out, uint8_t* recovered_out, bool votes_only = false,
-                         const ibft_group_hash* ghash = nullptr, uint32_t* counted_out = nullptr) {
+                         const ibft_group_hash* ghash = nullptr, uint32_t* counted_out = nullptr, bool async_call = false) {
   // votes_only: a shard of a multi-device call -- record the votes, leave the reduce to the coordinator's merge
   // ghash: the groups' hash bindings, given only when at least one group is bound (checked by check_group_hashes)
+  // async_call: the call returns before its copies have run (ibft_verify_submit), so no caller buffer may be read after it
   if (L->pending.active) { set_err("a submitted call is still pending; wait for it first"); return IBFT_ERR_INVALID_ARG; }
   if ((n && !items) || (n && !bitmap_out) || (arena_len && !arena) || (n_groups && !groups)) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   if (n > L->cap_items || arena_len > L->cap_arena || n_groups > e->p.max_groups) {
@@ -3360,6 +3361,16 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
     CU(cudaEventRecord(L->chunk_ev[n_chunks], st));
     CU(cudaStreamWaitEvent(L->copy_stream, L->chunk_ev[n_chunks], 0));
   }
+  // A caller that already holds the tuples in page-locked memory (cudaHostAlloc / cudaHostRegister, e.g. torch pin_memory)
+  // is copied from directly by a synchronous call, which waits for its copies before it returns.  Pageable memory (Go heap
+  // through cgo) goes through the engine's pinned staging first -- and so does every tuple of an asynchronous call, whose DMA
+  // would otherwise read the caller's buffer after the call has returned it.
+  bool direct = false;
+  if (n && !async_call) {
+    cudaPointerAttributes pa;
+    if (cudaPointerGetAttributes(&pa, items) == cudaSuccess) direct = pa.type == cudaMemoryTypeHost;
+    else (void)cudaGetLastError();
+  }
   int rc = IBFT_OK;
 #if IBFT_WC > 0
   // One mid-size round (the chain + helper kernel's range, e.g. 10,000 seals = 1.28 MB of tuples): the staging copy and the
@@ -3369,10 +3380,6 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
   const bool lat_pieces = e->recover_path.load() == IBFT_PATH_AUTO && n > (uint32_t)e->sm_count * 2u * IBFT_QSPLIT_SIGS &&
                           n <= (uint32_t)e->sm_count * IBFT_SPLIT_SIGS && arena_len / n <= 256;
   if (lat_pieces) {
-    bool pinned = false;
-    cudaPointerAttributes pa;
-    if (cudaPointerGetAttributes(&pa, items) == cudaSuccess) pinned = pa.type == cudaMemoryTypeHost;
-    else (void)cudaGetLastError();
     CU(cudaEventRecord(L->lat_ev[4], st));  // arena / groups uploads of this call
     const uint32_t per = ((n + 3) / 4 + IBFT_SPLIT_SIGS - 1) / IBFT_SPLIT_SIGS * IBFT_SPLIT_SIGS;
     // with a key registry the pieces go through the known-key pass (one-warp CTAs) + worklist; without, chain + helper warps
@@ -3382,7 +3389,7 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
       if (hi <= lo) break;
       cudaStream_t ls = L->lat_stream[c];
       const ibft_sig_item* src = items + lo;
-      if (!pinned) {
+      if (!direct) {
         memcpy(L->h_items + lo, items + lo, (size_t)(hi - lo) * sizeof(ibft_sig_item));
         src = L->h_items + lo;
       }
@@ -3397,14 +3404,6 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
     n_chunks = 0;  // the generic chunk loop below has nothing left to do
   }
 #endif
-  // A caller that already holds the tuples in page-locked memory (cudaHostAlloc / cudaHostRegister, e.g. torch pin_memory)
-  // is copied from directly; pageable memory (Go heap through cgo) goes through the engine's pinned staging first.
-  bool caller_pinned = false;
-  if (n) {
-    cudaPointerAttributes pa;
-    if (cudaPointerGetAttributes(&pa, items) == cudaSuccess) caller_pinned = pa.type == cudaMemoryTypeHost;
-    else (void)cudaGetLastError();
-  }
   // Several chunks: chunk c's kernels run on one of two alternating streams, so that the tail of one chunk (the last CTAs of a
   // 1,024-CTA launch on 444 resident slots) overlaps the head of the next instead of idling the SMs eight times per batch.
   if (n_chunks > 1) {
@@ -3415,7 +3414,7 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
   for (uint32_t c = 0; c < n_chunks; c++) {
     uint32_t lo = c * CHUNK, hi = std::min(n, lo + CHUNK);
     const ibft_sig_item* src = items + lo;
-    if (!caller_pinned) {
+    if (!direct) {
       stage_copy(L->h_items + lo, items + lo, (size_t)(hi - lo) * sizeof(ibft_sig_item));
       src = L->h_items + lo;
     }
@@ -3700,7 +3699,8 @@ extern "C" int ibft_verify_submit(ibft_engine* e, const ibft_sig_item* items, ui
   if (e->multi) return multi_submit(e, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out);
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
-  return submit_locked(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out);
+  return submit_locked(e, L, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, false, nullptr, nullptr,
+                       /*async_call=*/true);
 }
 
 extern "C" int ibft_verify_poll(ibft_engine* e, int* done) {
@@ -4383,7 +4383,7 @@ static int multi_merge_enqueue(multi_engine* M, int kind, uint32_t used, uint32_
 static int multi_submit_locked(ibft_engine* E, int kind, uint32_t used, const ibft_sig_item* items, uint32_t n, const uint8_t* arena,
                                size_t arena_len, const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
                                ibft_group_result* results_out, uint8_t* recovered_out, multi_call& mc,
-                               const ibft_group_hash* ghash = nullptr, uint32_t* counted_out = nullptr) {
+                               const ibft_group_hash* ghash = nullptr, uint32_t* counted_out = nullptr, bool async_call = false) {
   multi_engine* M = E->multi;
   ibft_engine* lead = M->subs[0];
   lane* L0 = &lead->lanes[kind];
@@ -4399,7 +4399,7 @@ static int multi_submit_locked(ibft_engine* E, int kind, uint32_t used, const ib
   mc.counted_out = counted_out;
   if (used == 1) {  // the lead's own call, as on a single-device engine
     int rc = submit_locked(lead, L0, items, n, arena, arena_len, groups, n_groups, bitmap_out, results_out, recovered_out, false, ghash,
-                           counted_out);
+                           counted_out, async_call);
     mc.active = rc == IBFT_OK;
     return rc;
   }
@@ -4679,7 +4679,7 @@ static int multi_submit(ibft_engine* E, const ibft_sig_item* items, uint32_t n, 
   std::shared_lock<std::shared_mutex> st(M->state_mu);
   multi_lanes_lock lk(M, 0, (uint32_t)M->subs.size());
   return multi_submit_locked(E, 0, shard_devices(n, (uint32_t)M->subs.size()), items, n, arena, arena_len, groups, n_groups, bitmap_out,
-                             results_out, recovered_out, M->pending);
+                             results_out, recovered_out, M->pending, nullptr, nullptr, /*async_call=*/true);
 }
 
 static int multi_poll(ibft_engine* E, int* done) {

@@ -360,7 +360,9 @@ int ibft_explain_batch(ibft_engine* e, const ibft_sig_item* items, uint32_t n, c
                        uint8_t* recovered_out);
 
 /* Asynchronous variant: same arguments; inputs are copied into engine-owned pinned staging before the call
- * returns (cgo rule: no Go pointer is retained).  ibft_verify_poll returns IBFT_OK with *done = 0/1;
+ * returns (cgo rule: no Go pointer is retained) -- tuples in page-locked caller memory too, which the synchronous
+ * calls copy from directly: the caller may overwrite or free every input buffer as soon as this returns.  Only the
+ * output buffers must stay valid until ibft_verify_wait.  ibft_verify_poll returns IBFT_OK with *done = 0/1;
  * ibft_verify_wait blocks and copies the outputs into the buffers given at submit time. */
 int ibft_verify_submit(ibft_engine* e, const ibft_sig_item* items, uint32_t n, const uint8_t* arena, size_t arena_len,
                        const ibft_group_desc* groups, uint32_t n_groups, uint32_t* bitmap_out,
