@@ -96,12 +96,8 @@ __device__ __forceinline__ uint32_t key_lookup(const slot_dev& s, uint32_t r, bo
 
 __device__ __forceinline__ uint32_t bswap32(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
 
-// binary search of a 20-byte address in a slot's sorted key table; returns validator index or -1
-__device__ int lookup_validator(const slot_dev& s, const uint8_t* addr) {
-  uint32_t a[5];
-#pragma unroll
-  for (int i = 0; i < 5; i++)
-    a[i] = ((uint32_t)addr[4 * i] << 24) | ((uint32_t)addr[4 * i + 1] << 16) | ((uint32_t)addr[4 * i + 2] << 8) | addr[4 * i + 3];
+// binary search of an address, as five big-endian words, in a slot's sorted key table; returns validator index or -1
+__device__ int lookup_validator_words(const slot_dev& s, const uint32_t* a) {
   int lo = 0, hi = (int)s.n - 1;
   while (lo <= hi) {
     int mid = (lo + hi) >> 1;
@@ -116,6 +112,64 @@ __device__ int lookup_validator(const slot_dev& s, const uint8_t* addr) {
     if (cmp < 0) lo = mid + 1; else hi = mid - 1;
   }
   return -1;
+}
+// the same for a 20-byte address
+__device__ int lookup_validator(const slot_dev& s, const uint8_t* addr) {
+  uint32_t a[5];
+#pragma unroll
+  for (int i = 0; i < 5; i++)
+    a[i] = ((uint32_t)addr[4 * i] << 24) | ((uint32_t)addr[4 * i + 1] << 16) | ((uint32_t)addr[4 * i + 2] << 8) | addr[4 * i + 3];
+  return lookup_validator_words(s, a);
+}
+
+// The last 32 bytes of a tuple, all that the quorum marking reads of it: the signer (words 0..4, as loaded), v | kind << 8 |
+// group << 16, payload_off, payload_len.  Two 16-byte loads instead of a copy of the whole tuple.
+struct item_tail {
+  uint32_t w[8];
+  __device__ __forceinline__ uint32_t group() const { return w[5] >> 16; }
+  __device__ __forceinline__ uint32_t kind() const { return (w[5] >> 8) & 0xFFu; }
+};
+__device__ __forceinline__ item_tail load_item_tail(const ibft_sig_item* it) {
+  const uint4* p = reinterpret_cast<const uint4*>(it) + 6;
+  const uint4 a = __ldg(p), b = __ldg(p + 1);
+  return item_tail{{a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}};
+}
+// the expected signer of a tuple as five big-endian words (raw frames: the frame's From); false when it has none
+__device__ bool item_signer_words(const item_tail& t, const uint8_t* arena, size_t arena_len, uint32_t* a) {
+  const uint32_t kind = t.kind();
+  if (kind == IBFT_KIND_WIRE || kind == IBFT_KIND_WIRE_SEAL) {
+    const uint32_t off = t.w[6], len = t.w[7];
+    if ((size_t)off + len > arena_len) return false;
+    const uint8_t* w = arena + off;
+    wire_frame f;
+    if (!parse_wire_frame(w, len, f) || f.from_len != 20) return false;
+    w += f.from_off;
+#pragma unroll
+    for (int i = 0; i < 5; i++)
+      a[i] = ((uint32_t)w[4 * i] << 24) | ((uint32_t)w[4 * i + 1] << 16) | ((uint32_t)w[4 * i + 2] << 8) | w[4 * i + 3];
+    return true;
+  }
+#pragma unroll
+  for (int i = 0; i < 5; i++) a[i] = bswap32(t.w[i]);
+  return true;
+}
+
+// One atomicAdd of the count per group and warp instead of one per valid item: the items of a warp mostly share one group,
+// and atomics on one address serialise at L2.  Every lane of the warp calls it (valid: the lane's item counts in group g).
+__device__ __forceinline__ void count_valid_warp(uint32_t* n_valid, bool valid, uint32_t g) {
+  const uint32_t m = __ballot_sync(0xFFFFFFFFu, valid);
+  if (!valid) return;
+  const uint32_t peers = __match_any_sync(m, g);
+  if ((threadIdx.x & 31u) == (uint32_t)(__ffs(peers) - 1)) atomicAdd(&n_valid[g], (uint32_t)__popc(peers));
+}
+// The same for the vote bits: the lanes that set bits of one voted word OR them together and one of them does the atomicOr.  A
+// warp's items mostly come from consecutive validators of one group, so most warps touch one or two words.  bit == 0: no vote.
+__device__ __forceinline__ void or_votes_warp(uint32_t* voted, uint32_t word, uint32_t bit) {
+  const uint32_t m = __ballot_sync(0xFFFFFFFFu, bit != 0);
+  if (bit == 0) return;
+  const uint32_t peers = __match_any_sync(m, word);
+  const uint32_t bits = __reduce_or_sync(peers, bit);
+  if ((threadIdx.x & 31u) == (uint32_t)(__ffs(peers) - 1)) atomicOr(&voted[word], bits);
 }
 
 struct group_dev {
@@ -155,6 +209,15 @@ __device__ __forceinline__ void record_vote(const vote_sink& sink, const ibft_gr
   if (groups == nullptr || sink.voted == nullptr) return;
   atomicAdd(&sink.n_valid[group], 1u);
   if (v >= 0) atomicOr(&sink.voted[sink.gdev[group].voted_off + ((uint32_t)v >> 5)], 1u << (v & 31));
+}
+// the same for the valid items of a whole warp: counts and vote bits go per warp (count_valid_warp, or_votes_warp).  Every lane
+// of the warp calls it.
+__device__ __forceinline__ void record_votes_warp(const vote_sink& sink, const ibft_group_desc* __restrict__ groups, uint32_t group,
+                                                  bool ok, int v) {
+  if (groups == nullptr || sink.voted == nullptr) return;
+  count_valid_warp(sink.n_valid, ok, group);
+  const bool vote = ok && v >= 0;
+  or_votes_warp(sink.voted, vote ? sink.gdev[group].voted_off + ((uint32_t)v >> 5) : 0u, vote ? 1u << (v & 31) : 0u);
 }
 // membership + vote for an item whose signature verified (the latency kernels look the signer up at the end)
 __device__ __forceinline__ bool member_and_vote(const ibft_group_desc* __restrict__ groups, uint32_t n_groups,
@@ -265,6 +328,7 @@ k_recover(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __
     for (int i = 0; i < 8; i++) w[i] = __ldg(src + i);
   }
   __syncthreads();  // the staging area becomes the R tables from here on
+  int v = -1;  // the signer's validator index
   if (active) {
     uint8_t addr[20];
 #pragma unroll
@@ -280,7 +344,6 @@ k_recover(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __
     rtab_view T{s_rtab + tid, (uint32_t)BLOCK};
     // the signer is looked up FIRST: an item of an unknown group / a non-member can never get verdict 1 (its signature is
     // still recovered when the caller asked for the recovered addresses)
-    int v = -1;
     uint32_t slot = IBFT_NO_TABLE;
     const bool member = have && group_member(groups, n_groups, slots, n_slots, it.group, ri.signer, &v, &slot);
     if (have && (member || recovered != nullptr)) {
@@ -300,13 +363,13 @@ k_recover(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __
       for (int i = 0; i < 20; i++) ok = ok && (addr[i] == ri.signer[i]);
       if (ok) learn_key(slots, slot, v, K);
     }
-    if (ok) record_vote(sink, groups, it.group, v);
     if (recovered != nullptr) {
 #pragma unroll
       for (int i = 0; i < 20; i++) recovered[(size_t)idx * 20 + i] = addr[i];
     }
     if (list != nullptr && ok) atomicOr(&bitmap[idx >> 5], 1u << (idx & 31u));
   }
+  record_votes_warp(sink, groups, ok ? (uint32_t)it.group : 0u, ok, v);
   if (list != nullptr) return;
   // warp-ballot reduction of the 32 verdicts into one bitmap word (shard bounds are multiples of 32)
   uint32_t word = __ballot_sync(0xFFFFFFFFu, ok);
@@ -1030,25 +1093,37 @@ k_recover_qsplit(const ibft_sig_item* __restrict__ items, uint32_t n, const uint
 // K3: quorum
 // ------------------------------------------------------------------------------------------------------------
 
+// the vote of a counted item of group g: its signer's bit in the group's voted set (*bit = 0: the group has no table, the item
+// no signer, or the signer is not in the table)
+__device__ __forceinline__ void quorum_vote(const item_tail& t, uint32_t g, const uint8_t* __restrict__ arena, size_t arena_len,
+                                            const ibft_group_desc* __restrict__ groups, const group_dev* __restrict__ gdev,
+                                            const slot_dev* __restrict__ slots, uint32_t n_slots, uint32_t* word, uint32_t* bit) {
+  const uint32_t slot = groups[g].table_slot;
+  if (slot == IBFT_NO_TABLE || slot >= n_slots || !slots[slot].valid) return;
+  uint32_t a[5];
+  if (!item_signer_words(t, arena, arena_len, a)) return;
+  const int v = lookup_validator_words(slots[slot], a);
+  if (v < 0) return;
+  *word = gdev[g].voted_off + ((uint32_t)v >> 5);
+  *bit = 1u << (v & 31);
+}
+
 __global__ void k_quorum_mark(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __restrict__ arena, size_t arena_len,
                               const uint32_t* __restrict__ bitmap,
                               const ibft_group_desc* __restrict__ groups, const group_dev* __restrict__ gdev,
                               uint32_t n_groups, const slot_dev* __restrict__ slots, uint32_t n_slots,
                               uint32_t* __restrict__ voted, uint32_t* __restrict__ n_valid, uint32_t lo, uint32_t hi) {
-  uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= hi || i >= n) return;
-  if (!((bitmap[i >> 5] >> (i & 31)) & 1u)) return;
-  const ibft_sig_item* it = items + i;
-  uint32_t g = it->group;
-  if (g >= n_groups) return;
-  atomicAdd(&n_valid[g], 1u);
-  uint32_t slot = groups[g].table_slot;
-  if (slot == IBFT_NO_TABLE || slot >= n_slots || !slots[slot].valid) return;
-  uint8_t addr[20];
-  ibft_sig_item local = *it;
-  if (!item_signer(local, arena, arena_len, addr)) return;
-  int v = lookup_validator(slots[slot], addr);
-  if (v >= 0) atomicOr(&voted[gdev[g].voted_off + ((uint32_t)v >> 5)], 1u << (v & 31));
+  const uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
+  const bool set = i < hi && i < n && ((bitmap[i >> 5] >> (i & 31)) & 1u);
+  if (__ballot_sync(0xFFFFFFFFu, set) == 0) return;  // a warp of rejected items reads nothing else
+  item_tail t{};
+  if (set) t = load_item_tail(items + i);
+  const uint32_t g = t.group();
+  const bool valid = set && g < n_groups;
+  count_valid_warp(n_valid, valid, g);
+  uint32_t word = 0, bit = 0;
+  if (valid) quorum_vote(t, g, arena, arena_len, groups, gdev, slots, n_slots, &word, &bit);
+  or_votes_warp(voted, word, bit);
 }
 
 // k_quorum_mark for calls in which a group is bound to the accepted proposal's hash (ibft_group_hash): an item of a bound group
@@ -1062,29 +1137,25 @@ __global__ void k_quorum_mark_hashed(const ibft_sig_item* __restrict__ items, ui
                                      const ibft_group_hash* __restrict__ ghash, const group_dev* __restrict__ gdev, uint32_t n_groups,
                                      const slot_dev* __restrict__ slots, uint32_t n_slots, uint32_t* __restrict__ voted,
                                      uint32_t* __restrict__ n_valid, uint32_t* __restrict__ counted, uint32_t lo, uint32_t hi) {
-  uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= hi || i >= n) return;
+  const uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
+  const bool in = i < hi && i < n;
   const ibft_sig_item* it = items + i;
-  const uint32_t g = it->group;
-  bool c = ((bitmap[i >> 5] >> (i & 31)) & 1u) && g < n_groups;
-  ibft_sig_item local;
+  item_tail t{};
+  if (in) t = load_item_tail(it);
+  const uint32_t g = t.group();
+  bool c = in && ((bitmap[i >> 5] >> (i & 31)) & 1u) && g < n_groups;
   if (c) {
-    local = *it;
     const uint32_t mt = ghash != nullptr ? ghash[g].msg_type : IBFT_HASH_UNBOUND;
-    if (mt != IBFT_HASH_UNBOUND) c = item_names_hash(local, arena, arena_len, mt, ghash[g].hash);
+    if (mt != IBFT_HASH_UNBOUND) c = item_names_hash(*it, arena, arena_len, mt, ghash[g].hash);
   }
-  if (counted != nullptr) {
+  if (counted != nullptr && in) {
     if (c) atomicOr(&counted[i >> 5], 1u << (i & 31));
     else atomicAnd(&counted[i >> 5], ~(1u << (i & 31)));
   }
-  if (!c) return;
-  atomicAdd(&n_valid[g], 1u);
-  uint32_t slot = groups[g].table_slot;
-  if (slot == IBFT_NO_TABLE || slot >= n_slots || !slots[slot].valid) return;
-  uint8_t addr[20];
-  if (!item_signer(local, arena, arena_len, addr)) return;
-  int v = lookup_validator(slots[slot], addr);
-  if (v >= 0) atomicOr(&voted[gdev[g].voted_off + ((uint32_t)v >> 5)], 1u << (v & 31));
+  count_valid_warp(n_valid, c, g);
+  uint32_t word = 0, bit = 0;
+  if (c) quorum_vote(t, g, arena, arena_len, groups, gdev, slots, n_slots, &word, &bit);
+  or_votes_warp(voted, word, bit);
 }
 
 // multi-GPU: OR the ranks' partial voted sets and add their valid counts (partial layout: voted words, then one count per group)

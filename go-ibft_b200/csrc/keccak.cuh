@@ -14,15 +14,25 @@ namespace ibft {
 
 IBFT_HD uint64_t rotl64(uint64_t v, int n) { return (v << n) | (v >> (64 - n)); }
 
+#define IBFT_KECCAK_RC                                                                            \
+  {0x0000000000000001ULL, 0x0000000000008082ULL, 0x800000000000808AULL, 0x8000000080008000ULL,    \
+   0x000000000000808BULL, 0x0000000080000001ULL, 0x8000000080008081ULL, 0x8000000000008009ULL,    \
+   0x000000000000008AULL, 0x0000000000000088ULL, 0x0000000080008009ULL, 0x000000008000000AULL,    \
+   0x000000008000808BULL, 0x800000000000008BULL, 0x8000000000008089ULL, 0x8000000000008003ULL,    \
+   0x8000000000008002ULL, 0x8000000000000080ULL, 0x000000000000800AULL, 0x800000008000000AULL,    \
+   0x8000000080008081ULL, 0x8000000000008080ULL, 0x0000000080000001ULL, 0x8000000080008008ULL}
+#if defined(__CUDACC__)
+// round constants in constant memory: every lane of a warp reads the same round's word (a broadcast).  A table local to the
+// function was built in local memory by 24 stores at every inlined permutation.
+__constant__ uint64_t c_keccak_rc[24] = IBFT_KECCAK_RC;
+#endif
 IBFT_HD uint64_t keccak_rc(int i) {
-  const uint64_t rc[24] = {
-      0x0000000000000001ULL, 0x0000000000008082ULL, 0x800000000000808AULL, 0x8000000080008000ULL,
-      0x000000000000808BULL, 0x0000000080000001ULL, 0x8000000080008081ULL, 0x8000000000008009ULL,
-      0x000000000000008AULL, 0x0000000000000088ULL, 0x0000000080008009ULL, 0x000000008000000AULL,
-      0x000000008000808BULL, 0x800000000000008BULL, 0x8000000000008089ULL, 0x8000000000008003ULL,
-      0x8000000000008002ULL, 0x8000000000000080ULL, 0x000000000000800AULL, 0x800000008000000AULL,
-      0x8000000080008081ULL, 0x8000000000008080ULL, 0x0000000080000001ULL, 0x8000000080008008ULL};
+#if defined(__CUDA_ARCH__)
+  return c_keccak_rc[i];
+#else
+  static const uint64_t rc[24] = IBFT_KECCAK_RC;
   return rc[i];
+#endif
 }
 
 IBFT_HD void keccak_f1600(uint64_t* a) {
@@ -113,24 +123,24 @@ IBFT_HD uint64_t load_le64_any(const uint8_t* p) {
 #endif
 }
 
-// Keccak-256 of an arbitrary byte string (multi-block), out = 32 bytes.
-IBFT_HD void keccak256_bytes(const uint8_t* data, uint32_t len, uint8_t* out) {
-  uint64_t st[25];
-#pragma unroll
-  for (int i = 0; i < 25; i++) st[i] = 0;
-  while (len >= 136) {
-#pragma unroll
-    for (int i = 0; i < 17; i++) st[i] ^= load_le64_any(data + 8 * i);
-    keccak_f1600(st);
-    data += 136;
-    len -= 136;
+// Lane q / 8 of the padded message p1[0, n1) || p2[0, n2) || 0x01 || 0 ...: 8 bytes straight from memory when they lie inside one
+// span, else byte by byte.  Every rate block is absorbed through this with compile-time lane indices, so the state stays in
+// registers; a state indexed by a run-time lane count, or a byte buffer staging the first span, lived in local memory.
+IBFT_HD uint64_t sponge_lane(const uint8_t* p1, uint32_t n1, const uint8_t* p2, uint32_t n2, uint64_t q) {
+  const uint64_t n = (uint64_t)n1 + n2;
+  if (q + 8 <= n1) return load_le64_any(p1 + q);
+  if (q >= n1 && q + 8 <= n) return load_le64_any(p2 + (q - n1));
+  uint64_t w = 0;
+  for (int b = 0; b < 8; b++) {
+    const uint64_t t = q + b;
+    const uint64_t x = t < n1 ? p1[t] : t < n ? p2[t - n1] : t == n ? 0x01u : 0u;
+    w |= x << (8 * b);
   }
-  // final (partial) block with padding 0x01 ... 0x80
-  int full = (int)(len >> 3), rem = (int)(len & 7);
-  for (int i = 0; i < full; i++) st[i] ^= load_le64_any(data + 8 * i);
-  st[full] ^= load_le64_partial(data + 8 * full, rem) | ((uint64_t)0x01 << (8 * rem));
-  st[16] ^= 0x8000000000000000ULL;
-  keccak_f1600(st);
+  return w;
+}
+
+// the digest (32 bytes) from the first four lanes of the squeezed state
+IBFT_HD void keccak_squeeze32(const uint64_t* st, uint8_t* out) {
 #pragma unroll
   for (int i = 0; i < 4; i++)
 #pragma unroll
@@ -138,50 +148,38 @@ IBFT_HD void keccak256_bytes(const uint8_t* data, uint32_t len, uint8_t* out) {
 }
 
 // Keccak-256 of the concatenation of two byte spans (a wire frame with its signature field cut out; a ROUND_CHANGE head + its
-// shared prepared certificate).  The first span is staged byte by byte up to a block boundary of the STREAM; from there on every
-// rate block lies entirely inside the second span and is absorbed as 17 lanes read straight from memory (load_le64_any).
+// shared prepared certificate), out = 32 bytes.  One rate block of 17 lanes per permutation; the block that holds the end of the
+// message (possibly all padding) is the last.
 IBFT_HD void keccak256_two_spans(const uint8_t* p1, uint32_t n1, const uint8_t* p2, uint32_t n2, uint8_t* out) {
   uint64_t st[25];
 #pragma unroll
   for (int i = 0; i < 25; i++) st[i] = 0;
-  uint8_t blk[136];
-  uint32_t pos = 0;
-  // span 1, and the bytes of span 2 that complete its last block
-  uint32_t i2 = 0;
-  for (int span = 0; span < 2; span++) {
-    const uint8_t* p = span ? p2 : p1;
-    const uint32_t n = span ? n2 : n1;
-    uint32_t i = 0;
-    for (; i < n && !(span == 1 && pos == 0); i++) {
-      blk[pos] = p[i];
-      if (++pos == 136) {
+  const uint64_t n = (uint64_t)n1 + n2;
+  for (uint64_t q = 0;; q += 136) {
 #pragma unroll
-        for (int k = 0; k < 17; k++) st[k] ^= load_le64_partial(blk + 8 * k, 8);
-        keccak_f1600(st);
-        pos = 0;
-      }
-    }
-    if (span == 1) i2 = i;
-  }
-  // whole blocks of span 2
-  while (n2 - i2 >= 136) {
-#pragma unroll
-    for (int k = 0; k < 17; k++) st[k] ^= load_le64_any(p2 + i2 + 8 * k);
+    for (int k = 0; k < 17; k++) st[k] ^= sponge_lane(p1, n1, p2, n2, q + 8 * k);
+    const bool last = n - q < 136;
+    if (last) st[16] ^= 0x8000000000000000ULL;
     keccak_f1600(st);
-    i2 += 136;
+    if (last) break;
   }
-  // tail (pos == 0 here unless span 2 ended inside the first loop)
-  for (; i2 < n2; i2++) blk[pos++] = p2[i2];
-  for (uint32_t i = pos; i < 136; i++) blk[i] = 0;
-  blk[pos] = 0x01;
-  blk[135] |= 0x80;
+  keccak_squeeze32(st, out);
+}
+
+// Keccak-256 of an arbitrary byte string (multi-block), out = 32 bytes.
+IBFT_HD void keccak256_bytes(const uint8_t* data, uint32_t len, uint8_t* out) { keccak256_two_spans(data, len, data + len, 0, out); }
+
+// Keccak-256(hash32 || 0x02): the digest a committed seal signs (one block, fixed layout: no buffer, no lane index at run time)
+IBFT_HD void keccak256_commit_seal(const uint8_t* hash32, uint8_t* out) {
+  uint64_t st[25];
 #pragma unroll
-  for (int k = 0; k < 17; k++) st[k] ^= load_le64_partial(blk + 8 * k, 8);
+  for (int i = 0; i < 25; i++) st[i] = 0;
+#pragma unroll
+  for (int i = 0; i < 4; i++) st[i] = load_le64_partial(hash32 + 8 * i, 8);
+  st[4] = 0x02ULL | (0x01ULL << 8);  // proto.MessageType_COMMIT, then the padding
+  st[16] = 0x8000000000000000ULL;
   keccak_f1600(st);
-#pragma unroll
-  for (int i = 0; i < 4; i++)
-#pragma unroll
-    for (int j = 0; j < 8; j++) out[8 * i + j] = (uint8_t)(st[i] >> (8 * j));
+  keccak_squeeze32(st, out);
 }
 
 // Keccak-256 of exactly 64 bytes given as two field elements (X||Y big-endian) -> last 20 bytes (the address)

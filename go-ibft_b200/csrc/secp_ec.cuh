@@ -747,12 +747,40 @@ IBFT_HD void ecmult_split_into(const sc& k, ecmult_digits& d, int first) {
   d.kneg[first] = h1.neg; d.kneg[first + 1] = h2.neg;
 }
 
+// The Booth digits of one R stream (WR-bit windows), highest window first, from five registers: c holds (k << 1) << (WR m)
+// mod 2^160 after m windows, so window j's (WR + 1)-bit field (booth_digit: bits WR j - 1 .. WR j + WR - 1 of k) is always the
+// low bits of c[4].  Read with booth_digit at the run-time window and stream, the digits were indexed in local memory, on the
+// chain that picks each table entry.
+struct booth_cursor {
+  uint32_t c[5];
+  bool neg;
+  IBFT_HD void init(const uint32_t* k, bool kneg) {
+#pragma unroll
+    for (int i = 4; i > 0; i--) c[i] = (k[i] << 1) | (k[i - 1] >> 31);
+    c[0] = k[0] << 1;
+    neg = kneg;
+  }
+  IBFT_HD int digit() const {
+    const uint32_t field = c[4] & ((2u << IBFT_WR) - 1u);
+    return (int)((field + 1u) >> 1) - ((int)((field >> IBFT_WR) & 1u) << IBFT_WR);
+  }
+  IBFT_HD void next() {
+#pragma unroll
+    for (int i = 4; i > 0; i--) c[i] = (c[i] << IBFT_WR) | (c[i - 1] >> (32 - IBFT_WR));
+    c[0] <<= IBFT_WR;
+  }
+};
+static_assert(IBFT_WR * (IBFT_NWIN_R - 1) == 128, "the top window's field starts at bit 0 of the cursor's word 4");
+
 // The interleaved window loop over the affine table T (streams 0, 1) and -- when with_g -- the generator table(s).
 IBFT_HD jac ecmult_streams(const ecmult_digits& dg, const gtab_view& G, const rtab_view& T, bool with_g) {
   const fe beta = fe_beta();
   jac acc;
   acc.x = fe_zero(); acc.y = fe_zero(); acc.z = fe_zero();
   acc.inf = true;
+  booth_cursor r0, r1;
+  r0.init(dg.ks[0], dg.kneg[0]);
+  r1.init(dg.ks[1], dg.kneg[1]);
   IBFT_ROLLED
   for (int j = IBFT_NWIN_R - 1; j >= 0; j--) {
     IBFT_OPCOUNT(IBFT_OP_WIN);
@@ -788,18 +816,20 @@ IBFT_HD jac ecmult_streams(const ecmult_digits& dg, const gtab_view& G, const rt
       } else
 #endif
       {
-        int d = s < 2 ? booth_digit<IBFT_WR>(dg.ks[s], j) : booth_digit<IBFT_WG>(dg.ks[s], j / (IBFT_WG / IBFT_WR));
+        int d = s == 0 ? r0.digit() : s == 1 ? r1.digit() : booth_digit<IBFT_WG>(dg.ks[s], j / (IBFT_WG / IBFT_WR));
         if (d == 0) continue;
         int idx = (d < 0 ? -d : d) - 1;
         if (s < 2) T.load(idx, x, y);
         else G.load(idx, x, y);
         use_beta = (s & 1) != 0;
-        neg = (d < 0) != dg.kneg[s];
+        neg = (d < 0) != (s == 0 ? r0.neg : s == 1 ? r1.neg : dg.kneg[s]);
       }
       if (use_beta) x = fe_mul(x, beta);  // lambda * (x, y) = (beta x, y)
       IBFT_OPCOUNT(IBFT_OP_WIN_ADD);
       acc = jac_add_affine(acc, x, y, neg);
     }
+    r0.next();
+    r1.next();
   }
   return acc;
 }

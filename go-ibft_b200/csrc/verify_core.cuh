@@ -48,12 +48,8 @@ IBFT_HD bool item_digest(const ibft_sig_item& it, const uint8_t* arena, size_t a
       return true;
     }
     case IBFT_KIND_SEAL: {
-      if (!want) return true;
-      uint8_t buf[33];
-#pragma unroll
-      for (int i = 0; i < 32; i++) buf[i] = it.digest[i];
-      buf[32] = 0x02;  // proto.MessageType_COMMIT (reference messages/proto/messages.proto:10)
-      keccak256_bytes(buf, 33, z);
+      // z = Keccak-256(proposalHash || 0x02), 0x02 = proto.MessageType_COMMIT (reference messages/proto/messages.proto:10)
+      if (want) keccak256_commit_seal(it.digest, z);
       return true;
     }
     default:
@@ -243,13 +239,7 @@ IBFT_HD int resolve_item(const ibft_sig_item& it, const uint8_t* arena, size_t a
       // IsValidCommittedSeal on the frame: ExtractCommitHash needs type == COMMIT and commitData (messages/helpers.go:51-62),
       // the seal is commitData.committedSeal with Signer = From (:38-48)
       if (f.type != 2 || f.payload_field != 7 || f.hash_len != 32 || f.seal_len != 65) return IBFT_ITEM_OK;
-      if (want_digest) {
-        uint8_t buf[33];
-#pragma unroll
-        for (int i = 0; i < 32; i++) buf[i] = w[f.hash_off + i];
-        buf[32] = 0x02;
-        keccak256_bytes(buf, 33, o.z);
-      }
+      if (want_digest) keccak256_commit_seal(w + f.hash_off, o.z);
 #pragma unroll
       for (int i = 0; i < 32; i++) { o.r[i] = w[f.seal_off + i]; o.s[i] = w[f.seal_off + 32 + i]; }
       o.v = w[f.seal_off + 64];
@@ -264,22 +254,6 @@ IBFT_HD int resolve_item(const ibft_sig_item& it, const uint8_t* arena, size_t a
   o.v = it.v;
   *valid = item_digest(it, arena, arena_len, o.z, want_digest);
   return IBFT_ITEM_OK;
-}
-
-// the expected signer of an item (for the quorum kernels); false when it has none
-IBFT_HD bool item_signer(const ibft_sig_item& it, const uint8_t* arena, size_t arena_len, uint8_t* signer20) {
-  if (it.kind == IBFT_KIND_WIRE || it.kind == IBFT_KIND_WIRE_SEAL) {
-    if ((size_t)it.payload_off + it.payload_len > arena_len) return false;
-    const uint8_t* w = arena + it.payload_off;
-    wire_frame f;
-    if (!parse_wire_frame(w, it.payload_len, f) || f.from_len != 20) return false;
-#pragma unroll
-    for (int i = 0; i < 20; i++) signer20[i] = w[f.from_off + i];
-    return true;
-  }
-#pragma unroll
-  for (int i = 0; i < 20; i++) signer20[i] = it.signer[i];
-  return true;
 }
 
 // Executor dispatch of Q = u1*G + u2*R -> affine (false = point at infinity).  The throughput path keeps its hand-scheduled
