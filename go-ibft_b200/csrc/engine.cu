@@ -33,6 +33,7 @@
 #include "key_share.cuh"
 #include "key_budget.hpp"
 #include "shard_plan.hpp"
+#include "recover_plan.hpp"
 
 #include "secp_gtable.inc"
 
@@ -43,7 +44,6 @@ static_assert(sizeof(ibft_group_desc) == 16, "group descriptor must be 16 bytes"
 static_assert(sizeof(ibft_group_hash) == 48, "group hash binding must be 48 bytes");
 static_assert(IBFT_GTABLE_WG == IBFT_WG, "regenerate secp_gtable.inc (tools/gen_tables.py) for this IBFT_WG");
 
-#define IBFT_BLOCK 128
 #ifndef IBFT_GTAB_SMEM
 #define IBFT_GTAB_SMEM (IBFT_WG <= 8 && IBFT_WC == 0)  // with a combined table the recover kernel never reads the small one
 #endif
@@ -435,7 +435,6 @@ k_verify_known(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
 // inversions) is simply replicated: the kernel does ~4x the work of k_recover and is only used when the batch is too small
 // to fill the machine anyway.  CTA = 128 threads = 32 signatures = one bitmap word.
 // ------------------------------------------------------------------------------------------------------------
-#define IBFT_QUAD_SIGS 32
 __global__ void __launch_bounds__(4 * IBFT_QUAD_SIGS, 2)
 k_recover_quad(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_t* __restrict__ arena, size_t arena_len,
                uint32_t shard_lo, uint32_t shard_hi, const ibft_group_desc* __restrict__ groups, uint32_t n_groups,
@@ -505,8 +504,6 @@ k_recover_quad(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
 // "Split pipeline").  Hand-off through shared memory and named barriers (bar.arrive by the helper, bar.sync by the chain).
 // Capacity of one wave: SMs x 96 signatures (12,672 on an H100).
 // ------------------------------------------------------------------------------------------------------------
-#define IBFT_SPLIT_CHAINS 3
-#define IBFT_SPLIT_SIGS (32 * IBFT_SPLIT_CHAINS)
 // Hand-off slot of the split kernels (k_recover_split, k_verify_split, k_recover_qsplit): word w of signature i at
 // s_slot[w * S + i], S = signatures per CTA.  The two phases have their own flag words: the helper may post phase 2 before a
 // chain warp has read phase 1 -- same bits either way, but two words keep the hand-off free of unordered accesses.
@@ -931,7 +928,6 @@ k_verify_split(const ibft_sig_item* __restrict__ items, uint32_t n, const uint8_
 // the helper supplies the digits of u2 early and y, u1*G later.  Verdict bits are OR-ed into a pre-zeroed bitmap
 // (24 signatures per CTA do not align with the 32-bit words).  Capacity of one wave: SMs x 24 signatures.
 // ------------------------------------------------------------------------------------------------------------
-#define IBFT_QSPLIT_SIGS 24
 #ifndef IBFT_QSPLIT_MIN_CTAS
 #define IBFT_QSPLIT_MIN_CTAS 1
 #endif
@@ -2178,6 +2174,13 @@ template <int BLOCK>
 static decltype(&k_recover<BLOCK, false>) recover_kernel(const ibft_engine* e) {
   return e->d_wtable != nullptr ? k_recover<BLOCK, true> : k_recover<BLOCK, false>;
 }
+// launches kernel k on st, counts it (ibft_launch_count) and returns its launch error
+template <typename... P, typename... A>
+static cudaError_t launch(ibft_engine* e, void (*k)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A... args) {
+  k<<<grid, block, smem, st>>>(args...);
+  e->launches++;
+  return cudaGetLastError();
+}
 // every lane, in index order (validator-table replacement and other engine-wide operations)
 struct all_lanes_lock {
   ibft_engine* e;
@@ -2386,9 +2389,7 @@ static int engine_alloc(ibft_engine* e) {
     // latency kernel's helper warps (36 MB in all: they fit in the H100's 50 MB L2 while a round is being verified)
     size_t entries = (size_t)IBFT_CTAB_ENTRIES;
     CU(cudaMalloc(&e->d_ctable, (size_t)IBFT_CTAB_POSITIONS * entries * IBFT_GTAB_ENTRY_WORDS * 4));
-    k_build_ctable<<<dim3((unsigned)((entries + 63) / 64), IBFT_CTAB_POSITIONS), 64, 0, L->stream>>>(e->d_ctable);
-    e->launches++;
-    CU(cudaGetLastError());
+    CU(launch(e, k_build_ctable, dim3((unsigned)((entries + 63) / 64), IBFT_CTAB_POSITIONS), 64, 0, L->stream, e->d_ctable));
   }
 #endif
   rc = wide_acquire(e, L->stream);
@@ -2887,14 +2888,11 @@ extern "C" int ibft_set_validators(ibft_engine* e, uint32_t table_slot, uint64_t
     if (ce == cudaSuccess && adopt)  // the others of [lo, hi) hold their address already
       ce = cudaMemcpy(e->reg.d_addr + 20 * (size_t)lo, e->reg.addr_of[lo].b, 20 * (size_t)(hi - lo), cudaMemcpyHostToDevice);
     if (ce == cudaSuccess && adopt && e->reg.d_shared) {
-      k_key_share_forget<<<(n + 255) / 256, 256>>>(s.d_key_ref, n, e->reg.d_shared);
-      e->launches++;
-      ce = cudaGetLastError();
+      ce = launch(e, k_key_share_forget, (n + 255) / 256, 256, 0, nullptr, s.d_key_ref, n, e->reg.d_shared);
     }
     if (ce == cudaSuccess && adopt) {
-      k_adopt_entries<<<(n + 255) / 256, 256>>>(s.d_key_ref, n, e->reg.d_state, e->reg.bounded ? e->reg.d_tab : nullptr);
-      e->launches++;
-      ce = cudaGetLastError();
+      ce = launch(e, k_adopt_entries, (n + 255) / 256, 256, 0, nullptr, s.d_key_ref, n, e->reg.d_state,
+                  e->reg.bounded ? e->reg.d_tab : nullptr);
       if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
     }
     for (auto& r : s.key_ref) r &= ~IBFT_KEY_REF_FRESH;
@@ -3081,10 +3079,8 @@ extern "C" int ibft_key_share_export_device(ibft_engine* e, void* d_block, void*
   int rc = key_share_begin(e);
   if (rc != IBFT_OK) return rc;
   const key_registry& R = e->reg;
-  k_key_export<<<1, 1024, 0, stream ? (cudaStream_t)stream : L->stream>>>(R.d_state, R.d_shared, R.d_key_xy, R.d_addr, R.used,
-                                                                          (uint32_t*)d_block);
-  e->launches++;
-  CU(cudaGetLastError());
+  CU(launch(e, k_key_export, 1, 1024, 0, stream ? (cudaStream_t)stream : L->stream, R.d_state, R.d_shared, R.d_key_xy, R.d_addr, R.used,
+            (uint32_t*)d_block));
   return IBFT_OK;
 #else
   (void)stream;
@@ -3112,11 +3108,8 @@ extern "C" int ibft_key_share_adopt_device(ibft_engine* e, const uint64_t* part_
   cudaStream_t st = stream ? (cudaStream_t)stream : L->stream;
   if (d_counts_out) CU(cudaMemsetAsync(d_counts_out, 0, 8, st));
   key_registry& R = e->reg;
-  k_key_adopt<<<dim3(IBFT_KEY_SHARE_RECORDS / 256, n_parts), 256, 0, st>>>(parts, self_part, e->d_slots, e->p.max_table_slots, R.d_state,
-                                                                          R.d_key_xy, R.d_addr, R.d_shared, R.d_learn_count,
-                                                                          (uint32_t*)d_counts_out);
-  e->launches++;
-  CU(cudaGetLastError());
+  CU(launch(e, k_key_adopt, dim3(IBFT_KEY_SHARE_RECORDS / 256, n_parts), 256, 0, st, parts, self_part, e->d_slots, e->p.max_table_slots,
+            R.d_state, R.d_key_xy, R.d_addr, R.d_shared, R.d_learn_count, (uint32_t*)d_counts_out));
   return IBFT_OK;
 #else
   (void)d_counts_out; (void)stream;
@@ -3199,154 +3192,111 @@ static int check_group_hashes(const ibft_group_desc* groups, uint32_t n_groups, 
   return IBFT_OK;
 }
 
+// The arguments every signature kernel takes, for one recover step over items [lo, hi)
+struct sig_args {
+  const ibft_sig_item* items; uint32_t n;
+  const uint8_t* arena; size_t arena_len;
+  uint32_t lo, hi;
+  const ibft_group_desc* groups; uint32_t n_groups;
+  const slot_dev* slots; uint32_t n_slots;
+  uint32_t* bitmap; uint8_t* recovered; uint8_t* status;
+  const uint32_t* ctable; vote_sink sink;
+};
+
+// Launches signature kernel k over a's items.  list: the worklist a known-key pass fills, or the one a recover kernel takes its
+// items from; such a worklist pass leaves the recovered addresses and the statuses to the known-key pass.
+static cudaError_t launch_sig(ibft_engine* e, sig_kernel k, const sig_args& a, uint32_t* list, cudaStream_t st) {
+  auto grid = [&](uint32_t cta_sigs) { return (a.hi - a.lo + cta_sigs - 1) / cta_sigs; };
+  uint8_t* const recovered = list ? nullptr : a.recovered;
+  uint8_t* const status = list ? nullptr : a.status;
+  const uint32_t chain_cta = 32 * (IBFT_SPLIT_CHAINS + 1), rtab_smem = IBFT_RTAB_WORDS * 4;
+#define IBFT_SIG_ARGS a.items, a.n, a.arena, a.arena_len, a.lo, a.hi, a.groups, a.n_groups, a.slots, a.n_slots, a.bitmap
+  switch (k) {
+    case SK_RECOVER_32:
+      return launch(e, recover_kernel<32>(e), grid(32), 32, 32 * rtab_smem, st, IBFT_SIG_ARGS, recovered, status, a.ctable, a.sink, list,
+                    e->d_wtable);
+    case SK_RECOVER_128:
+      return launch(e, recover_kernel<IBFT_BLOCK>(e), grid(IBFT_BLOCK), IBFT_BLOCK, IBFT_BLOCK * rtab_smem, st, IBFT_SIG_ARGS, recovered,
+                    status, a.ctable, a.sink, list, e->d_wtable);
+    case SK_QUAD:
+      return launch(e, k_recover_quad, grid(IBFT_QUAD_SIGS), 4 * IBFT_QUAD_SIGS, 0, st, IBFT_SIG_ARGS, recovered, status, a.ctable, a.sink);
+#if IBFT_WC > 0
+    case SK_SPLIT:
+      return launch(e, k_recover_split, grid(IBFT_SPLIT_SIGS), chain_cta, IBFT_SPLIT_SMEM, st, IBFT_SIG_ARGS, recovered, status, a.ctable,
+                    a.sink);
+    case SK_QSPLIT:
+      return launch(e, k_recover_qsplit, grid(IBFT_QSPLIT_SIGS), 128, 0, st, IBFT_SIG_ARGS, recovered, status, a.ctable, a.sink, list);
+    case SK_VERIFY_KNOWN_32:
+      return launch(e, k_verify_known<32>, grid(32), 32, 0, st, IBFT_SIG_ARGS, a.status, a.ctable, a.sink, list);
+    case SK_VERIFY_KNOWN_128:
+      return launch(e, k_verify_known<IBFT_BLOCK>, grid(IBFT_BLOCK), IBFT_BLOCK, 0, st, IBFT_SIG_ARGS, a.status, a.ctable, a.sink, list);
+    case SK_VERIFY_SPLIT:
+      return launch(e, k_verify_split, grid(IBFT_SPLIT_SIGS), chain_cta, IBFT_VSPLIT_SMEM, st, IBFT_SIG_ARGS, a.status, a.ctable, a.sink,
+                    list);
+#endif
+    default:
+      return cudaErrorInvalidDeviceFunction;  // a kernel this build does not have
+  }
+#undef IBFT_SIG_ARGS
+}
+
+// One recover step over items [lo, hi) on `path` (ibft_set_recover_path): the kernels plan_recover picks (recover_plan.hpp)
 static int launch_recover(ibft_engine* e, lane* L, const ibft_sig_item* d_items, uint32_t n, const uint8_t* d_arena, size_t arena_len,
                           uint32_t lo, uint32_t hi, const ibft_group_desc* d_groups, uint32_t n_groups, uint32_t* d_bitmap,
-                          uint8_t* d_recovered, cudaStream_t st, uint8_t* d_status = nullptr, int forced_path = IBFT_PATH_AUTO,
+                          uint8_t* d_recovered, cudaStream_t st, int path, uint8_t* d_status = nullptr,
                           vote_sink sink = vote_sink{nullptr, nullptr, nullptr}, uint32_t worklist_index = 0) {
   if (hi <= lo) return IBFT_OK;
-  uint32_t* const worklist = L->d_worklist ? L->d_worklist + (size_t)worklist_index * ((size_t)L->cap_items + 1) : nullptr;
-  auto note_worklist = [&]() {  // host-side record for ibft_debug_known_handed_back
-    const uint32_t bit = 1u << (worklist_index & 3u);
-    if (L->wl_used & bit) L->wl_reused = true;
-    L->wl_used |= bit;
-  };
-  // path selection (ibft_set_recover_path).  AUTO picks by how many warps each of the SM's four schedulers would hold:
-  //   <= SMs x 24 signatures   four-lane chain warps + helper warp, one CTA (3 + 1 warps) per SM
-  //   <= SMs x 48              the same, two CTAs per SM (two warps per scheduler)
-  //   <= SMs x 96              chain warps + helper warp, one CTA (3 + 1 warps) per SM (a 10k-validator round)
-  //   <= SMs x 192             the same, two CTAs per SM
-  //   beyond                   one thread per signature: one-warp CTAs while one wave covers them, then the 128-thread
-  //                            throughput kernel
   const uint32_t cnt = hi - lo;
-  int path = forced_path != IBFT_PATH_AUTO ? forced_path : e->recover_path.load();
-  // key-registry path possible: the worklist holds max_items indices (a larger device-resident shard takes the plain recover
-  // path), recovered addresses are not wanted, groups are bound
-  const bool known_ok = (e->p.flags & IBFT_FLAG_KEY_CACHE) && d_recovered == nullptr && d_groups != nullptr && worklist != nullptr &&
-                        cnt <= L->cap_items;
-  // ... and its latency form: one-warp CTAs spread a round over all SMs, and whatever the verification does not accept is
-  // recovered by the four-lane kernel in worklist mode (short payloads only: its helper warp hashes for 24 signatures)
-  const bool small_batch = cnt <= (uint32_t)e->sm_count * 32u * 8u;
-  if (path == IBFT_PATH_AUTO) {
-#if IBFT_WC > 0
-    // with learned keys, verifying against the validator's comb table (51 additions, no doubling) beats every recover kernel at
-    // every batch size -- also the four-lane one: the known-key pass goes first, the recover kernels take what it leaves over
-    if (known_ok) path = IBFT_PATH_THREAD;
-    else
-    // long payloads (ROUND_CHANGE messages with their certificates: up to 909 KB of signed bytes each): the helper warp of the
-    // latency kernels hashes for three (or 24) signatures one after the other, which serialises the sponges that dominate such a
-    // batch -- one thread per signature hashes them all in parallel (config 4: 10,000 x 909 KB)
-    if (arena_len / cnt > 256) path = IBFT_PATH_THREAD;
-    else if (cnt <= (uint32_t)e->sm_count * 2u * IBFT_QSPLIT_SIGS) path = IBFT_PATH_QSPLIT;
-    else if (cnt <= (uint32_t)e->sm_count * 2u * IBFT_SPLIT_SIGS) path = IBFT_PATH_SPLIT;
-    else path = IBFT_PATH_THREAD;
-#else
-    path = cnt <= (uint32_t)e->sm_count * IBFT_QUAD_SIGS ? IBFT_PATH_QUAD : IBFT_PATH_THREAD;
-#endif
+  uint32_t* const worklist = L->d_worklist ? L->d_worklist + (size_t)worklist_index * ((size_t)L->cap_items + 1) : nullptr;
+  const bool known = known_key_ok((e->p.flags & IBFT_FLAG_KEY_CACHE) != 0, d_recovered != nullptr, d_groups != nullptr,
+                                  worklist != nullptr, cnt, L->cap_items);
+  const recover_plan plan = plan_recover(path, cnt, arena_len, (uint32_t)e->sm_count, known, IBFT_WC > 0);
+  const sig_args a{d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots, e->p.max_table_slots, d_bitmap,
+                   d_recovered, d_status, e->d_ctable, sink};
+  if (plan.worklist == SK_NONE) {
+    if (plan.first == SK_QSPLIT)  // its verdict bits are OR-ed in
+      CU(cudaMemsetAsync(d_bitmap + (lo >> 5), 0, (size_t)((hi + 31) / 32 - (lo >> 5)) * 4, st));
+    CU(launch_sig(e, plan.first, a, nullptr, st));
+    return IBFT_OK;
   }
-#if IBFT_WC > 0
-  if (path == IBFT_PATH_QSPLIT) {
-    uint32_t blocks = (cnt + IBFT_QSPLIT_SIGS - 1) / IBFT_QSPLIT_SIGS;
-    CU(cudaMemsetAsync(d_bitmap + (lo >> 5), 0, (size_t)((hi + 31) / 32 - (lo >> 5)) * 4, st));  // verdict bits are OR-ed in
-    k_recover_qsplit<<<blocks, 128, 0, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots,
-                                             e->p.max_table_slots, d_bitmap, d_recovered, d_status, e->d_ctable, sink, nullptr);
-  } else if (path == IBFT_PATH_SPLIT && known_ok) {
-    // known-key latency path: verify against the learned keys, then recover whatever was not accepted (worklist; the second
-    // launch finds it empty -- and returns at once -- when every signature of the round verified)
-    uint32_t blocks = (cnt + IBFT_SPLIT_SIGS - 1) / IBFT_SPLIT_SIGS;
-    note_worklist();
-    CU(cudaStreamWaitEvent(st, L->wl_ev[worklist_index & 3u], 0));
-    CU(cudaMemsetAsync(worklist, 0, 4, st));
-    k_verify_split<<<blocks, 32 * (IBFT_SPLIT_CHAINS + 1), IBFT_VSPLIT_SMEM, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups,
-                                                                              e->d_slots, e->p.max_table_slots, d_bitmap, d_status, e->d_ctable,
-                                                                              sink, worklist);
-    e->launches++;
-    CU(cudaGetLastError());
-    uint32_t blocks2 = (cnt + IBFT_QSPLIT_SIGS - 1) / IBFT_QSPLIT_SIGS;
-    k_recover_qsplit<<<blocks2, 128, 0, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots, e->p.max_table_slots,
-                                              d_bitmap, nullptr, nullptr, e->d_ctable, sink, worklist);
-    CU(cudaEventRecord(L->wl_ev[worklist_index & 3u], st));
-  } else if (path == IBFT_PATH_SPLIT) {
-    uint32_t blocks = (cnt + IBFT_SPLIT_SIGS - 1) / IBFT_SPLIT_SIGS;
-    k_recover_split<<<blocks, 32 * (IBFT_SPLIT_CHAINS + 1), IBFT_SPLIT_SMEM, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups,
-                                                                              e->d_slots, e->p.max_table_slots, d_bitmap, d_recovered,
-                                                                              d_status, e->d_ctable, sink);
-  } else
-#endif
-  if (path == IBFT_PATH_QUAD) {
-    uint32_t blocks = (cnt + IBFT_QUAD_SIGS - 1) / IBFT_QUAD_SIGS;
-    k_recover_quad<<<blocks, 4 * IBFT_QUAD_SIGS, 0, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots,
-                                                         e->p.max_table_slots, d_bitmap, d_recovered, d_status, e->d_ctable, sink);
-  } else
-#if IBFT_WC > 0
-  if (known_ok) {
-    // key-registry path (one thread per signature, any batch size): verify what can be verified, then recover the rest from
-    // the worklist (dense second launch; the threads beyond the worklist's length leave at once)
-    // device-resident callers may use different streams: launches sharing a worklist are ordered on the device
-    note_worklist();
-    CU(cudaStreamWaitEvent(st, L->wl_ev[worklist_index & 3u], 0));
-    CU(cudaMemsetAsync(worklist, 0, 4, st));
-    if (small_batch) {
-      k_verify_known<32><<<(cnt + 31) / 32, 32, 0, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots,
-                                                        e->p.max_table_slots, d_bitmap, d_status, e->d_ctable, sink, worklist);
-    } else {
-      k_verify_known<IBFT_BLOCK><<<(cnt + IBFT_BLOCK - 1) / IBFT_BLOCK, IBFT_BLOCK, 0, st>>>(
-          d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots, e->p.max_table_slots, d_bitmap, d_status, e->d_ctable, sink,
-          worklist);
-    }
-    e->launches++;
-    CU(cudaGetLastError());
-    if (small_batch && arena_len / cnt <= 256) {
-      k_recover_qsplit<<<(cnt + IBFT_QSPLIT_SIGS - 1) / IBFT_QSPLIT_SIGS, 128, 0, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups,
-                                                                                    e->d_slots, e->p.max_table_slots, d_bitmap, nullptr, nullptr,
-                                                                                    e->d_ctable, sink, worklist);
-    } else {
-      recover_kernel<IBFT_BLOCK>(e)<<<(cnt + IBFT_BLOCK - 1) / IBFT_BLOCK, IBFT_BLOCK, IBFT_BLOCK * IBFT_RTAB_WORDS * 4, st>>>(
-          d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots, e->p.max_table_slots, d_bitmap, nullptr, nullptr, e->d_ctable,
-          sink, worklist, e->d_wtable);
-    }
-    CU(cudaEventRecord(L->wl_ev[worklist_index & 3u], st));
-  } else
-#endif
-  if (small_batch) {  // one-warp CTAs
-    uint32_t blocks = (cnt + 31) / 32;
-    recover_kernel<32>(e)<<<blocks, 32, 32 * IBFT_RTAB_WORDS * 4, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots,
-                                         e->p.max_table_slots, d_bitmap, d_recovered, d_status, e->d_ctable, sink, nullptr, e->d_wtable);
-  } else {
-    uint32_t blocks = (cnt + IBFT_BLOCK - 1) / IBFT_BLOCK;
-    recover_kernel<IBFT_BLOCK>(e)<<<blocks, IBFT_BLOCK, IBFT_BLOCK * IBFT_RTAB_WORDS * 4, st>>>(d_items, n, d_arena, arena_len, lo, hi, d_groups, n_groups, e->d_slots,
-                                                         e->p.max_table_slots, d_bitmap, d_recovered, d_status, e->d_ctable, sink, nullptr,
-                                                         e->d_wtable);
-  }
-  e->launches++;
-  CU(cudaGetLastError());
+  // the known-key pass, then the recover pass over the worklist of what it did not accept (which finds it empty, and returns at
+  // once, when every signature verified).  Device-resident callers may use different streams: launches sharing a worklist are
+  // ordered on the device.
+  const uint32_t bit = 1u << (worklist_index & 3u);  // host-side record for ibft_debug_known_handed_back
+  if (L->wl_used & bit) L->wl_reused = true;
+  L->wl_used |= bit;
+  CU(cudaStreamWaitEvent(st, L->wl_ev[worklist_index & 3u], 0));
+  CU(cudaMemsetAsync(worklist, 0, 4, st));
+  CU(launch_sig(e, plan.first, a, worklist, st));
+  CU(launch_sig(e, plan.worklist, a, worklist, st));
+  CU(cudaEventRecord(L->wl_ev[worklist_index & 3u], st));
   return IBFT_OK;
 }
 
-static int launch_quorum(ibft_engine* e, lane* L, const ibft_sig_item* d_items, uint32_t n, const uint8_t* d_arena, size_t arena_len, const uint32_t* d_bitmap,
-                         const ibft_group_desc* d_groups, const group_dev* d_gdev, uint32_t n_groups, size_t voted_words,
-                         ibft_group_result* d_results, cudaStream_t st, bool already_marked = false,
-                         const ibft_group_hash* d_ghash = nullptr, uint32_t* d_counted = nullptr) {
-  if (n_groups == 0) return IBFT_OK;
-  if (!already_marked) {
-    CU(cudaMemsetAsync(L->d_voted, 0, std::max<size_t>(voted_words, 1) * 4, st));
-    CU(cudaMemsetAsync(L->d_nvalid, 0, (size_t)n_groups * 4, st));
-  }
-  if (n && !already_marked && (d_ghash != nullptr || d_counted != nullptr)) {
-    k_quorum_mark_hashed<<<(n + 255) / 256, 256, 0, st>>>(d_items, n, d_arena, arena_len, d_bitmap, d_groups, d_ghash, d_gdev, n_groups,
-                                                           e->d_slots, e->p.max_table_slots, L->d_voted, L->d_nvalid, d_counted, 0u, n);
-    e->launches++;
-    CU(cudaGetLastError());
-  } else if (n && !already_marked) {
-    k_quorum_mark<<<(n + 255) / 256, 256, 0, st>>>(d_items, n, d_arena, arena_len, d_bitmap, d_groups, d_gdev, n_groups, e->d_slots,
-                                                    e->p.max_table_slots, L->d_voted, L->d_nvalid, 0u, n);
-    e->launches++;
-    CU(cudaGetLastError());
-  }
-  k_quorum_reduce<<<n_groups, IBFT_REDUCE_THREADS, 0, st>>>(d_groups, d_gdev, n_groups, e->d_slots, e->p.max_table_slots, L->d_voted,
-                                            L->d_nvalid, d_results);
-  e->launches++;
-  CU(cudaGetLastError());
-  return IBFT_OK;
+// Marks the votes of the passing items of [lo, hi) into voted / nvalid: k_quorum_mark_hashed when a group is bound to a hash
+// (d_ghash) or the counted bits are wanted, else k_quorum_mark
+static cudaError_t mark_votes(ibft_engine* e, lane* L, const ibft_sig_item* d_items, uint32_t n, const uint8_t* d_arena, size_t arena_len,
+                              const uint32_t* d_bitmap, uint32_t n_groups, const ibft_group_hash* d_ghash, uint32_t* d_counted,
+                              uint32_t* voted, uint32_t* nvalid, uint32_t lo, uint32_t hi, cudaStream_t st) {
+  const uint32_t grid = (hi - lo + 255) / 256;
+  if (d_ghash || d_counted)
+    return launch(e, k_quorum_mark_hashed, grid, 256, 0, st, d_items, n, d_arena, arena_len, d_bitmap, L->d_groups, d_ghash, L->d_gdev,
+                  n_groups, e->d_slots, e->p.max_table_slots, voted, nvalid, d_counted, lo, hi);
+  return launch(e, k_quorum_mark, grid, 256, 0, st, d_items, n, d_arena, arena_len, d_bitmap, L->d_groups, L->d_gdev, n_groups,
+                e->d_slots, e->p.max_table_slots, voted, nvalid, lo, hi);
+}
+
+// the quorum decision of each of the lane's groups from its voted sets
+static cudaError_t reduce_votes(ibft_engine* e, lane* L, uint32_t n_groups, ibft_group_result* d_results, cudaStream_t st) {
+  return launch(e, k_quorum_reduce, n_groups, IBFT_REDUCE_THREADS, 0, st, L->d_groups, L->d_gdev, n_groups, e->d_slots,
+                e->p.max_table_slots, L->d_voted, L->d_nvalid, d_results);
+}
+
+// words of the voted sets of the lane's groups
+static size_t lane_voted_words(const lane* L) {
+  size_t words = 0;
+  for (const group_dev& g : L->last_gdev) words += g.n_words;
+  return words;
 }
 
 // Staging copy of a chunk of pageable caller memory (a cgo caller's Go heap) into the lane's pinned buffer.  One thread moves
@@ -3443,20 +3393,15 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
     else (void)cudaGetLastError();
   }
   int rc = IBFT_OK;
-#if IBFT_WC > 0
-  // One mid-size round (the chain + helper kernel's range, e.g. 10,000 seals = 1.28 MB of tuples): the staging copy and the
-  // H2D transfer would sit in front of a kernel that cannot start before its last tuple has arrived.  Cut the round into four
-  // pieces, each with its own stream -- stage, copy and launch piece k while piece k+1 is being staged; the four kernels
-  // (<= 37 CTAs each) run side by side on different SMs and the main stream joins them before the quorum kernels.
-  const bool lat_pieces = e->recover_path.load() == IBFT_PATH_AUTO && n > (uint32_t)e->sm_count * 2u * IBFT_QSPLIT_SIGS &&
-                          n <= (uint32_t)e->sm_count * IBFT_SPLIT_SIGS && arena_len / n <= 256;
-  if (lat_pieces) {
+  const int path = e->recover_path.load();  // read once: a concurrent ibft_set_recover_path cannot mix kernels within the call
+  // a mid-size round in latency pieces (recover_plan.hpp); the main stream joins them before the quorum kernels
+  const bool known = known_key_ok((e->p.flags & IBFT_FLAG_KEY_CACHE) != 0, recovered_out != nullptr, n_groups != 0,
+                                  L->d_worklist != nullptr, n, L->cap_items);
+  const piece_plan pieces = plan_pieces(path, n, arena_len, (uint32_t)e->sm_count, known, IBFT_WC > 0);
+  if (pieces.per) {
     CU(cudaEventRecord(L->lat_ev[4], st));  // arena / groups uploads of this call
-    const uint32_t per = ((n + 3) / 4 + IBFT_SPLIT_SIGS - 1) / IBFT_SPLIT_SIGS * IBFT_SPLIT_SIGS;
-    // with a key registry the pieces go through the known-key pass (one-warp CTAs) + worklist; without, chain + helper warps
-    const int piece_path = ((e->p.flags & IBFT_FLAG_KEY_CACHE) && !recovered_out && n_groups && L->d_worklist) ? IBFT_PATH_THREAD : IBFT_PATH_SPLIT;
-    for (uint32_t c = 0; c < 4; c++) {
-      uint32_t lo = std::min(n, c * per), hi = std::min(n, lo + per);
+    for (uint32_t c = 0; c < IBFT_LAT_PIECES; c++) {
+      uint32_t lo = std::min(n, c * pieces.per), hi = std::min(n, lo + pieces.per);
       if (hi <= lo) break;
       cudaStream_t ls = L->lat_stream[c];
       const ibft_sig_item* src = items + lo;
@@ -3467,14 +3412,13 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
       CU(cudaStreamWaitEvent(ls, L->lat_ev[4], 0));
       CU(cudaMemcpyAsync(L->d_items + lo, src, (size_t)(hi - lo) * sizeof(ibft_sig_item), cudaMemcpyHostToDevice, ls));
       rc = launch_recover(e, L, L->d_items, n, L->d_arena, arena_len, lo, hi, n_groups ? L->d_groups : nullptr, n_groups, L->d_bitmap,
-                          recovered_out ? L->d_recovered : nullptr, ls, L->d_status, piece_path, sink, c);
+                          recovered_out ? L->d_recovered : nullptr, ls, pieces.path, L->d_status, sink, c);
       if (rc != IBFT_OK) return rc;
       CU(cudaEventRecord(L->lat_ev[c], ls));
       CU(cudaStreamWaitEvent(st, L->lat_ev[c], 0));
     }
     n_chunks = 0;  // the generic chunk loop below has nothing left to do
   }
-#endif
   // Several chunks: chunk c's kernels run on one of two alternating streams, so that the tail of one chunk (the last CTAs of a
   // 1,024-CTA launch on 444 resident slots) overlaps the head of the next instead of idling the SMs eight times per batch.
   if (n_chunks > 1) {
@@ -3497,7 +3441,7 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
       CU(cudaStreamWaitEvent(ks, L->chunk_ev[c], 0));
     }
     rc = launch_recover(e, L, L->d_items, n, L->d_arena, arena_len, lo, hi, n_groups ? L->d_groups : nullptr, n_groups, L->d_bitmap,
-                        recovered_out ? L->d_recovered : nullptr, ks, L->d_status, IBFT_PATH_AUTO, sink, c & 1u);
+                        recovered_out ? L->d_recovered : nullptr, ks, path, L->d_status, sink, c & 1u);
     if (rc != IBFT_OK) return rc;
   }
   if (n_chunks > 1) {
@@ -3507,17 +3451,12 @@ static int submit_locked(ibft_engine* e, lane* L, const ibft_sig_item* items, ui
     }
   }
   if (hashed && n) {
-    k_quorum_mark_hashed<<<(n + 255) / 256, 256, 0, st>>>(L->d_items, n, L->d_arena, arena_len, L->d_bitmap, L->d_groups, L->d_ghash, L->d_gdev,
-                                                           n_groups, e->d_slots, e->p.max_table_slots, L->d_voted, L->d_nvalid, L->d_counted,
-                                                           0u, n);
-    e->launches++;
-    CU(cudaGetLastError());
+    CU(mark_votes(e, L, L->d_items, n, L->d_arena, arena_len, L->d_bitmap, n_groups, L->d_ghash, L->d_counted, L->d_voted, L->d_nvalid, 0u, n,
+                  st));
     if (counted_out) CU(cudaMemcpyAsync(L->h_counted, L->d_counted, (size_t)((n + 31) / 32) * 4, cudaMemcpyDeviceToHost, st));
   }
   if (n_groups && results_out) {
-    rc = launch_quorum(e, L, L->d_items, n, L->d_arena, arena_len, L->d_bitmap, L->d_groups, L->d_gdev, n_groups, voted_words, L->d_results, st,
-                       /*already_marked=*/true);
-    if (rc != IBFT_OK) return rc;
+    CU(reduce_votes(e, L, n_groups, L->d_results, st));
     CU(cudaMemcpyAsync(L->h_results, L->d_results, (size_t)n_groups * sizeof(ibft_group_result), cudaMemcpyDeviceToHost, st));
   }
   if (n) {
@@ -3725,11 +3664,9 @@ static int explain_batch(ibft_engine* e, const ibft_sig_item* items, uint32_t n,
     }
     CU(cudaMemcpyAsync(L->d_items, L->h_items, (size_t)m * sizeof(ibft_sig_item), cudaMemcpyHostToDevice, st));
     auto kernel = e->d_wtable != nullptr ? k_explain<true> : k_explain<false>;
-    kernel<<<(m + 31) / 32, 32, 32 * IBFT_RTAB_WORDS * 4, st>>>(L->d_items, m, L->d_arena, arena_len, n_groups ? d_groups : nullptr, n_groups,
-                                                                e->d_slots, e->p.max_table_slots, e->d_ctable, e->d_wtable, L->d_status,
-                                                                L->d_recovered);
-    e->launches++;
-    CU(cudaGetLastError());
+    CU(launch(e, kernel, (m + 31) / 32, 32, 32 * IBFT_RTAB_WORDS * 4, st, L->d_items, m, L->d_arena, arena_len,
+              n_groups ? d_groups : nullptr, n_groups, e->d_slots, e->p.max_table_slots, e->d_ctable, e->d_wtable, L->d_status,
+              L->d_recovered));
     // the answers land in the pinned tuple staging, which the upload above (same stream) has finished with
     uint8_t* h_out = reinterpret_cast<uint8_t*>(L->h_items);
     CU(cudaMemcpyAsync(h_out, L->d_status, m, cudaMemcpyDeviceToHost, st));
@@ -3815,7 +3752,7 @@ extern "C" int ibft_verify_batch_device(ibft_engine* e, const void* d_items, uin
   // membership is applied by ibft_quorum_reduce_device / the host mirror in this mode when no groups are bound
   return launch_recover(e, L, (const ibft_sig_item*)d_items, n, (const uint8_t*)d_arena, arena_len, shard_lo, shard_hi,
                         L->last_groups.empty() ? nullptr : L->d_groups, (uint32_t)L->last_groups.size(), (uint32_t*)d_bitmap,
-                        (uint8_t*)d_recovered, st);
+                        (uint8_t*)d_recovered, st, e->recover_path.load());
 }
 
 extern "C" int ibft_explain_batch_device(ibft_engine* e, const void* d_items, uint32_t n, const void* d_arena, size_t arena_len,
@@ -3845,15 +3782,11 @@ extern "C" int ibft_explain_batch_device(ibft_engine* e, const void* d_items, ui
   for (uint32_t lo = shard_lo; lo < shard_hi; lo += std::min(chunk, shard_hi - lo)) {
     const uint32_t cnt = std::min(chunk, shard_hi - lo);
     CU(cudaMemsetAsync(wl, 0, 4, st));
-    k_explain_compact<<<(cnt + 255) / 256, 256, 0, st>>>((const uint32_t*)d_bitmap, lo, lo + cnt, (uint8_t*)d_reasons,
-                                                         (uint8_t*)d_recovered, wl, count);
-    e->launches++;
-    CU(cudaGetLastError());
-    kernel<<<(cnt + 31) / 32, 32, 32 * IBFT_RTAB_WORDS * 4, st>>>((const ibft_sig_item*)d_items, (const uint8_t*)d_arena, arena_len, groups,
-                                                                  n_groups, e->d_slots, e->p.max_table_slots, e->d_ctable, e->d_wtable, wl,
-                                                                  (uint8_t*)d_reasons, (uint8_t*)d_recovered);
-    e->launches++;
-    CU(cudaGetLastError());
+    CU(launch(e, k_explain_compact, (cnt + 255) / 256, 256, 0, st, (const uint32_t*)d_bitmap, lo, lo + cnt, (uint8_t*)d_reasons,
+              (uint8_t*)d_recovered, wl, count));
+    CU(launch(e, kernel, (cnt + 31) / 32, 32, 32 * IBFT_RTAB_WORDS * 4, st, (const ibft_sig_item*)d_items, (const uint8_t*)d_arena,
+              arena_len, groups, n_groups, e->d_slots, e->p.max_table_slots, e->d_ctable, e->d_wtable, wl, (uint8_t*)d_reasons,
+              (uint8_t*)d_recovered));
   }
   CU(cudaEventRecord(e->explain_ev, st));
   return IBFT_OK;
@@ -3927,11 +3860,14 @@ extern "C" int ibft_quorum_reduce_device_ex(ibft_engine* e, const void* d_items,
   (void)d_groups;  // the bound copy is authoritative (its voted-set layout was planned on the host)
   CU(cudaSetDevice(e->p.device));
   cudaStream_t st = stream ? (cudaStream_t)stream : L->stream;
-  size_t voted_words = 0;
-  for (auto& g : L->last_gdev) voted_words += g.n_words;
-  return launch_quorum(e, L, (const ibft_sig_item*)d_items, n, L->dev_arena, L->dev_arena_len, (const uint32_t*)d_bitmap, L->d_groups,
-                       L->d_gdev, n_groups, voted_words, (ibft_group_result*)d_results, st, false,
-                       L->last_hashes.empty() ? nullptr : L->d_ghash, (uint32_t*)d_counted);
+  if (n_groups == 0) return IBFT_OK;
+  CU(cudaMemsetAsync(L->d_voted, 0, std::max<size_t>(lane_voted_words(L), 1) * 4, st));
+  CU(cudaMemsetAsync(L->d_nvalid, 0, (size_t)n_groups * 4, st));
+  if (n)
+    CU(mark_votes(e, L, (const ibft_sig_item*)d_items, n, L->dev_arena, L->dev_arena_len, (const uint32_t*)d_bitmap, n_groups,
+                  L->last_hashes.empty() ? nullptr : L->d_ghash, (uint32_t*)d_counted, L->d_voted, L->d_nvalid, 0u, n, st));
+  CU(reduce_votes(e, L, n_groups, (ibft_group_result*)d_results, st));
+  return IBFT_OK;
 }
 
 extern "C" int ibft_quorum_partial_words(ibft_engine* e, uint32_t* words_out) {
@@ -3939,9 +3875,7 @@ extern "C" int ibft_quorum_partial_words(ibft_engine* e, uint32_t* words_out) {
   if (!e || !words_out) { set_err("null argument"); return IBFT_ERR_INVALID_ARG; }
   lane* L = &e->lanes[0];
   std::lock_guard<std::mutex> lk(L->mu);
-  size_t voted_words = 0;
-  for (auto& g : L->last_gdev) voted_words += g.n_words;
-  *words_out = (uint32_t)(voted_words + L->last_groups.size());
+  *words_out = (uint32_t)(lane_voted_words(L) + L->last_groups.size());
   return IBFT_OK;
 }
 
@@ -3961,24 +3895,12 @@ extern "C" int ibft_quorum_mark_device_ex(ibft_engine* e, const void* d_items, u
   if (n_groups == 0) { set_err("call ibft_bind_groups first"); return IBFT_ERR_INVALID_ARG; }
   CU(cudaSetDevice(e->p.device));
   cudaStream_t st = stream ? (cudaStream_t)stream : L->stream;
-  size_t voted_words = 0;
-  for (auto& g : L->last_gdev) voted_words += g.n_words;
+  const size_t voted_words = lane_voted_words(L);
   uint32_t* part = (uint32_t*)d_partial;
   CU(cudaMemsetAsync(part, 0, (voted_words + n_groups) * 4, st));
-  if (shard_hi > shard_lo && (!L->last_hashes.empty() || d_counted != nullptr)) {
-    k_quorum_mark_hashed<<<(shard_hi - shard_lo + 255) / 256, 256, 0, st>>>(
-        (const ibft_sig_item*)d_items, n, L->dev_arena, L->dev_arena_len, (const uint32_t*)d_bitmap, L->d_groups,
-        L->last_hashes.empty() ? nullptr : L->d_ghash, L->d_gdev, n_groups, e->d_slots, e->p.max_table_slots, part, part + voted_words,
-        (uint32_t*)d_counted, shard_lo, shard_hi);
-    e->launches++;
-    CU(cudaGetLastError());
-  } else if (shard_hi > shard_lo) {
-    k_quorum_mark<<<(shard_hi - shard_lo + 255) / 256, 256, 0, st>>>((const ibft_sig_item*)d_items, n, L->dev_arena, L->dev_arena_len,
-                                                                     (const uint32_t*)d_bitmap, L->d_groups, L->d_gdev, n_groups, e->d_slots,
-                                                                     e->p.max_table_slots, part, part + voted_words, shard_lo, shard_hi);
-    e->launches++;
-    CU(cudaGetLastError());
-  }
+  if (shard_hi > shard_lo)
+    CU(mark_votes(e, L, (const ibft_sig_item*)d_items, n, L->dev_arena, L->dev_arena_len, (const uint32_t*)d_bitmap, n_groups,
+                  L->last_hashes.empty() ? nullptr : L->d_ghash, (uint32_t*)d_counted, part, part + voted_words, shard_lo, shard_hi, st));
   return IBFT_OK;
 }
 
@@ -3992,18 +3914,12 @@ extern "C" int ibft_quorum_merge_device(ibft_engine* e, const void* d_partials, 
   if (n_groups == 0) { set_err("call ibft_bind_groups first"); return IBFT_ERR_INVALID_ARG; }
   CU(cudaSetDevice(e->p.device));
   cudaStream_t st = stream ? (cudaStream_t)stream : L->stream;
-  size_t voted_words = 0;
-  for (auto& g : L->last_gdev) voted_words += g.n_words;
+  const size_t voted_words = lane_voted_words(L);
   if (part_stride_words < voted_words + n_groups) { set_err("partial stride too small"); return IBFT_ERR_INVALID_ARG; }
   uint32_t total = (uint32_t)(voted_words + n_groups);
-  k_quorum_merge<<<(total + 255) / 256, 256, 0, st>>>((const uint32_t*)d_partials, n_parts, part_stride_words, (uint32_t)voted_words,
-                                                      n_groups, L->d_voted, L->d_nvalid);
-  e->launches++;
-  CU(cudaGetLastError());
-  k_quorum_reduce<<<n_groups, IBFT_REDUCE_THREADS, 0, st>>>(L->d_groups, L->d_gdev, n_groups, e->d_slots, e->p.max_table_slots, L->d_voted, L->d_nvalid,
-                                            (ibft_group_result*)d_results);
-  e->launches++;
-  CU(cudaGetLastError());
+  CU(launch(e, k_quorum_merge, (total + 255) / 256, 256, 0, st, (const uint32_t*)d_partials, n_parts, part_stride_words,
+            (uint32_t)voted_words, n_groups, L->d_voted, L->d_nvalid));
+  CU(reduce_votes(e, L, n_groups, (ibft_group_result*)d_results, st));
   return IBFT_OK;
 }
 
@@ -4071,8 +3987,7 @@ extern "C" int ibft_quorum_exchange_device(ibft_engine* e, const uint64_t* peer_
   std::lock_guard<std::mutex> lk(L->mu);
   uint32_t n_groups = (uint32_t)L->last_groups.size();
   if (n_groups == 0) { set_err("call ibft_bind_groups first"); return IBFT_ERR_INVALID_ARG; }
-  size_t voted_words = 0;
-  for (auto& g : L->last_gdev) voted_words += g.n_words;
+  const size_t voted_words = lane_voted_words(L);
   if (words_per_rank < bitmap_words_per_rank + voted_words + n_groups) { set_err("exchange buffer too small"); return IBFT_ERR_INVALID_ARG; }
   CU(cudaSetDevice(e->p.device));
   cudaStream_t st = stream ? (cudaStream_t)stream : L->stream;
@@ -4082,15 +3997,9 @@ extern "C" int ibft_quorum_exchange_device(ibft_engine* e, const uint64_t* peer_
   }
   const uint32_t total = world * bitmap_words_per_rank + (uint32_t)voted_words + n_groups;
   const uint32_t blocks = std::max(1u, std::min(64u, (total + 255u) / 256u));
-  k_quorum_exchange<<<blocks, 256, 0, st>>>(pb, world, rank, words_per_rank, bitmap_words_per_rank, (uint32_t)voted_words, n_groups, epoch,
-                                            /*spin_limit=*/400000u, (uint32_t*)d_bitmap_full, L->d_voted, L->d_nvalid,
-                                            (uint32_t*)d_timeout_flag);
-  e->launches++;
-  CU(cudaGetLastError());
-  k_quorum_reduce<<<n_groups, IBFT_REDUCE_THREADS, 0, st>>>(L->d_groups, L->d_gdev, n_groups, e->d_slots, e->p.max_table_slots, L->d_voted, L->d_nvalid,
-                                            (ibft_group_result*)d_results);
-  e->launches++;
-  CU(cudaGetLastError());
+  CU(launch(e, k_quorum_exchange, blocks, 256, 0, st, pb, world, rank, words_per_rank, bitmap_words_per_rank, (uint32_t)voted_words,
+            n_groups, epoch, /*spin_limit=*/400000u, (uint32_t*)d_bitmap_full, L->d_voted, L->d_nvalid, (uint32_t*)d_timeout_flag));
+  CU(reduce_votes(e, L, n_groups, (ibft_group_result*)d_results, st));
   return IBFT_OK;
 }
 
@@ -4149,10 +4058,8 @@ static int hash_batch_locked(ibft_engine* e, const uint8_t* arena, size_t arena_
     CU(cudaMemcpyAsync(e->hs_arena, e->hs_h_arena, arena_len, cudaMemcpyHostToDevice, st));
   }
   CU(cudaMemcpyAsync(dm, hm, o_out, cudaMemcpyHostToDevice, st));
-  k_keccak_batch<<<(n + 63) / 64, 64, 0, st>>>(e->hs_arena, arena_len, (const uint32_t*)(dm + o_off), (const uint32_t*)(dm + o_len),
-                                               rounds ? (const uint64_t*)dm : nullptr, n, dm + o_out);
-  e->launches++;
-  CU(cudaGetLastError());
+  CU(launch(e, k_keccak_batch, (n + 63) / 64, 64, 0, st, e->hs_arena, arena_len, (const uint32_t*)(dm + o_off),
+            (const uint32_t*)(dm + o_len), rounds ? (const uint64_t*)dm : nullptr, n, dm + o_out));
   CU(cudaMemcpyAsync(hm + o_out, dm + o_out, (size_t)n * 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   memcpy(out32, hm + o_out, (size_t)n * 32);
@@ -4201,9 +4108,7 @@ static int sign_batch(ibft_engine* e, const uint8_t* privkeys, const uint8_t* di
     CUK(cudaMalloc(&d_k, (size_t)n * 32));
     CUK(cudaMemcpyAsync(d_k, nonces, (size_t)n * 32, cudaMemcpyHostToDevice, L->stream));
   }
-  k_sign<<<(n + 63) / 64, 64, 0, L->stream>>>(d_d, d_z, d_k, rfc6979, n, d_s);
-  e->launches++;
-  CUK(cudaGetLastError());
+  CUK(launch(e, k_sign, (n + 63) / 64, 64, 0, L->stream, d_d, d_z, d_k, rfc6979, n, d_s));
   CUK(cudaMemcpyAsync(sigs65_out, d_s, (size_t)n * 65, cudaMemcpyDeviceToHost, L->stream));
   CUK(cudaStreamSynchronize(L->stream));
   // private keys do not stay on the device
@@ -4301,9 +4206,7 @@ extern "C" int ibft_debug_op(ibft_engine* e, int op, const uint8_t* a, const uin
   if (c) { CUK(cudaMalloc(&d_c, (size_t)n * 64)); CUK(cudaMemcpyAsync(d_c, c, (size_t)n * 64, cudaMemcpyHostToDevice, L->stream)); }
   CUK(cudaMalloc(&d_o, (size_t)n * out_stride));
   CUK(cudaMemsetAsync(d_o, 0, (size_t)n * out_stride, L->stream));
-  k_debug_op<<<(n + 63) / 64, 64, 0, L->stream>>>(op, d_a, d_b, d_c, n, d_o, out_stride);
-  e->launches++;
-  CUK(cudaGetLastError());
+  CUK(launch(e, k_debug_op, (n + 63) / 64, 64, 0, L->stream, op, d_a, d_b, d_c, n, d_o, out_stride));
   CUK(cudaMemcpyAsync(out, d_o, (size_t)n * out_stride, cudaMemcpyDeviceToHost, L->stream));
   CUK(cudaStreamSynchronize(L->stream));
 done:
@@ -4420,8 +4323,7 @@ static int for_devices(uint32_t used, bool parallel, const std::function<int(uin
 static int multi_merge_enqueue(multi_engine* M, int kind, uint32_t used, uint32_t n_groups) {
   ibft_engine* lead = M->subs[0];
   lane* L0 = &lead->lanes[kind];
-  size_t vw = 0;
-  for (auto& g : L0->last_gdev) vw += g.n_words;
+  const size_t vw = lane_voted_words(L0);
   const size_t stride = vw + n_groups;
   CU(cudaSetDevice(lead->p.device));
   cudaStream_t st = L0->stream;
@@ -4436,14 +4338,9 @@ static int multi_merge_enqueue(multi_engine* M, int kind, uint32_t used, uint32_
     CU(cudaMemcpyPeerAsync(dst + vw, lead->p.device, L->d_nvalid, s->p.device, (size_t)n_groups * 4, st));
     parts++;
   }
-  k_quorum_merge<<<(uint32_t)((stride + 255) / 256), 256, 0, st>>>(M->d_parts[kind], parts, (uint32_t)stride, (uint32_t)vw, n_groups,
-                                                                   L0->d_voted, L0->d_nvalid);
-  lead->launches++;
-  CU(cudaGetLastError());
-  k_quorum_reduce<<<n_groups, IBFT_REDUCE_THREADS, 0, st>>>(L0->d_groups, L0->d_gdev, n_groups, lead->d_slots, lead->p.max_table_slots,
-                                                            L0->d_voted, L0->d_nvalid, L0->d_results);
-  lead->launches++;
-  CU(cudaGetLastError());
+  CU(launch(lead, k_quorum_merge, (uint32_t)((stride + 255) / 256), 256, 0, st, M->d_parts[kind], parts, (uint32_t)stride, (uint32_t)vw,
+            n_groups, L0->d_voted, L0->d_nvalid));
+  CU(reduce_votes(lead, L0, n_groups, L0->d_results, st));
   CU(cudaMemcpyAsync(L0->h_results, L0->d_results, (size_t)n_groups * sizeof(ibft_group_result), cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(M->merged[kind], st));
   return IBFT_OK;
@@ -4580,10 +4477,8 @@ static int multi_adopt_keys(multi_engine* M) {
       // state first: a key the state copy shows as learned was written before that state (learn_key's fence)
       CU(cudaMemcpyPeerAsync(sc, D->p.device, S->reg.d_state, S->p.device, (size_t)n * 4, ks));
       CU(cudaMemcpyPeerAsync(sc + R.capacity, D->p.device, S->reg.d_key_xy, S->p.device, (size_t)n * 64, ks));
-      k_adopt_peer_keys<<<(n + 255) / 256, 256, 0, ks>>>(sc, sc + R.capacity, n, R.d_state, R.d_key_xy, R.d_addr, R.d_learn_count,
-                                                        adopted);
-      D->launches++;
-      CU(cudaGetLastError());
+      CU(launch(D, k_adopt_peer_keys, (n + 255) / 256, 256, 0, ks, sc, sc + R.capacity, n, R.d_state, R.d_key_xy, R.d_addr,
+                R.d_learn_count, adopted));
     }
     CU(cudaMemcpyAsync(h + 2 * d + 1, adopted, 4, cudaMemcpyDeviceToHost, ks));
   }

@@ -512,8 +512,8 @@ int ibft_sign_batch_rfc6979(ibft_engine* e, const uint8_t* privkeys, const uint8
 
 /* measurement / test hooks ------------------------------------------------------------------------- */
 /* Kernel selection of the recover step (the verdicts are identical on every path; only latency / throughput differ):
- *   AUTO    by batch size: up to SMs x 48 signatures (6,336 on an H100) QSPLIT, up to SMs x 192 (25,344) SPLIT, beyond
- *           that THREAD (the throughput kernel);
+ *   AUTO    by batch size, payload length and the key registry, as go-ibft_b200/csrc/recover_plan.hpp states it (which also
+ *           says when a host-buffer call is cut into latency pieces);
  *   THREAD  always one thread per signature;  QUAD  always four lanes per signature;
  *   SPLIT   chain warps (one lane per signature) + a helper warp per CTA that takes the digest, r^-1, sqrt and u1*G off the
  *           chain (mid-size batches: up to SMs x 96 signatures in one wave, e.g. a 10k-validator COMMIT round);
